@@ -128,6 +128,14 @@ struct Ctx {
   DevBuf<uint32_t> m_sq_idx, m_sq_idx2;
   DevBuf<uint64_t> h_grp, h_pos;
   DevBuf<uint64_t> m_read_hit_off;  // per query read (+1)
+  // stage-1 self-join (map.cu): per micromizer slot of reads [j_first, i_last), its
+  // query posting << 32 | hit count; valid for index build j_gen filtered at
+  // j_occurrence
+  uint64_t i_gen = 0, j_gen = 0;
+  uint32_t j_occurrence = 0, j_first = 0;
+  std::vector<uint64_t> h_j_off;
+  DevBuf<uint64_t> j_off, j_packed;
+  DevBuf<uint32_t> j_cursor;
   DevBuf<uint64_t> m_scratch64;     // oversize chain scratch
   DevBuf<uint32_t> m_scratch32, m_fallback;
   // split chain path: pair descriptors, pair-contiguous hits, overlap keys

@@ -445,6 +445,7 @@ void BuildIndexFrom(Ctx& c, ValView src_val, const uint64_t* src_org, uint64_t n
   c.i_sorted_ids = false;
   c.i_from_sketch = false;
   c.occurrence = 0xFFFFFFFFu;
+  ++c.i_gen;  // (results derived from an earlier index are stale)
   if (n >= 0xFFFFFFFFULL) {
     throw LimitError("index batch holds 2^32 or more minimizers");
   }

@@ -290,63 +290,153 @@ ExpandWarpKernel(IndexView ix, const uint64_t* __restrict__ q_org, uint64_t q_be
 // value: a posting (value v, read r, position p) is a query iff it passes r's
 // selection rule (thr_val, thr_pos; sketch.cu), and its hits are the postings of the
 // same run with a larger read id - the ones that follow it, the run being in read
-// order. No query sort, no table probe, no binary search: two sweeps over the sorted
-// postings (count, then emit through per-read cursors; the order of the hits inside
-// a read is free, see the header). Runs longer than `occurrence` give no hits.
+// order. No query sort and no table probe: one sweep over the sorted postings fills
+// the slots of the index batch's reads from its first join flush on, and each flush expands
+// its own reads' slots (the order of the hits inside a read is free, see the
+// header). Runs longer than `occurrence` give no hits.
 struct JoinView {
   ValView val;
   const uint64_t* org;
   uint64_t n;
   uint32_t occurrence;
-  const uint64_t* thr_val;  // of reads [thr_first, ...)
+  const uint64_t* thr_val;  // of reads [first, last)
   const uint32_t* thr_pos;
-  uint32_t thr_first;
-  uint32_t first, last;     // query reads of this flush
+  uint32_t first, last;     // query reads: the index batch's reads from the first join flush on
 };
-
-// number of hits of posting i (read r, value v) and the offset of the first one
-__device__ __forceinline__ uint32_t JoinKept(const JoinView& jv, uint64_t i, uint64_t v,
-                                             uint32_t r, uint32_t* skip) {
-  uint32_t fw = 0, same = 0;
-  for (uint64_t j = i + 1; j < jv.n && jv.val[j] == v; ++j) {
-    ++fw;
-    if (fw > jv.occurrence) return 0;
-    if (static_cast<uint32_t>(jv.org[j] >> 32) == r) ++same;
-  }
-  if (fw == same) return 0;
-  if (jv.occurrence != 0xFFFFFFFFu) {
-    uint32_t len = fw + 1;
-    if (len > jv.occurrence) return 0;
-    for (uint64_t j = i; j > 0 && jv.val[j - 1] == v; --j) {
-      if (++len > jv.occurrence) return 0;
-    }
-  }
-  *skip = same;
-  return fw - same;
-}
 
 __device__ __forceinline__ bool JoinIsQuery(const JoinView& jv, uint64_t v, uint64_t o) {
   const uint32_t r = static_cast<uint32_t>(o >> 32);
   if (r < jv.first || r >= jv.last) return false;
-  const uint64_t t = jv.thr_val[r - jv.thr_first];
-  return v < t || (v == t && (static_cast<uint32_t>(o) >> 1) < jv.thr_pos[r - jv.thr_first]);
+  const uint64_t t = jv.thr_val[r - jv.first];
+  return v < t || (v == t && (static_cast<uint32_t>(o) >> 1) < jv.thr_pos[r - jv.first]);
 }
 
-// sweep over the sorted postings: every query posting with hits takes the next free
-// slot of its read (slots [q_off[r], q_off[r + 1]) - one per micromizer - in any
-// order) and leaves (posting index, number of hits) there
+// First position in [lo, hi] at which the predicate `past` holds, `past` being false
+// then true over [lo, hi) and taken as true at hi. The whole warp searches: each step
+// probes 32 evenly spaced positions and keeps the stretch between the last false and
+// the first true probe, so a range of L positions takes ceil(log32 L) steps.
+template <typename Pred>
+__device__ __forceinline__ uint64_t WarpFirst(uint64_t lo, uint64_t hi, uint32_t lane,
+                                              Pred past) {
+  while (lo < hi) {
+    const uint64_t step = (hi - lo + 31) / 32;
+    const uint64_t p = lo + (lane + 1) * step - 1;
+    const uint32_t b = __ballot_sync(0xFFFFFFFFu, p >= hi || past(p));
+    if (!b) return hi;  // (lane 31 probed hi - 1)
+    const uint64_t f = __ffs(b) - 1;
+    hi = min(hi, lo + (f + 1) * step - 1);
+    lo += f * step;
+  }
+  return lo;
+}
+
+// One warp per 32 consecutive postings. The hits of query posting i (value v, read r)
+// are the postings of v's run that follow the segment of (v, r), so what i needs is
+// its run's start and end and its segment's end: ballots of "value changes" and
+// "value or read changes" between neighbours find the ones inside the warp. A run
+// crossing the warp's edge costs one more coalesced step of 32 postings past the
+// edge, which settles most runs, and past that a WarpFirst search, no further than
+// `occurrence` + 1 postings when the threshold is set (a longer run gives no hits).
+// So a warp costs O(1 + log32 L) steps for a run of L postings, whatever L and the
+// threshold, and the sweep is linear in the postings up to that factor.
+// Every query posting with hits takes the next free slot of its read (slots
+// [q_off[r], q_off[r + 1]) - one per micromizer - in any order) and leaves (posting
+// index, number of hits) there: ONE scattered 8-byte store per query, as a partial-
+// sector write costs a read-modify-write in HBM.
 __global__ void __launch_bounds__(kThreads)
-JoinProbeKernel(JoinView jv, const uint64_t* __restrict__ q_off, uint64_t q_begin,
+JoinSweepKernel(JoinView jv, const uint64_t* __restrict__ q_off,
                 uint32_t* __restrict__ cursor, uint64_t* __restrict__ packed) {
-  const uint64_t i = static_cast<uint64_t>(blockIdx.x) * kThreads + threadIdx.x;
-  if (i >= jv.n) return;
-  const uint64_t v = jv.val[i], o = jv.org[i];
-  if (!JoinIsQuery(jv, v, o)) return;
+  constexpr uint32_t kAll = 0xFFFFFFFFu;
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t base = (static_cast<uint64_t>(blockIdx.x) * kThreads + threadIdx.x) & ~31ULL;
+  if (base >= jv.n) return;  // (whole warps)
+  const uint64_t i = base + lane;
+  const bool valid = i < jv.n;
+  const uint64_t v = valid ? jv.val[i] : 0;
+  const uint64_t o = valid ? jv.org[i] : 0;
   const uint32_t r = static_cast<uint32_t>(o >> 32);
-  uint32_t skip;
-  const uint32_t kept = JoinKept(jv, i, v, r, &skip);
+  const bool q = valid && JoinIsQuery(jv, v, o);
+  if (!__any_sync(kAll, q)) return;
+
+  uint64_t vn = __shfl_down_sync(kAll, v, 1);
+  uint32_t rn = __shfl_down_sync(kAll, r, 1);
+  uint64_t vp = __shfl_up_sync(kAll, v, 1);
+  const bool has_next = i + 1 < jv.n;
+  if (lane == 31 && has_next) {
+    vn = jv.val[i + 1];
+    rn = static_cast<uint32_t>(jv.org[i + 1] >> 32);
+  }
+  if (lane == 0 && i > 0) vp = jv.val[i - 1];
+  const bool run_tail = !has_next || vn != v;  // (lanes beyond n: tails)
+  const uint32_t tails = __ballot_sync(kAll, run_tail);
+  const uint32_t seg_tails = __ballot_sync(kAll, run_tail || rn != r);
+  const uint32_t heads = __ballot_sync(kAll, i == 0 || vp != v);
+  const uint32_t at_or_above = kAll << lane, at_or_below = kAll >> (31 - lane);
+  // ends are exclusive; 0 = beyond the warp (every end inside it is >= 1)
+  uint64_t run_end = (tails & at_or_above) ? base + __ffs(tails & at_or_above) : 0;
+  uint64_t seg_end = (seg_tails & at_or_above) ? base + __ffs(seg_tails & at_or_above) : 0;
+  bool over = false;
+  const bool limited = jv.occurrence != kAll;
+
+  // the warp's last run goes on past it
+  if (__any_sync(kAll, q && run_end == 0)) {
+    const uint64_t vl = __shfl_sync(kAll, v, 31);
+    const uint32_t rl = __shfl_sync(kAll, r, 31);
+    const uint64_t j = base + 32, k = j + lane;
+    const bool dv = k >= jv.n || jv.val[k] != vl;
+    const uint32_t bv = __ballot_sync(kAll, dv);
+    const uint32_t bs =
+        __ballot_sync(kAll, dv || static_cast<uint32_t>(jv.org[k] >> 32) != rl);
+    uint64_t e_run = bv ? j + __ffs(bv) - 1 : 0;
+    bool o_fw = false;
+    if (!bv) {  // the run holds [base + 31, j + 32), so j + 32 <= n
+      if (limited && 33 > jv.occurrence) {
+        o_fw = true;
+      } else {
+        const uint64_t hi = limited ? min(jv.n, base + 32 + jv.occurrence) : jv.n;
+        e_run = WarpFirst(j + 32, hi, lane, [&](uint64_t p) { return jv.val[p] != vl; });
+        // still v at hi: the run holds [base + 31, hi], occurrence + 2 postings
+        o_fw = e_run == hi && hi < jv.n && jv.val[hi] == vl;
+      }
+    }
+    uint64_t e_seg = bs ? j + __ffs(bs) - 1 : 0;
+    if (!bs && !o_fw) {  // postings [j + 32, e_run) are all of v's run, in read order
+      e_seg = WarpFirst(j + 32, e_run, lane, [&](uint64_t p) {
+        return static_cast<uint32_t>(jv.org[p] >> 32) != rl;
+      });
+    }
+    if (run_end == 0) {
+      run_end = e_run;
+      over = o_fw;
+    }
+    if (seg_end == 0) seg_end = e_seg;
+  }
+  // the warp's first run began before it (only its length matters)
+  uint32_t run_start =
+      (heads & at_or_below) ? static_cast<uint32_t>(base) + 31 - __clz(heads & at_or_below) : 0;
+  if (limited && __any_sync(kAll, q && !over && !(heads & at_or_below))) {
+    const uint64_t vf = __shfl_sync(kAll, v, 0);
+    const uint64_t e0 = __shfl_sync(kAll, run_end, 0);  // (that run's end)
+    const int64_t j = static_cast<int64_t>(base) - 32, k = j + lane;
+    const uint32_t bv = __ballot_sync(kAll, k < 0 || jv.val[k] != vf);
+    uint64_t s_run;
+    if (bv) {
+      s_run = static_cast<uint64_t>(j + 32 - __clz(bv));
+    } else {
+      // the run holds [j, e0); a start before e0 - occurrence - 1 changes nothing
+      const uint64_t lo = e0 > jv.occurrence + 1ULL ? e0 - jv.occurrence - 1 : 0;
+      s_run = lo >= static_cast<uint64_t>(j)
+                  ? static_cast<uint64_t>(j)
+                  : WarpFirst(lo, static_cast<uint64_t>(j), lane,
+                              [&](uint64_t p) { return jv.val[p] == vf; });
+    }
+    if (!(heads & at_or_below)) run_start = static_cast<uint32_t>(s_run);
+  }
+  if (!q || over || (limited && run_end - run_start > jv.occurrence)) return;
+  const uint32_t kept = static_cast<uint32_t>(run_end - seg_end);
   if (!kept) return;
-  const uint64_t slot = q_off[r - jv.thr_first] - q_begin + atomicAdd(cursor + (r - jv.first), 1u);
+  const uint32_t rr = r - jv.first;
+  const uint64_t slot = q_off[rr] + atomicAdd(cursor + rr, 1u);
   packed[slot] = (i << 32) | kept;
 }
 
@@ -356,7 +446,7 @@ __global__ void UnpackJoin(const uint64_t* __restrict__ packed, uint64_t n,
   if (i < n) cnt[i] = static_cast<uint32_t>(packed[i]);
 }
 
-// ExpandWarpKernel over the slots of JoinProbeKernel: the query's own posting gives
+// ExpandWarpKernel over the slots of JoinSweepKernel: the query's own posting gives
 // its origin, its hits follow it in the run (after the postings of the same read)
 __global__ void __launch_bounds__(kThreads)
 ExpandJoinKernel(const uint64_t* __restrict__ i_org, const uint64_t* __restrict__ packed,
@@ -1359,6 +1449,39 @@ __global__ void ReorderOverlaps(const rvn_overlap* __restrict__ raw,
   for (uint32_t i = threadIdx.x & 31; i < cnt * 2; i += 32) d[i] = s[i];
 }
 
+// The self-join's slots for reads [first, i_last): one sweep per index (and occurrence
+// threshold) serves all later flushes of the batch, which stage 1 runs in read order.
+// Reads before `first` are left out: their flushes took the probe path, and their
+// thresholds would cost a sketch of reads that are no longer sketched. The slot
+// offsets are kept with the slots, as a flush over reads outside the batch replaces
+// the micromizer counts (c.h_q_off). Needs the thresholds of reads [first, i_last).
+void JoinSweep(Ctx& c, uint32_t first) {
+  const uint32_t nr = c.i_last - first;
+  const uint64_t t0 = first - c.qt_first, base = c.h_q_off[t0];
+  c.h_j_off.resize(nr + 1ULL);
+  for (uint32_t i = 0; i <= nr; ++i) c.h_j_off[i] = c.h_q_off[t0 + i] - base;
+  const uint64_t n_q = c.h_j_off[nr];
+  uint64_t* off = c.j_off.reserve(nr + 1ULL);
+  RVN_CUDA(cudaMemcpyAsync(off, c.h_j_off.data(), (nr + 1ULL) * sizeof(uint64_t),
+                           cudaMemcpyHostToDevice, c.stream));
+  uint32_t* cursor = c.j_cursor.reserve(nr + 1ULL);
+  uint64_t* packed = c.j_packed.reserve(n_q + 1);
+  RVN_CUDA(cudaMemsetAsync(cursor, 0, (nr + 1ULL) * sizeof(uint32_t), c.stream));
+  RVN_CUDA(cudaMemsetAsync(packed, 0, (n_q + 1) * sizeof(uint64_t), c.stream));
+  if (c.i_n > 0 && n_q > 0) {
+    JoinView jv{ValView{c.i_val.get(), c.i_is32 ? 1 : 0}, c.i_org.get(), c.i_n, c.occurrence,
+                c.qt_val.get() + t0, c.qt_pos.get() + t0, first, c.i_last};
+    JoinSweepKernel<<<CeilDiv(c.i_n, kThreads), kThreads, 0, c.stream>>>(jv, off, cursor,
+                                                                          packed);
+    RVN_LAUNCH_CHECK();
+    ++c.launches;
+  }
+  RVN_CUDA(cudaStreamSynchronize(c.stream));  // (h_j_off staging)
+  c.j_gen = c.i_gen;
+  c.j_occurrence = c.occurrence;
+  c.j_first = first;
+}
+
 }  // namespace
 
 // Chains hits that are already grouped by query read: hits of read i of the
@@ -1625,34 +1748,27 @@ void MapRange(Ctx& c, uint32_t first, uint32_t last, bool avoid_equal,
   const bool join = c.self_join && minhash && avoid_equal && avoid_symmetric && !want_filtered &&
                     c.i_from_sketch && c.i_sorted_ids && c.ids_identity && first >= c.i_first &&
                     last <= c.i_last;
-  if (join && !(c.qt_valid && c.qt_first <= first && last <= c.qt_last)) {
-    EnsureThresholds(c, first, last);  // (e.g. after a flush of reads outside the batch)
-  }
   uint64_t n_q = 0, n_hits = 0;
   uint64_t *hg = nullptr, *hp = nullptr;
   uint64_t* read_hit_off = c.m_read_hit_off.reserve(nr + 2ULL);
   std::vector<uint64_t> h_rho(nr + 1ULL);
   if (join) {
-    JoinView jv{ValView{c.i_val.get(), c.i_is32 ? 1 : 0}, c.i_org.get(), c.i_n, c.occurrence,
-                c.qt_val.get(), c.qt_pos.get(), c.qt_first, first, last};
+    const bool sweep = c.j_gen != c.i_gen || c.j_occurrence != c.occurrence || first < c.j_first;
+    if (sweep && !(c.qt_valid && c.qt_first <= first && c.i_last <= c.qt_last)) {
+      EnsureThresholds(c, first, c.i_last);  // (its sketch and micromize time are not probe's)
+    }
     TimerBegin(c, "probe");
-    const uint64_t b0 = first - c.qt_first;
-    const uint64_t q_begin = c.h_q_off[b0];
-    n_q = c.h_q_off[b0 + nr] - q_begin;
-    uint32_t* cnt = c.m_cnt.reserve(n_q + 1);
-    uint32_t* cursor = c.m_first.reserve(nr + 1ULL);
-    uint64_t* packed = c.m_sq_key.reserve(n_q + 2);
+    if (sweep) JoinSweep(c, first);
+    const uint64_t b0 = first - c.j_first;
+    const uint64_t q_begin = c.h_j_off[b0];
+    n_q = c.h_j_off[b0 + nr] - q_begin;
+    const uint64_t* packed = c.j_packed.get() + q_begin;
     uint64_t* hit_off = c.m_hit_off.reserve(n_q + 2);
-    RVN_CUDA(cudaMemsetAsync(cursor, 0, (nr + 1ULL) * sizeof(uint32_t), c.stream));
-    RVN_CUDA(cudaMemsetAsync(packed, 0, (n_q + 1) * sizeof(uint64_t), c.stream));
-    if (c.i_n > 0 && n_q > 0) {
-      JoinProbeKernel<<<CeilDiv(c.i_n, kThreads), kThreads, 0, c.stream>>>(
-          jv, c.q_off.get(), q_begin, cursor, packed);
+    if (n_q > 0) {
+      uint32_t* cnt = c.m_cnt.reserve(n_q + 1);
       UnpackJoin<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(packed, n_q, cnt);
       RVN_LAUNCH_CHECK();
-      c.launches += 2;
-    }
-    if (n_q > 0) {
+      ++c.launches;
       ExclusiveScanU32(c, cnt, hit_off, n_q);
       n_hits = ReadU64(c, hit_off + n_q);
     } else {
@@ -1669,7 +1785,7 @@ void MapRange(Ctx& c, uint32_t first, uint32_t last, bool avoid_equal,
       ++c.launches;
     }
     GatherU64<<<CeilDiv(nr + 1ULL, kThreads), kThreads, 0, c.stream>>>(
-        hit_off, c.q_off.get() + b0, q_begin, nr + 1ULL, read_hit_off);
+        hit_off, c.j_off.get() + b0, q_begin, nr + 1ULL, read_hit_off);
     RVN_LAUNCH_CHECK();
     ++c.launches;
     RVN_CUDA(cudaMemcpyAsync(h_rho.data(), read_hit_off, (nr + 1ULL) * sizeof(uint64_t),
