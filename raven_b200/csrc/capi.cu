@@ -751,6 +751,12 @@ RVN_API int rvn_set_option(rvn_ctx* ctx, const char* name, int64_t value) {
       c.async_upload = value != 0;
     } else if (name && std::strcmp(name, "self_join") == 0) {
       c.self_join = value != 0;
+    } else if (name && std::strcmp(name, "bare_count") == 0) {
+      if (value != 0 && value != 1 && value != 8 && value != 16) {
+        throw InvalidArgument("bare_count: 0, 1, 8 or 16");
+      }
+      c.bare_count = value;
+      c.bare_cluster = 0;  // (chosen again at the next build)
     } else if (name && std::strcmp(name, "tier_min_records") == 0) {
       c.tier_min_records = value < 0 ? 0 : static_cast<uint64_t>(value);
     } else if (name && std::strcmp(name, "reset_stats") == 0) {

@@ -96,6 +96,9 @@ struct Ctx {
   uint64_t group_count_min = 0;  // fewer keys per group of equal upper bits: full sort instead
   bool i_from_sketch = false;  // the index holds the FULL sketches of reads [i_first, i_last)
   int64_t self_join = 1;       // option: stage-1 hits by a self-join over the index
+  // option: multiplicities of the bare keys by one partition pass + cluster counters
+  // (1: clusters of 8 CTAs, 8 or 16: that cluster size) instead of a sort (0)
+  int64_t bare_count = 1;
 
   // ---- index ----
   bool i_valid = false;
@@ -110,6 +113,10 @@ struct Ctx {
   DevBuf<uint64_t> t_off, t_aval, t_aorg, t_b0, t_b1, t_b2, t_narrow;
   const uint32_t* t_sorted_b = nullptr;
   uint64_t t_nb = 0;
+  bool t_b_sorted = true;       // t_sorted_b is in full key order (else: partitioned or unsorted)
+  DevBuf<uint32_t> t_bstart;    // first bare key of every bucket of the partition
+  int bare_cluster = 0;         // cluster size of BareCountKernel on this device (0: not chosen)
+  int bare_clusters = 0;        // clusters of that size resident at once
   uint64_t tier_min_records = 1ULL << 18;  // smaller index batches are not worth a partition
   DevBuf<uint32_t> i_bucket;
   int i_bucket_bits = 0;
@@ -258,8 +265,10 @@ void BuildIndex(Ctx& c, uint32_t first, uint32_t last, bool minhash,
 uint64_t MaxMicromizerValue(Ctx& c, uint32_t first, uint32_t last);
 // index from device records already in (read, position) order (values as u32
 // or u64, see ValView)
+// count_bare: the bare keys of a tiered build are counted by partition + BareCountKernel
+// (c.bare_count permitting) instead of being sorted
 void BuildIndexFrom(Ctx& c, ValView src_val, const uint64_t* src_org, uint64_t n,
-                    uint64_t index_bases, uint64_t value_limit = ~0ULL);
+                    uint64_t index_bases, uint64_t value_limit = ~0ULL, bool count_bare = false);
 
 // ---- radix.cu ---- stable LSD radix sort on key bits [begin_bit, end_bit).
 // The source arrays are only read (src may alias buffer b: it is dead once the
@@ -279,6 +288,10 @@ int RadixSortPairs(Ctx& c, const uint64_t* src_keys, uint64_t* keys_a, uint64_t*
                    int begin_bit, int end_bit, bool descending = false);
 int RadixSortKeys(Ctx& c, const uint32_t* src_keys, uint32_t* keys_a, uint32_t* keys_b,
                   uint64_t n, int begin_bit, int end_bit);
+// unstable partition of u32 keys on bits [begin_bit, end_bit) (at most 10): digit d's
+// keys land in dst[bin_start[d], bin_start[d + 1]) (n past the last digit), in any order
+void RadixPartitionKeys(Ctx& c, const uint32_t* src, uint32_t* dst, uint64_t n, int begin_bit,
+                        int end_bit, uint32_t* bin_start);
 // run-length histogram of the index keys (c.i_hist: 65536 u64 bins + #keys), filled by the build
 uint64_t* IndexHistogram(Ctx& c);
 uint32_t ThresholdFromHistogram(Ctx& c, const uint64_t* h_hist, uint64_t n_keys,

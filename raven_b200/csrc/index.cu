@@ -14,6 +14,8 @@
 #include <algorithm>
 #include <cmath>
 
+#include <cooperative_groups.h>
+
 #include "engine.cuh"
 
 namespace rvn {
@@ -399,6 +401,172 @@ GroupCountKernel(const uint32_t* __restrict__ key, uint64_t n, unsigned long lon
   }
 }
 
+// Multiplicities of bare keys that are only partitioned on their top kBareBucketBits
+// bits (bucket = 2^span_bits consecutive values; one bucket of all values when the
+// keys have 20 bits or fewer and were not partitioned at all). A cluster of C CTAs
+// owns one bucket at a time and counts it in u32 counters spread over the CTAs'
+// shared memory (distributed shared memory): value u of a sweep belongs to CTA
+// u >> slot_bits, counter u & (2^slot_bits - 1). Every CTA streams its 1/C of the
+// bucket's keys with coalesced loads and adds 1 to the owner's counter; after the
+// cluster barrier every CTA reads its own counters off as runs (nonzero counter =
+// one key, its value = the run length) - the histogram GroupCountKernel and
+// IndexTableKernel<., false> take from sorted keys - and clears them. A bucket wider
+// than the cluster's counters takes several sweeps over its keys (the repeats read
+// the bucket from L2).
+constexpr int kBareBucketBits = 10;
+constexpr int kBareThreads = 1024;
+constexpr int kBareSlotBits = 15;  // 32768 counters = 128 KB per CTA
+
+__global__ void __launch_bounds__(kBareThreads, 1)
+BareCountKernel(const uint32_t* __restrict__ key, uint64_t n, const uint32_t* __restrict__ bstart,
+                uint32_t first_bucket, uint32_t n_buckets, int span_bits, int slot_bits,
+                unsigned long long* __restrict__ hist) {
+  extern __shared__ __align__(16) uint32_t bare_smem[];
+  __shared__ uint32_t keys_total;
+  namespace cg = cooperative_groups;
+  cg::cluster_group cluster = cg::this_cluster();
+  const uint32_t csize = cluster.num_blocks();
+  const uint32_t crank = cluster.block_rank();
+  const uint32_t n_slots = 1u << slot_bits;
+  uint32_t* ctr = bare_smem;
+  uint32_t* sh = bare_smem + n_slots;  // kSmemBins
+  for (uint32_t i = threadIdx.x; i < n_slots; i += kBareThreads) ctr[i] = 0;
+  for (uint32_t i = threadIdx.x; i < kSmemBins; i += kBareThreads) sh[i] = 0;
+  if (threadIdx.x == 0) keys_total = 0;
+  const uint32_t ctr_addr = static_cast<uint32_t>(__cvta_generic_to_shared(ctr));
+  const uint32_t span_mask = (1u << span_bits) - 1u;
+  const uint32_t sweep_span = n_slots * csize;  // (csize: a power of two)
+  const uint32_t slot_mask = n_slots - 1u;
+  uint32_t h1 = 0, h2 = 0, h3 = 0, h4 = 0, nkeys = 0;
+  cluster.sync();  // every CTA's counters are zero before the first remote add
+  const uint32_t n_clusters = gridDim.x / csize;
+  for (uint32_t b = first_bucket + blockIdx.x / csize; b < n_buckets; b += n_clusters) {
+    const uint64_t lo = bstart ? bstart[b] : 0;
+    const uint64_t hi = bstart && b + 1 < n_buckets ? bstart[b + 1] : n;
+    if (lo >= hi) continue;  // (the same for every CTA of the cluster)
+    for (uint64_t s0 = 0; s0 <= span_mask; s0 += sweep_span) {
+      constexpr int kUnroll = 4;
+      const uint64_t stride = static_cast<uint64_t>(csize) * kBareThreads;
+      for (uint64_t i0 = lo + crank * kBareThreads + threadIdx.x; i0 < hi; i0 += kUnroll * stride) {
+        uint32_t k4[kUnroll];
+#pragma unroll
+        for (int u = 0; u < kUnroll; ++u) {
+          const uint64_t i = i0 + u * stride;
+          k4[u] = i < hi ? key[i] : 0u;
+        }
+#pragma unroll
+        for (int u = 0; u < kUnroll; ++u) {
+          const uint64_t v = static_cast<uint64_t>(k4[u] & span_mask) - s0;
+          if (i0 + u * stride < hi && v < sweep_span) {
+            const uint32_t owner = static_cast<uint32_t>(v) >> slot_bits;
+            const uint32_t local = ctr_addr + 4u * (static_cast<uint32_t>(v) & slot_mask);
+            uint32_t remote;
+            asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local), "r"(owner));
+            asm volatile("red.relaxed.cluster.shared::cluster.add.u32 [%0], 1;" ::"r"(remote) : "memory");
+          }
+        }
+      }
+      cluster.sync();  // every add of the sweep has landed
+      for (uint32_t t = threadIdx.x; t < n_slots; t += kBareThreads) {
+        const uint32_t c = ctr[t];
+        if (c == 0) continue;
+        ctr[t] = 0;
+        ++nkeys;
+        if (c <= 4) {
+          h1 += c == 1;
+          h2 += c == 2;
+          h3 += c == 3;
+          h4 += c == 4;
+        } else if (c < kSmemBins) {
+          atomicAdd(&sh[c], 1u);
+        } else {
+          atomicAdd(&hist[min(c, kHistBins - 1)], 1ULL);
+        }
+      }
+      cluster.sync();  // every counter is clear before the next sweep's adds
+    }
+  }
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) {
+    h1 += __shfl_xor_sync(0xFFFFFFFFu, h1, d);
+    h2 += __shfl_xor_sync(0xFFFFFFFFu, h2, d);
+    h3 += __shfl_xor_sync(0xFFFFFFFFu, h3, d);
+    h4 += __shfl_xor_sync(0xFFFFFFFFu, h4, d);
+    nkeys += __shfl_xor_sync(0xFFFFFFFFu, nkeys, d);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    atomicAdd(&sh[1], h1);
+    atomicAdd(&sh[2], h2);
+    atomicAdd(&sh[3], h3);
+    atomicAdd(&sh[4], h4);
+    atomicAdd(&keys_total, nkeys);
+  }
+  __syncthreads();
+  for (uint32_t i = threadIdx.x; i < kSmemBins; i += kBareThreads) {
+    if (sh[i]) atomicAdd(&hist[i], static_cast<unsigned long long>(sh[i]));
+  }
+  if (threadIdx.x == 0 && keys_total) {
+    atomicAdd(&hist[kHistBins], static_cast<unsigned long long>(keys_total));
+  }
+}
+
+// run-length histogram + #keys of the n bare keys (all > limit) in `keys`, added to
+// hist; bstart: first key of every bucket of the partition (nullptr: not partitioned,
+// keys of at most 2 * kBareBucketBits bits)
+void BareCount(Ctx& c, const uint32_t* keys, uint64_t n, int key_bits, uint32_t limit,
+               const uint32_t* bstart, unsigned long long* hist) {
+  const int span_bits = bstart ? key_bits - kBareBucketBits : key_bits;
+  const uint32_t n_buckets = bstart ? (1u << kBareBucketBits) : 1u;
+  const uint32_t first_bucket = bstart ? (limit >> span_bits) : 0u;
+  if (c.bare_cluster == 0) {
+    // cluster size: the option's, else 8 (portable; on an H100 it measured faster than
+    // 16 with its half as many sweeps: the remote adds bound the kernel, not the reads)
+    const int size = c.bare_count > 1 ? static_cast<int>(c.bare_count) : 8;
+    const size_t smem = ((1u << kBareSlotBits) + kSmemBins) * sizeof(uint32_t);
+    RVN_CUDA(cudaFuncSetAttribute(BareCountKernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  static_cast<int>(smem)));
+    RVN_CUDA(cudaFuncSetAttribute(BareCountKernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(static_cast<unsigned>(size));
+    cfg.blockDim = dim3(kBareThreads);
+    cfg.dynamicSmemBytes = smem;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = static_cast<unsigned>(size);
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    int clusters = 0;
+    RVN_CUDA(cudaOccupancyMaxActiveClusters(&clusters, BareCountKernel, &cfg));
+    if (clusters < 1) throw CudaError("BareCountKernel: a cluster does not fit the device");
+    c.bare_cluster = size;
+    c.bare_clusters = clusters;
+  }
+  const int csize = c.bare_cluster;
+  int log_c = 0;
+  while ((1 << log_c) < csize) ++log_c;
+  const int slot_bits = std::max(0, std::min(kBareSlotBits, span_bits - log_c));
+  const unsigned clusters =
+      static_cast<unsigned>(std::min<uint64_t>(n_buckets - first_bucket, c.bare_clusters));
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(clusters * csize);
+  cfg.blockDim = dim3(kBareThreads);
+  cfg.dynamicSmemBytes = ((1u << slot_bits) + kSmemBins) * sizeof(uint32_t);
+  cfg.stream = c.stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = static_cast<unsigned>(csize);
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  RVN_CUDA(cudaLaunchKernelEx(&cfg, BareCountKernel, keys, n, bstart, first_bucket, n_buckets,
+                              span_bits, slot_bits, hist));
+  RVN_LAUNCH_CHECK();
+  ++c.launches;
+}
+
 }  // namespace
 
 // largest micromizer value of reads [first, last): the largest of their selection
@@ -434,13 +602,14 @@ void BuildIndex(Ctx& c, uint32_t first, uint32_t last, bool minhash, uint64_t va
   for (uint32_t r = first; r < last; ++r) bases += c.h_len[r];
   c.i_first = first;
   c.i_last = last;
-  BuildIndexFrom(c, src_val, src_org, n, bases, minhash ? ~0ULL : value_limit);
+  BuildIndexFrom(c, src_val, src_org, n, bases, minhash ? ~0ULL : value_limit,
+                 /*count_bare=*/true);
   c.i_sorted_ids = c.ids_ascending;
   c.i_from_sketch = !minhash;
 }
 
 void BuildIndexFrom(Ctx& c, ValView src_val, const uint64_t* src_org, uint64_t n,
-                    uint64_t index_bases, uint64_t value_limit) {
+                    uint64_t index_bases, uint64_t value_limit, bool count_bare) {
   c.i_valid = false;
   c.i_sorted_ids = false;
   c.i_from_sketch = false;
@@ -472,6 +641,8 @@ void BuildIndexFrom(Ctx& c, ValView src_val, const uint64_t* src_org, uint64_t n
   c.i_limit = tiered ? value_limit : ~0ULL;
   uint64_t n_a = n, n_b = 0;
   const uint32_t* sorted_b = nullptr;
+  const bool bare = tiered && count_bare && c.bare_count != 0;
+  const uint32_t* bstart = nullptr;  // (bare: buckets of the partitioned keys)
 
   TimerBegin(c, "index_sort");
   // stable LSD radix sort on the value bits (radix.cu). The sketch arrays are
@@ -513,19 +684,35 @@ void BuildIndexFrom(Ctx& c, ValView src_val, const uint64_t* src_org, uint64_t n
     }
     // the rest: bare keys, only their multiplicities matter
     uint32_t* b1 = reinterpret_cast<uint32_t*>(c.t_b1.reserve(n_b / 2 + 2));
-    uint32_t* b2 = reinterpret_cast<uint32_t*>(c.t_b2.reserve(n_b / 2 + 2));
-    // (sorted above their low bits only: GroupCountKernel reads the multiplicities
-    //  off groups of equal upper bits)
-    // - while a group holds a few hundred keys: the rank of a partitioned run owns
-    // 1/N of the keys of every group, and zeroing and reading 1024 counters per
-    // group then costs more than the third pass
-    const uint64_t n_groups = ((value_mask - value_limit) >> kGroupLowBits) + 1;
-    c.t_b_low = (key_bits > 2 * kGroupLowBits && n_b / n_groups >= c.group_count_min)
-                    ? kGroupLowBits
-                    : 0;
-    if (n_b > 0) {
-      const int where = RadixSortKeys(c, b_src, b1, b2, n_b, c.t_b_low, key_bits);
-      sorted_b = where < 0 ? b_src : (where == 0 ? b1 : b2);
+    if (bare) {
+      // one unstable partition on the top kBareBucketBits key bits (none when every
+      // key fits one bucket), BareCountKernel counts inside the buckets
+      c.t_b2.release();
+      c.t_b_low = 0;
+      c.t_b_sorted = false;
+      sorted_b = n_b > 0 ? b_src : nullptr;
+      if (n_b > 0 && key_bits > 2 * kBareBucketBits) {
+        uint32_t* starts = c.t_bstart.reserve(1u << kBareBucketBits);
+        RadixPartitionKeys(c, b_src, b1, n_b, key_bits - kBareBucketBits, key_bits, starts);
+        sorted_b = b1;
+        bstart = starts;
+      }
+    } else {
+      uint32_t* b2 = reinterpret_cast<uint32_t*>(c.t_b2.reserve(n_b / 2 + 2));
+      // (sorted above their low bits only: GroupCountKernel reads the multiplicities
+      //  off groups of equal upper bits)
+      // - while a group holds a few hundred keys: the rank of a partitioned run owns
+      // 1/N of the keys of every group, and zeroing and reading 1024 counters per
+      // group then costs more than the third pass
+      const uint64_t n_groups = ((value_mask - value_limit) >> kGroupLowBits) + 1;
+      c.t_b_low = (key_bits > 2 * kGroupLowBits && n_b / n_groups >= c.group_count_min)
+                      ? kGroupLowBits
+                      : 0;
+      c.t_b_sorted = c.t_b_low == 0;
+      if (n_b > 0) {
+        const int where = RadixSortKeys(c, b_src, b1, b2, n_b, c.t_b_low, key_bits);
+        sorted_b = where < 0 ? b_src : (where == 0 ? b1 : b2);
+      }
     }
     c.t_sorted_b = sorted_b;
     c.t_nb = n_b;
@@ -554,6 +741,7 @@ void BuildIndexFrom(Ctx& c, ValView src_val, const uint64_t* src_org, uint64_t n
     }
     c.t_sorted_b = nullptr;
     c.t_nb = 0;
+    c.t_b_sorted = true;
   }
   c.i_n = n_a;
   TimerEnd(c);
@@ -586,7 +774,11 @@ void BuildIndexFrom(Ctx& c, ValView src_val, const uint64_t* src_org, uint64_t n
         reinterpret_cast<const uint32_t*>(kv), n_a, shift, n_buckets, bucket,
         reinterpret_cast<unsigned long long*>(hist), gaps);
     if (tiered && n_b > 0) {  // multiplicities of the keys beyond the limit
-      if (c.t_b_low) {
+      if (bare) {
+        BareCount(c, sorted_b, n_b, key_bits, limit32, bstart,
+                  reinterpret_cast<unsigned long long*>(hist));
+        --c.launches;  // (counted by BareCount)
+      } else if (c.t_b_low) {
         GroupCountKernel<<<std::min<unsigned>(CeilDiv(n_b, kGroupChunk * (kThreads / 32)), c.sms * 6),
                            kThreads, 0, c.stream>>>(sorted_b, n_b,
                                                     reinterpret_cast<unsigned long long*>(hist));
@@ -674,19 +866,22 @@ uint32_t FilterIndex(Ctx& c, double frequency) {
       CollectLongRuns<uint32_t><<<CeilDiv(c.i_n, kThreads), kThreads, 0, c.stream>>>(
           reinterpret_cast<const uint32_t*>(c.i_val.get()), c.i_n,
           reinterpret_cast<unsigned long long*>(counter), out);
-      if (c.t_sorted_b && c.t_nb && c.t_b_low) {  // (runs of >= 65535: order the low bits too)
+      if (c.t_sorted_b && c.t_nb && !c.t_b_sorted) {  // (runs of >= 65535: sort the bare keys)
+        // a full key sort is right from any order; the source buffer doubles as the
+        // sort's second buffer (it is dead after the first pass)
         uint32_t* bufs[3] = {reinterpret_cast<uint32_t*>(c.t_b0.get()),
                              reinterpret_cast<uint32_t*>(c.t_b1.get()),
                              reinterpret_cast<uint32_t*>(c.t_b2.get())};
-        uint32_t* free_buf[2];
-        int nf = 0;
+        uint32_t* src = nullptr;
         for (uint32_t* p : bufs) {
-          if (p != c.t_sorted_b && nf < 2) free_buf[nf++] = p;
+          if (p == c.t_sorted_b) src = p;
         }
-        const int where = RadixSortKeys(c, c.t_sorted_b, free_buf[0], free_buf[1], c.t_nb, 0,
+        uint32_t* other = src == bufs[0] ? bufs[1] : bufs[0];
+        const int where = RadixSortKeys(c, src, other, src, c.t_nb, 0,
                                         static_cast<int>(2 * c.prm.k));
-        c.t_sorted_b = where < 0 ? c.t_sorted_b : (where == 0 ? free_buf[0] : free_buf[1]);
+        c.t_sorted_b = where == 0 ? other : src;
         c.t_b_low = 0;
+        c.t_b_sorted = true;
       }
       if (c.t_sorted_b && c.t_nb) {  // tiered build: the keys beyond the limit too
         CollectLongRuns<uint32_t><<<CeilDiv(c.t_nb, kThreads), kThreads, 0, c.stream>>>(

@@ -100,6 +100,81 @@ RadixScanBinsKernel(const unsigned long long* __restrict__ hist, int n_passes,
   }
 }
 
+// Decoupled look-back over the status words of one (tile, bin) grid: publishes the
+// tile's counts of the thread's kBinsPerThread bins and returns in excl the counts
+// of those bins in all tiles before it.
+// A thread owns 4 neighbouring bins = ONE 16-byte status word per tile: all four
+// aggregates are published in one store before any waiting, and one 16-byte load
+// per step walks the four chains back together (a per-bin walk would put up to
+// #resident-tiles dependent L2 round trips in series, four times over).
+__device__ __forceinline__ void ChainTileCounts(uint32_t* __restrict__ status, uint32_t tile,
+                                                const uint32_t (&cnt)[kBinsPerThread],
+                                                uint32_t (&excl)[kBinsPerThread]) {
+  uint4* st4 = reinterpret_cast<uint4*>(status);
+  const uint64_t my4 = static_cast<uint64_t>(tile) * (kBins / 4) + threadIdx.x;
+#pragma unroll
+  for (int j = 0; j < kBinsPerThread; ++j) excl[j] = 0;
+  static_assert(kBinsPerThread == 4, "one uint4 of status words per thread");
+  if (tile > 0) {
+    uint4 agg;
+    agg.x = kFlagAggregate | cnt[0];
+    agg.y = kFlagAggregate | cnt[1];
+    agg.z = kFlagAggregate | cnt[2];
+    agg.w = kFlagAggregate | cnt[3];
+    asm volatile("st.volatile.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(st4 + my4),
+                 "r"(agg.x), "r"(agg.y), "r"(agg.z), "r"(agg.w)
+                 : "memory");
+    // kLook predecessors per round, their loads in flight together: one
+    // dependent L2 round trip per tile would make the walk slower than the rate
+    // at which tiles start, and the chain would grow to every tile in flight
+    constexpr int kLook = 4;
+    uint32_t open = 0xF;  // chains still walking
+    int64_t p = static_cast<int64_t>(tile) - 1;
+    while (open) {
+      uint4 v[kLook];
+#pragma unroll
+      for (int u = 0; u < kLook; ++u) {
+        const int64_t q = p - u;
+        if (q >= 0) {
+          const uint4* src = st4 + static_cast<uint64_t>(q) * (kBins / 4) + threadIdx.x;
+          asm volatile("ld.volatile.global.v4.u32 {%0, %1, %2, %3}, [%4];"
+                       : "=r"(v[u].x), "=r"(v[u].y), "=r"(v[u].z), "=r"(v[u].w)
+                       : "l"(src)
+                       : "memory");
+        } else {  // before tile 0: empty prefixes
+          v[u] = make_uint4(kFlagPrefix, kFlagPrefix, kFlagPrefix, kFlagPrefix);
+        }
+      }
+      int used = 0;
+#pragma unroll
+      for (int u = 0; u < kLook; ++u) {
+        const uint32_t vv[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
+        const bool ready = (vv[0] & kFlagMask) && (vv[1] & kFlagMask) && (vv[2] & kFlagMask) &&
+                           (vv[3] & kFlagMask);
+        if (used == u && ready && open) {  // (in order; stop at the first unwritten tile)
+#pragma unroll
+          for (int j = 0; j < kBinsPerThread; ++j) {
+            if (open & (1u << j)) {
+              excl[j] += vv[j] & kValueMask;
+              if ((vv[j] & kFlagMask) == kFlagPrefix) open &= ~(1u << j);
+            }
+          }
+          used = u + 1;
+        }
+      }
+      p -= used;  // (used == 0: the nearest tile has not published yet - poll again)
+    }
+  }
+  uint4 pre;
+  pre.x = kFlagPrefix | (excl[0] + cnt[0]);
+  pre.y = kFlagPrefix | (excl[1] + cnt[1]);
+  pre.z = kFlagPrefix | (excl[2] + cnt[2]);
+  pre.w = kFlagPrefix | (excl[3] + cnt[3]);
+  asm volatile("st.volatile.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(st4 + my4), "r"(pre.x),
+               "r"(pre.y), "r"(pre.z), "r"(pre.w)
+               : "memory");
+}
+
 template <typename KeyT, typename ValT, bool HAS_VAL>
 struct __align__(16) PassSmem {
   static constexpr int kTile = kThreads * Items<KeyT>::value;
@@ -219,73 +294,9 @@ OnesweepPass(const KeyT* __restrict__ keys_in, KeyT* __restrict__ keys_out,
   }
 
   // ---- chain the tile's bin counts to the tiles before it (decoupled look-back) ----
-  // A thread owns 4 neighbouring bins = ONE 16-byte status word per tile: all four
-  // aggregates are published in one store before any waiting, and one 16-byte load
-  // per step walks the four chains back together (a per-bin walk would put up to
-  // #resident-tiles dependent L2 round trips in series, four times over).
   {
-    uint4* st4 = reinterpret_cast<uint4*>(status);
-    const uint64_t my4 = static_cast<uint64_t>(tile) * (kBins / 4) + threadIdx.x;
-    uint32_t excl[kBinsPerThread] = {0, 0, 0, 0};
-    static_assert(kBinsPerThread == 4, "one uint4 of status words per thread");
-    if (tile > 0) {
-      uint4 agg;
-      agg.x = kFlagAggregate | cnt[0];
-      agg.y = kFlagAggregate | cnt[1];
-      agg.z = kFlagAggregate | cnt[2];
-      agg.w = kFlagAggregate | cnt[3];
-      asm volatile("st.volatile.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(st4 + my4),
-                   "r"(agg.x), "r"(agg.y), "r"(agg.z), "r"(agg.w)
-                   : "memory");
-      // kLook predecessors per round, their loads in flight together: one
-      // dependent L2 round trip per tile would make the walk slower than the rate
-      // at which tiles start, and the chain would grow to every tile in flight
-      constexpr int kLook = 4;
-      uint32_t open = 0xF;  // chains still walking
-      int64_t p = static_cast<int64_t>(tile) - 1;
-      while (open) {
-        uint4 v[kLook];
-#pragma unroll
-        for (int u = 0; u < kLook; ++u) {
-          const int64_t q = p - u;
-          if (q >= 0) {
-            const uint4* src = st4 + static_cast<uint64_t>(q) * (kBins / 4) + threadIdx.x;
-            asm volatile("ld.volatile.global.v4.u32 {%0, %1, %2, %3}, [%4];"
-                         : "=r"(v[u].x), "=r"(v[u].y), "=r"(v[u].z), "=r"(v[u].w)
-                         : "l"(src)
-                         : "memory");
-          } else {  // before tile 0: empty prefixes
-            v[u] = make_uint4(kFlagPrefix, kFlagPrefix, kFlagPrefix, kFlagPrefix);
-          }
-        }
-        int used = 0;
-#pragma unroll
-        for (int u = 0; u < kLook; ++u) {
-          const uint32_t vv[4] = {v[u].x, v[u].y, v[u].z, v[u].w};
-          const bool ready = (vv[0] & kFlagMask) && (vv[1] & kFlagMask) && (vv[2] & kFlagMask) &&
-                             (vv[3] & kFlagMask);
-          if (used == u && ready && open) {  // (in order; stop at the first unwritten tile)
-#pragma unroll
-            for (int j = 0; j < kBinsPerThread; ++j) {
-              if (open & (1u << j)) {
-                excl[j] += vv[j] & kValueMask;
-                if ((vv[j] & kFlagMask) == kFlagPrefix) open &= ~(1u << j);
-              }
-            }
-            used = u + 1;
-          }
-        }
-        p -= used;  // (used == 0: the nearest tile has not published yet - poll again)
-      }
-    }
-    uint4 pre;
-    pre.x = kFlagPrefix | (excl[0] + cnt[0]);
-    pre.y = kFlagPrefix | (excl[1] + cnt[1]);
-    pre.z = kFlagPrefix | (excl[2] + cnt[2]);
-    pre.w = kFlagPrefix | (excl[3] + cnt[3]);
-    asm volatile("st.volatile.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(st4 + my4), "r"(pre.x),
-                 "r"(pre.y), "r"(pre.z), "r"(pre.w)
-                 : "memory");
+    uint32_t excl[kBinsPerThread];
+    ChainTileCounts(status, tile, cnt, excl);
 #pragma unroll
     for (int j = 0; j < kBinsPerThread; ++j) {
       const uint32_t b = threadIdx.x * kBinsPerThread + j;
@@ -351,6 +362,104 @@ OnesweepPass(const KeyT* __restrict__ keys_in, KeyT* __restrict__ keys_out,
     if (s < tile_count) {
       const KeyT k = sm.stage.keys[s];
       keys_out[sm.bin_dst[Digit<KeyT>(k, flip, begin_bit, dmask)] + s] = k;
+    }
+  }
+}
+
+// One UNSTABLE key-only pass over a digit of up to kRadixMaxBits bits: same tiles,
+// look-back and staging as OnesweepPass<u32, u32, false>, but every key takes its
+// slot with one shared-memory atomicAdd on the tile's bin counter instead of the
+// warp's ten ballots. Keys of a bin land in any order inside their tile's share of
+// the bin; for callers that need only the multiset of every bin.
+struct PartitionSmem {
+  uint32_t bin_cnt[kBins];  // keys of the tile per bin
+  uint32_t bin_off[kBins];  // first staging slot of the bin inside the tile
+  uint32_t bin_dst[kBins];  // global index of staging slot s of bin d = bin_dst[d] + s
+  uint32_t scan[34];
+  uint32_t tile;
+  uint32_t keys[kThreads * Items<uint32_t>::value];
+};
+
+__global__ void __launch_bounds__(kThreads, 2)
+PartitionPass(const uint32_t* __restrict__ keys_in, uint32_t* __restrict__ keys_out, uint32_t n,
+              int begin_bit, int pass_bits, const uint32_t* __restrict__ bin_base,
+              uint32_t* __restrict__ bin_next, uint32_t* __restrict__ status,
+              unsigned int* __restrict__ ticket) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  PartitionSmem& sm = *reinterpret_cast<PartitionSmem*>(smem_raw);
+  constexpr int kItems = Items<uint32_t>::value;
+  constexpr int kTile = kThreads * kItems;
+  constexpr int kWarpTile = 32 * kItems;
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint32_t dmask = (1u << pass_bits) - 1u;
+
+  if (threadIdx.x == 0) sm.tile = atomicAdd(ticket, 1u);
+#pragma unroll
+  for (int j = 0; j < kBinsPerThread; ++j) sm.bin_cnt[j * kThreads + threadIdx.x] = 0;
+  __syncthreads();
+  const uint32_t tile = sm.tile;
+  const uint64_t tile_base = static_cast<uint64_t>(tile) * kTile;
+  const uint32_t tile_count =
+      static_cast<uint32_t>(min(static_cast<uint64_t>(kTile), static_cast<uint64_t>(n) - tile_base));
+
+  uint32_t key[kItems];
+  const uint32_t warp_base = warp * kWarpTile;
+#pragma unroll
+  for (int i = 0; i < kItems; ++i) {
+    const uint32_t t = warp_base + i * 32 + lane;
+    key[i] = t < tile_count ? keys_in[tile_base + t] : 0u;
+  }
+  // rank inside the tile's bin: the counter's value before this key's increment
+  uint16_t rank[kItems];
+#pragma unroll
+  for (int i = 0; i < kItems; ++i) {
+    const uint32_t t = warp_base + i * 32 + lane;
+    if (t < tile_count) {
+      rank[i] = static_cast<uint16_t>(atomicAdd(&sm.bin_cnt[(key[i] >> begin_bit) & dmask], 1u));
+    }
+  }
+  __syncthreads();
+
+  uint32_t cnt[kBinsPerThread];
+  uint32_t mine = 0;
+#pragma unroll
+  for (int j = 0; j < kBinsPerThread; ++j) {
+    cnt[j] = sm.bin_cnt[threadIdx.x * kBinsPerThread + j];
+    mine += cnt[j];
+  }
+  uint32_t total;
+  uint32_t ex = BlockExclusiveSum<uint32_t, kThreads>(mine, sm.scan, &total);
+#pragma unroll
+  for (int j = 0; j < kBinsPerThread; ++j) {
+    sm.bin_off[threadIdx.x * kBinsPerThread + j] = ex;
+    ex += cnt[j];
+  }
+  {
+    uint32_t excl[kBinsPerThread];
+    ChainTileCounts(status, tile, cnt, excl);
+#pragma unroll
+    for (int j = 0; j < kBinsPerThread; ++j) {
+      const uint32_t b = threadIdx.x * kBinsPerThread + j;
+      const uint32_t base = bin_base[b];
+      sm.bin_dst[b] = base + excl[j] - sm.bin_off[b];
+      if (tile == gridDim.x - 1) bin_next[b] = base + excl[j] + cnt[j];
+    }
+  }
+  __syncthreads();
+
+  // staging in bin order, then every bin's run leaves the SM as one coalesced store
+#pragma unroll
+  for (int i = 0; i < kItems; ++i) {
+    const uint32_t t = warp_base + i * 32 + lane;
+    if (t < tile_count) sm.keys[sm.bin_off[(key[i] >> begin_bit) & dmask] + rank[i]] = key[i];
+  }
+  __syncthreads();
+#pragma unroll
+  for (int i = 0; i < kItems; ++i) {
+    const uint32_t s = i * kThreads + threadIdx.x;
+    if (s < tile_count) {
+      const uint32_t k = sm.keys[s];
+      keys_out[sm.bin_dst[(k >> begin_bit) & dmask] + s] = k;
     }
   }
 }
@@ -475,6 +584,68 @@ int RadixSortKeys(Ctx& c, const uint32_t* src_keys, uint32_t* keys_a, uint32_t* 
                   int begin_bit, int end_bit) {
   return SortImpl<uint32_t, uint32_t, false>(c, src_keys, keys_a, keys_b, nullptr, nullptr, nullptr,
                                              n, begin_bit, end_bit, false);
+}
+
+// Unstable partition of u32 keys on their bits [begin_bit, end_bit) (at most 10):
+// the keys of digit d land in dst[bin_start[d], bin_start[d + 1]) in no particular
+// order (bin_start[d + 1] = n past the last digit). bin_start: 1024 entries, left on
+// the device for the caller.
+void RadixPartitionKeys(Ctx& c, const uint32_t* src, uint32_t* dst, uint64_t n, int begin_bit,
+                        int end_bit, uint32_t* bin_start) {
+  if (n >= 0xFFFFFFFFULL) throw LimitError("radix partition of 2^32 or more records");
+  if (end_bit - begin_bit < 1 || end_bit - begin_bit > kRadixMaxBits) {
+    throw InvalidArgument("radix partition: 1 to 10 key bits");
+  }
+  PassPlan plan{};
+  plan.n_passes = 1;
+  plan.begin[0] = begin_bit;
+  plan.bits[0] = end_bit - begin_bit;
+  constexpr uint64_t kTile = kThreads * Items<uint32_t>::value;
+  // status words count below 2^30: portion by portion, as in SortImpl
+  const uint64_t portion = ((1ULL << 30) - 1) / kTile * kTile;
+  const uint64_t n_portions = (n + portion - 1) / portion;
+  const uint64_t max_tiles = (std::min(n, portion) + kTile - 1) / kTile;
+  const size_t hist_bytes = sizeof(uint64_t) * kBins;
+  const size_t base_bytes = sizeof(uint32_t) * kBins;
+  const size_t ticket_bytes = sizeof(unsigned int) * kMaxPasses * 8;
+  if (n_portions > kMaxPasses * 8) throw LimitError("radix partition: too many launches");
+  const size_t head = hist_bytes + 2 * base_bytes + ticket_bytes;
+  const size_t status_bytes = sizeof(uint32_t) * max_tiles * kBins;
+  uint8_t* scratch = c.sort_tmp.reserve(head + status_bytes + 256);
+  auto* hist = reinterpret_cast<unsigned long long*>(scratch);
+  uint32_t* bases[2] = {reinterpret_cast<uint32_t*>(scratch + hist_bytes),
+                        reinterpret_cast<uint32_t*>(scratch + hist_bytes + base_bytes)};
+  auto* ticket = reinterpret_cast<unsigned int*>(scratch + hist_bytes + 2 * base_bytes);
+  auto* status = reinterpret_cast<uint32_t*>(scratch + head);
+  RVN_CUDA(cudaMemsetAsync(scratch, 0, head, c.stream));
+  if (n == 0) {
+    RVN_CUDA(cudaMemsetAsync(bin_start, 0, base_bytes, c.stream));
+    return;
+  }
+  const unsigned hgrid =
+      static_cast<unsigned>(std::min<uint64_t>((n + kThreads - 1) / kThreads, c.sms * 8));
+  RadixHistogramKernel<uint32_t><<<hgrid, kThreads, sizeof(uint32_t) * kBins, c.stream>>>(
+      src, n, plan, 0u, hist);
+  RadixScanBinsKernel<<<1, kBins, 0, c.stream>>>(hist, 1, bases[0]);
+  RVN_LAUNCH_CHECK();
+  c.launches += 2;
+  // (bases[0] is overwritten from the third portion on)
+  RVN_CUDA(cudaMemcpyAsync(bin_start, bases[0], base_bytes, cudaMemcpyDeviceToDevice, c.stream));
+  RVN_CUDA(cudaFuncSetAttribute(PartitionPass, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                static_cast<int>(sizeof(PartitionSmem))));
+  int cur = 0;
+  for (uint64_t q = 0; q < n_portions; ++q) {
+    const uint64_t first = q * portion;
+    const uint64_t cnt = std::min(portion, n - first);
+    const uint64_t tiles = (cnt + kTile - 1) / kTile;
+    RVN_CUDA(cudaMemsetAsync(status, 0, sizeof(uint32_t) * tiles * kBins, c.stream));
+    PartitionPass<<<static_cast<unsigned>(tiles), kThreads, sizeof(PartitionSmem), c.stream>>>(
+        src + first, dst, static_cast<uint32_t>(cnt), plan.begin[0], plan.bits[0], bases[cur],
+        bases[cur ^ 1], status, ticket + q);
+    RVN_LAUNCH_CHECK();
+    ++c.launches;
+    cur ^= 1;
+  }
 }
 
 }  // namespace rvn
