@@ -8,7 +8,7 @@ import subprocess
 import sys
 
 HOT = ["SketchFastKernel", "OnesweepPass", "RadixHistogramKernel", "TierScatterKernel",
-       "GroupCountKernel", "IndexTableKernel", "MicromizeKernel", "JoinProbeKernel",
+       "GroupCountKernel", "IndexTableKernel", "MicromizeKernel", "JoinSweepKernel",
        "ExpandJoinKernel", "SplitKernel", "GroupChainKernel", "PairChainKernel",
        "ColumnsWarpKernel", "LeafKernel", "BandedMyersKernel", "PoaKernelFast",
        "PileRegionsKernel"]

@@ -30,6 +30,7 @@
 #include <cstring>
 
 #include "engine.cuh"
+#include "seed.cuh"
 
 namespace rvn {
 
@@ -120,70 +121,15 @@ __global__ void GatherBoundaries(const uint64_t* __restrict__ src, uint64_t stri
 // ---------------------------------------------------------------------------
 // seed lookup of received queries, hits written into per-destination runs
 // ---------------------------------------------------------------------------
-struct IndexView2 {
-  ValView val;
-  const uint64_t* org;
-  const uint32_t* bucket;
-  uint64_t n;
-  int shift;
-  uint32_t occurrence;
-  uint64_t limit;  // values beyond it are not indexed (tiered build)
-};
-
-__device__ __forceinline__ void Lookup2(const IndexView2& ix, uint64_t v, uint32_t* first,
-                                        uint32_t* count) {
-  if (v > ix.limit) {
-    *first = 0;
-    *count = 0;
-    return;
-  }
-  const uint64_t b = v >> ix.shift;
-  uint32_t lo = ix.bucket[b], hi = ix.bucket[b + 1];
-  while (hi - lo > 8) {
-    const uint32_t mid = lo + (hi - lo) / 2;
-    if (ix.val[mid] < v) lo = mid + 1; else hi = mid;
-  }
-  const uint32_t end = ix.bucket[b + 1];
-  while (lo < end && ix.val[lo] < v) ++lo;
-  if (lo >= end || ix.val[lo] != v) {
-    *first = 0;
-    *count = 0;
-    return;
-  }
-  *first = lo;
-  if (ix.occurrence != 0xFFFFFFFFu && static_cast<uint64_t>(lo) + ix.occurrence < ix.n &&
-      ix.val[static_cast<uint64_t>(lo) + ix.occurrence] == v) {
-    *count = ix.occurrence + 1;
-    return;
-  }
-  uint32_t n = 1;
-  while (static_cast<uint64_t>(lo) + n < ix.n && ix.val[lo + n] == v) ++n;
-  *count = n;
-}
-
-__device__ __forceinline__ bool Keep2(uint32_t lhs_id, uint64_t origin, bool ae, bool as) {
-  const uint32_t rhs_id = static_cast<uint32_t>(origin >> 32);
-  if (ae && lhs_id == rhs_id) return false;
-  if (as && lhs_id > rhs_id) return false;
-  return true;
-}
-
 __global__ void __launch_bounds__(kThreads)
-ProbeOwned(IndexView2 ix, const uint64_t* __restrict__ q_val,
+ProbeOwned(IndexView ix, const uint64_t* __restrict__ q_val,
            const uint64_t* __restrict__ q_org, uint64_t n_q, bool ae, bool as,
            uint32_t* __restrict__ cnt, uint32_t* __restrict__ first) {
   const uint64_t i = static_cast<uint64_t>(blockIdx.x) * kThreads + threadIdx.x;
   if (i >= n_q) return;
-  const uint64_t v = q_val[i];
-  const uint32_t lhs_id = static_cast<uint32_t>(q_org[i] >> 32);
-  uint32_t f, n;
-  Lookup2(ix, v, &f, &n);
-  uint32_t kept = 0;
-  if (n <= ix.occurrence) {
-    for (uint32_t j = 0; j < n; ++j) kept += Keep2(lhs_id, ix.org[f + j], ae, as);
-  }
-  cnt[i] = kept;
-  first[i] = f;
+  uint8_t over;
+  ProbeRun(ix, q_val[i], static_cast<uint32_t>(q_org[i] >> 32), ae, as, first + i, cnt + i,
+           &over);
 }
 
 // the received query records are sorted by read id:
@@ -216,8 +162,21 @@ __global__ void ReadHitTotals(const uint64_t* __restrict__ start,
   tot[Slot(r, parts, per_part)] = static_cast<uint32_t>(t);
 }
 
+// hit stores of the owner path: the query read goes with every hit
+struct OwnedHitStore {
+  uint64_t* grp;
+  uint64_t* pos;
+  uint32_t* lhs;
+  __device__ __forceinline__ void operator()(uint64_t d, uint64_t g, uint64_t p,
+                                             uint32_t lhs_id) const {
+    grp[d] = g;
+    pos[d] = p;
+    lhs[d] = lhs_id;
+  }
+};
+
 __global__ void __launch_bounds__(kThreads)
-ExpandOwned(IndexView2 ix, const uint64_t* __restrict__ q_val,
+ExpandOwned(IndexView ix, const uint64_t* __restrict__ q_val,
             const uint64_t* __restrict__ q_org, uint64_t n_q, bool ae, bool as,
             const uint32_t* __restrict__ cnt, const uint32_t* __restrict__ first,
             const uint64_t* __restrict__ hit_off, const uint64_t* __restrict__ start,
@@ -232,62 +191,34 @@ ExpandOwned(IndexView2 ix, const uint64_t* __restrict__ q_val,
     *bad = 2;  // query records not sorted by read (or a read out of range)
     return;
   }
-  uint32_t left = cnt[i];
+  const uint32_t left = cnt[i];
   if (left == 0) return;
   const uint64_t v = q_val[i];
-  const uint64_t lhs_pos = static_cast<uint32_t>(lo) >> 1;
-  uint64_t dst = read_base[Slot(lhs_id, parts, per_part)] + (hit_off[i] - hit_off[start[lhs_id]]);
-  for (uint64_t j = first[i]; left > 0 && j < ix.n && ix.val[j] == v; ++j) {
-    const uint64_t o = ix.org[j];
-    if (!Keep2(lhs_id, o, ae, as)) continue;
-    const uint64_t rhs_id = o >> 32;
-    const uint64_t strand = (lo & 1) == (o & 1);
-    const uint64_t rhs_pos = static_cast<uint32_t>(o) >> 1;
-    const uint64_t diagonal =
-        !strand ? rhs_pos + lhs_pos : rhs_pos - lhs_pos + (3ULL << 30);
-    h_grp[dst] = (((rhs_id << 1) | strand) << 32) | diagonal;
-    h_pos[dst] = (lhs_pos << 32) | rhs_pos;
-    h_lhs[dst] = lhs_id;
-    ++dst;
-    --left;
-  }
+  const uint64_t dst =
+      read_base[Slot(lhs_id, parts, per_part)] + (hit_off[i] - hit_off[start[lhs_id]]);
+  ExpandRun(ix, v, lo, first[i], left, ae, as, dst, OwnedHitStore{h_grp, h_pos, h_lhs});
 }
 
 // the same two steps for the stage-1 flags (avoid_equal && avoid_symmetric): the
-// kept postings are a suffix of the run (see map.cu: ProbeSuffixKernel), the
-// expansion is done by whole warps with coalesced stores
+// kept postings are a suffix of the run (seed.cuh: ProbeSuffix), the expansion is
+// done by whole warps with coalesced stores
 __global__ void __launch_bounds__(kThreads)
-ProbeOwnedSuffix(IndexView2 ix, const uint64_t* __restrict__ q_val,
+ProbeOwnedSuffix(IndexView ix, const uint64_t* __restrict__ q_val,
                  const uint64_t* __restrict__ q_org, uint64_t n_q,
                  uint32_t* __restrict__ cnt, uint32_t* __restrict__ first) {
   const uint64_t i = static_cast<uint64_t>(blockIdx.x) * kThreads + threadIdx.x;
   if (i >= n_q) return;
-  const uint64_t v = q_val[i];
-  const uint32_t lhs_id = static_cast<uint32_t>(q_org[i] >> 32);
-  uint32_t f, n;
-  Lookup2(ix, v, &f, &n);
-  uint32_t kept = 0, fk = f;
-  if (n <= ix.occurrence && n > 0) {
-    uint32_t lo = f, hi = f + n;  // first posting with rhs_id > lhs_id
-    while (lo < hi) {
-      const uint32_t mid = lo + (hi - lo) / 2;
-      if (static_cast<uint32_t>(ix.org[mid] >> 32) <= lhs_id) lo = mid + 1; else hi = mid;
-    }
-    fk = lo;
-    kept = f + n - fk;
-  }
-  cnt[i] = kept;
-  first[i] = fk;
+  uint8_t over;
+  ProbeSuffix(ix, q_val[i], true, q_org, i, first + i, cnt + i, &over);
 }
 
 __global__ void __launch_bounds__(kThreads)
-ExpandOwnedWarp(IndexView2 ix, const uint64_t* __restrict__ q_org, uint64_t n_q,
+ExpandOwnedWarp(IndexView ix, const uint64_t* __restrict__ q_org, uint64_t n_q,
                 const uint32_t* __restrict__ cnt, const uint32_t* __restrict__ first,
                 const uint64_t* __restrict__ hit_off, const uint64_t* __restrict__ start,
                 const uint64_t* __restrict__ read_base, uint32_t n_reads, uint32_t parts,
                 uint32_t per_part, uint64_t* __restrict__ h_grp, uint64_t* __restrict__ h_pos,
                 uint32_t* __restrict__ h_lhs, uint32_t* __restrict__ bad) {
-  const uint32_t lane = threadIdx.x & 31;
   const uint64_t i = static_cast<uint64_t>(blockIdx.x) * kThreads + threadIdx.x;
   bool valid = i < n_q;
   uint32_t my_cnt = 0, my_first = 0;
@@ -304,41 +235,8 @@ ExpandOwnedWarp(IndexView2 ix, const uint64_t* __restrict__ q_org, uint64_t n_q,
       my_dst = read_base[Slot(lhs_id, parts, per_part)] + (hit_off[i] - hit_off[start[lhs_id]]);
     }
   }
-  // exclusive prefix of the 32 counts
-  uint32_t incl = my_cnt;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const uint32_t o = __shfl_up_sync(0xFFFFFFFFu, incl, d);
-    if (lane >= static_cast<uint32_t>(d)) incl += o;
-  }
-  const uint32_t rel = incl - my_cnt;
-  const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
-  for (uint32_t t0 = 0; t0 < total; t0 += 32) {
-    const uint32_t t = t0 + lane;
-    uint32_t q = 0;  // largest q with rel[q] <= t
-#pragma unroll
-    for (uint32_t step = 16; step > 0; step >>= 1) {
-      const uint32_t r = __shfl_sync(0xFFFFFFFFu, rel, q + step);
-      if (r <= t) q += step;
-    }
-    const uint32_t qrel = __shfl_sync(0xFFFFFFFFu, rel, q);
-    const uint32_t qfirst = __shfl_sync(0xFFFFFFFFu, my_first, q);
-    const uint64_t lo = __shfl_sync(0xFFFFFFFFu, my_org, q);
-    const uint64_t qdst = __shfl_sync(0xFFFFFFFFu, my_dst, q);
-    if (t < total) {
-      const uint64_t o = ix.org[qfirst + (t - qrel)];
-      const uint64_t lhs_pos = static_cast<uint32_t>(lo) >> 1;
-      const uint64_t rhs_id = o >> 32;
-      const uint64_t strand = (lo & 1) == (o & 1);
-      const uint64_t rhs_pos = static_cast<uint32_t>(o) >> 1;
-      const uint64_t diagonal =
-          !strand ? rhs_pos + lhs_pos : rhs_pos - lhs_pos + (3ULL << 30);
-      const uint64_t dst = qdst + (t - qrel);
-      h_grp[dst] = (((rhs_id << 1) | strand) << 32) | diagonal;
-      h_pos[dst] = (lhs_pos << 32) | rhs_pos;
-      h_lhs[dst] = static_cast<uint32_t>(lo >> 32);
-    }
-  }
+  ExpandWarp(ix.org, threadIdx.x & 31, my_cnt, my_first, my_org, my_dst,
+             OwnedHitStore{h_grp, h_pos, h_lhs});
 }
 
 // ---------------------------------------------------------------------------
@@ -576,8 +474,8 @@ void DistHitsSplit(Ctx& c, const uint64_t* d_qval, const uint64_t* d_qorg, uint6
   if (!c.i_valid) throw StateError("no index");
   CheckParts(parts, 0);
   if (n_query > c.n_reads) throw InvalidArgument("query range out of bounds");
-  IndexView2 ix{ValView{c.i_val.get(), c.i_is32 ? 1 : 0}, c.i_org.get(), c.i_bucket.get(), c.i_n,
-                c.i_shift, c.occurrence, c.i_limit};
+  IndexView ix{ValView{c.i_val.get(), c.i_is32 ? 1 : 0}, c.i_org.get(), c.i_bucket.get(), c.i_n,
+               c.i_shift, c.occurrence, c.i_limit};
   const uint32_t per_part = CeilDiv(n_query, parts);
   const uint64_t slots = static_cast<uint64_t>(per_part) * parts;
   uint32_t* cnt = c.m_cnt.reserve(n_q + 1);

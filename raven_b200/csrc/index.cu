@@ -17,6 +17,7 @@
 #include <cooperative_groups.h>
 
 #include "engine.cuh"
+#include "seed.cuh"
 
 namespace rvn {
 
@@ -122,22 +123,11 @@ IndexTableKernel(const ValT* __restrict__ val, uint64_t n, int shift,
   // total belongs to the lane found by a shuffle search over the prefixes
   {
     const uint32_t lane = threadIdx.x & 31;
-    uint32_t incl = fill_cnt;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const uint32_t o = __shfl_up_sync(0xFFFFFFFFu, incl, d);
-      if (lane >= static_cast<uint32_t>(d)) incl += o;
-    }
-    const uint32_t rel = incl - fill_cnt;
-    const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
+    uint32_t total;
+    const uint32_t rel = WarpExclusiveSum(fill_cnt, lane, &total);
     for (uint32_t t0 = 0; t0 < total; t0 += 32) {
       const uint32_t t = t0 + lane;
-      uint32_t q = 0;
-#pragma unroll
-      for (uint32_t step = 16; step > 0; step >>= 1) {
-        const uint32_t r = __shfl_sync(0xFFFFFFFFu, rel, q + step);
-        if (r <= t) q += step;
-      }
+      const uint32_t q = WarpSlotLane(rel, t);
       const uint32_t qrel = __shfl_sync(0xFFFFFFFFu, rel, q);
       const uint64_t qlo = __shfl_sync(0xFFFFFFFFu, fill_lo, q);
       if (kFill && t < total) bucket[qlo + (t - qrel)] = static_cast<uint32_t>(base + (threadIdx.x & ~31u) + q);

@@ -24,69 +24,13 @@
 #include <algorithm>
 
 #include "engine.cuh"
+#include "seed.cuh"
 
 namespace rvn {
 
 namespace {
 
 constexpr int kThreads = 256;
-
-struct IndexView {
-  ValView val;  // sorted values, u32 or u64
-  const uint64_t* org;
-  const uint32_t* bucket;
-  uint64_t n;
-  int shift;
-  uint32_t occurrence;
-  uint64_t limit;  // values beyond it are not indexed (tiered build)
-};
-
-// first record with value v and the run length capped at occurrence+1
-__device__ __forceinline__ void Lookup(const IndexView& ix, uint64_t v,
-                                       uint32_t* first, uint32_t* count) {
-  if (v > ix.limit) {
-    *first = 0;
-    *count = 0;
-    return;
-  }
-  const uint64_t b = v >> ix.shift;
-  uint32_t lo = ix.bucket[b], hi = ix.bucket[b + 1];
-  while (hi - lo > 8) {  // long buckets: bisect down to a short scan
-    const uint32_t mid = lo + (hi - lo) / 2;
-    if (ix.val[mid] < v) {
-      lo = mid + 1;
-    } else {
-      hi = mid;
-    }
-  }
-  // here every record before lo is < v; the run (if any) starts in [lo, hi]
-  const uint32_t end = ix.bucket[b + 1];
-  while (lo < end && ix.val[lo] < v) ++lo;
-  if (lo >= end || ix.val[lo] != v) {
-    *first = 0;
-    *count = 0;
-    return;
-  }
-  *first = lo;
-  if (ix.occurrence != 0xFFFFFFFFu &&
-      static_cast<uint64_t>(lo) + ix.occurrence < ix.n &&
-      ix.val[static_cast<uint64_t>(lo) + ix.occurrence] == v) {
-    *count = ix.occurrence + 1;  // over the threshold, exact length not needed
-    return;
-  }
-  uint32_t n = 1;
-  while (static_cast<uint64_t>(lo) + n < ix.n && ix.val[lo + n] == v) ++n;
-  *count = n;
-}
-
-__device__ __forceinline__ bool KeepPosting(uint32_t lhs_id, uint64_t origin,
-                                            bool avoid_equal,
-                                            bool avoid_symmetric) {
-  const uint32_t rhs_id = static_cast<uint32_t>(origin >> 32);
-  if (avoid_equal && lhs_id == rhs_id) return false;
-  if (avoid_symmetric && lhs_id > rhs_id) return false;
-  return true;
-}
 
 __global__ void __launch_bounds__(kThreads)
 ProbeKernel(IndexView ix, ValView q_val,
@@ -96,25 +40,22 @@ ProbeKernel(IndexView ix, ValView q_val,
             uint8_t* __restrict__ filt) {
   const uint64_t i = static_cast<uint64_t>(blockIdx.x) * kThreads + threadIdx.x;
   if (i >= n_q) return;
-  const uint64_t v = q_val[q_begin + i];
   const uint32_t lhs_id = static_cast<uint32_t>(q_org[q_begin + i] >> 32);
-  uint32_t f, n;
-  Lookup(ix, v, &f, &n);
-  uint32_t kept = 0;
-  uint8_t over = 0;
-  if (n > ix.occurrence) {
-    over = 1;
-    n = 0;
-  } else {
-    for (uint32_t j = 0; j < n; ++j) {
-      kept += KeepPosting(lhs_id, ix.org[f + j], avoid_equal, avoid_symmetric);
-    }
-  }
-  cnt[i] = kept;
-  first[i] = f;
-  filt[i] = over;
+  ProbeRun(ix, q_val[q_begin + i], lhs_id, avoid_equal, avoid_symmetric, first + i, cnt + i,
+           filt + i);
   // the posting count is re-derived in ExpandKernel from the run itself
 }
+
+// hit stores of the single-GPU map: one array of groups, one of positions
+struct HitStore {
+  uint64_t* grp;
+  uint64_t* pos;
+  __device__ __forceinline__ void operator()(uint64_t d, uint64_t g, uint64_t p,
+                                             uint32_t) const {
+    grp[d] = g;
+    pos[d] = p;
+  }
+};
 
 __global__ void __launch_bounds__(kThreads)
 ExpandKernel(IndexView ix, ValView q_val,
@@ -126,36 +67,20 @@ ExpandKernel(IndexView ix, ValView q_val,
              uint64_t* __restrict__ h_pos) {
   const uint64_t i = static_cast<uint64_t>(blockIdx.x) * kThreads + threadIdx.x;
   if (i >= n_q) return;
-  uint32_t left = cnt[i];
+  const uint32_t left = cnt[i];
   if (left == 0) return;
   const uint64_t v = q_val[q_begin + i];
   const uint64_t lo = q_org[q_begin + i];
-  const uint32_t lhs_id = static_cast<uint32_t>(lo >> 32);
-  const uint64_t lhs_pos = static_cast<uint32_t>(lo) >> 1;
-  uint64_t dst = hit_off[i];
-  for (uint64_t j = first[i]; left > 0 && j < ix.n && ix.val[j] == v; ++j) {
-    const uint64_t o = ix.org[j];
-    if (!KeepPosting(lhs_id, o, avoid_equal, avoid_symmetric)) continue;
-    const uint64_t rhs_id = o >> 32;
-    const uint64_t strand = (lo & 1) == (o & 1);
-    const uint64_t rhs_pos = static_cast<uint32_t>(o) >> 1;
-    const uint64_t diagonal =
-        !strand ? rhs_pos + lhs_pos : rhs_pos - lhs_pos + (3ULL << 30);
-    h_grp[dst] = (((rhs_id << 1) | strand) << 32) | diagonal;
-    h_pos[dst] = (lhs_pos << 32) | rhs_pos;
-    ++dst;
-    --left;
-  }
+  const uint64_t dst = hit_off[i];
+  ExpandRun(ix, v, lo, first[i], left, avoid_equal, avoid_symmetric, dst,
+            HitStore{h_grp, h_pos});
 }
 
 // ---- fast path of probe + expand -------------------------------------------
-// The postings of a key are in read order (the index sort is stable over
-// records in (read, position) order), so with avoid_equal && avoid_symmetric
-// the kept postings (rhs_id > lhs_id) are a SUFFIX of the run - and with both
-// flags off they are the whole run. The probe then only needs the first kept
-// posting (a binary search in the run), and the expansion can be done by whole
-// warps with fully coalesced stores: hit t of a warp's 32 queries is located
-// by a shuffle search over the 32 exclusive prefixes.
+// With avoid_equal && avoid_symmetric over an index sorted by read, or with both
+// flags off, the kept postings are a SUFFIX of the run (seed.cuh: ProbeSuffix). The
+// probe then only needs the first kept posting, and the expansion can be done by
+// whole warps with fully coalesced stores (seed.cuh: ExpandWarp).
 __global__ void __launch_bounds__(kThreads)
 ProbeSuffixKernel(IndexView ix, ValView q_val,
                   const uint64_t* __restrict__ q_org, uint64_t q_begin, uint64_t n_q,
@@ -163,28 +88,8 @@ ProbeSuffixKernel(IndexView ix, ValView q_val,
                   uint32_t* __restrict__ first, uint8_t* __restrict__ filt) {
   const uint64_t i = static_cast<uint64_t>(blockIdx.x) * kThreads + threadIdx.x;
   if (i >= n_q) return;
-  const uint64_t v = q_val[q_begin + i];
-  uint32_t f, n;
-  Lookup(ix, v, &f, &n);
-  uint8_t over = 0;
-  uint32_t kept = 0, fk = f;
-  if (n > ix.occurrence) {
-    over = 1;
-  } else if (n > 0) {
-    if (strict_above) {
-      const uint32_t lhs_id = static_cast<uint32_t>(q_org[q_begin + i] >> 32);
-      uint32_t lo = f, hi = f + n;  // first posting with rhs_id > lhs_id
-      while (lo < hi) {
-        const uint32_t mid = lo + (hi - lo) / 2;
-        if (static_cast<uint32_t>(ix.org[mid] >> 32) <= lhs_id) lo = mid + 1; else hi = mid;
-      }
-      fk = lo;
-    }
-    kept = f + n - fk;
-  }
-  cnt[i] = kept;
-  first[i] = fk;
-  filt[i] = over;
+  ProbeSuffix(ix, q_val[q_begin + i], strict_above, q_org + q_begin, i, first + i, cnt + i,
+              filt + i);
 }
 
 // the same probe over queries sorted by value: neighbouring threads walk
@@ -199,24 +104,9 @@ ProbeSortedKernel(IndexView ix, ValView sorted_val,
   if (t >= n_q) return;
   const uint64_t v = sorted_val[t];
   const uint32_t i = sorted_idx[t];
-  uint32_t f, n;
-  Lookup(ix, v, &f, &n);
-  uint8_t over = 0;
-  uint32_t kept = 0, fk = f;
-  if (n > ix.occurrence) {
-    over = 1;
-  } else if (n > 0) {
-    if (strict_above) {
-      const uint32_t lhs_id = static_cast<uint32_t>(q_org[q_begin + i] >> 32);
-      uint32_t lo = f, hi = f + n;
-      while (lo < hi) {
-        const uint32_t mid = lo + (hi - lo) / 2;
-        if (static_cast<uint32_t>(ix.org[mid] >> 32) <= lhs_id) lo = mid + 1; else hi = mid;
-      }
-      fk = lo;
-    }
-    kept = f + n - fk;
-  }
+  uint32_t fk, kept;
+  uint8_t over;
+  ProbeSuffix(ix, v, strict_above, q_org + q_begin, i, &fk, &kept, &over);
   // ONE scattered store per query (a partial-sector write costs a read-modify-
   // write in HBM): first kept posting | over-threshold flag | kept count
   packed[i] = (static_cast<uint64_t>(fk) << 32) | (static_cast<uint64_t>(over) << 31) | kept;
@@ -239,49 +129,10 @@ ExpandWarpKernel(IndexView ix, const uint64_t* __restrict__ q_org, uint64_t q_be
                  uint64_t n_q, const uint32_t* __restrict__ cnt,
                  const uint32_t* __restrict__ first, const uint64_t* __restrict__ hit_off,
                  uint64_t* __restrict__ h_grp, uint64_t* __restrict__ h_pos) {
-  const uint32_t lane = threadIdx.x & 31;
   const uint64_t i = (static_cast<uint64_t>(blockIdx.x) * kThreads + threadIdx.x);
   const bool valid = i < n_q;
-  const uint32_t my_cnt = valid ? cnt[i] : 0;
-  const uint32_t my_first = valid ? first[i] : 0;
-  const uint64_t my_org = valid ? q_org[q_begin + i] : 0;
-  const uint64_t my_off = valid ? hit_off[i] : 0;
-  // exclusive prefix of the warp, relative to its first query (lanes beyond n_q
-  // only occur at the very end: give them the running end)
-  const uint64_t base = __shfl_sync(0xFFFFFFFFu, my_off, 0);
-  uint32_t rel = valid ? static_cast<uint32_t>(my_off - base) : 0;
-  // total and a monotone prefix for the invalid tail lanes
-  uint32_t run = valid ? rel + my_cnt : 0;
-  for (int d = 1; d < 32; d <<= 1) {
-    const uint32_t o = __shfl_up_sync(0xFFFFFFFFu, run, d);
-    if (lane >= d && o > run) run = o;
-  }
-  if (!valid) rel = run;
-  const uint32_t total = __shfl_sync(0xFFFFFFFFu, run, 31);
-  for (uint32_t t0 = 0; t0 < total; t0 += 32) {
-    const uint32_t t = t0 + lane;
-    // largest q with rel[q] <= t
-    uint32_t q = 0;
-#pragma unroll
-    for (uint32_t step = 16; step > 0; step >>= 1) {
-      const uint32_t r = __shfl_sync(0xFFFFFFFFu, rel, q + step);
-      if (r <= t) q += step;
-    }
-    const uint32_t qrel = __shfl_sync(0xFFFFFFFFu, rel, q);
-    const uint32_t qfirst = __shfl_sync(0xFFFFFFFFu, my_first, q);
-    const uint64_t lo = __shfl_sync(0xFFFFFFFFu, my_org, q);
-    if (t < total) {
-      const uint64_t o = ix.org[qfirst + (t - qrel)];
-      const uint64_t lhs_pos = static_cast<uint32_t>(lo) >> 1;
-      const uint64_t rhs_id = o >> 32;
-      const uint64_t strand = (lo & 1) == (o & 1);
-      const uint64_t rhs_pos = static_cast<uint32_t>(o) >> 1;
-      const uint64_t diagonal =
-          !strand ? rhs_pos + lhs_pos : rhs_pos - lhs_pos + (3ULL << 30);
-      h_grp[base + t] = (((rhs_id << 1) | strand) << 32) | diagonal;
-      h_pos[base + t] = (lhs_pos << 32) | rhs_pos;
-    }
-  }
+  ExpandWarp(ix.org, threadIdx.x & 31, valid ? cnt[i] : 0, valid ? first[i] : 0,
+             valid ? q_org[q_begin + i] : 0, valid ? hit_off[i] : 0, HitStore{h_grp, h_pos});
 }
 
 // ---- stage-1 hits by a self-join over the index ----
@@ -452,7 +303,6 @@ __global__ void __launch_bounds__(kThreads)
 ExpandJoinKernel(const uint64_t* __restrict__ i_org, const uint64_t* __restrict__ packed,
                  uint64_t n_q, const uint64_t* __restrict__ hit_off,
                  uint64_t* __restrict__ h_grp, uint64_t* __restrict__ h_pos) {
-  const uint32_t lane = threadIdx.x & 31;
   const uint64_t i = (static_cast<uint64_t>(blockIdx.x) * kThreads + threadIdx.x);
   const bool valid = i < n_q;
   const uint64_t pk = valid ? packed[i] : 0;
@@ -465,39 +315,8 @@ ExpandJoinKernel(const uint64_t* __restrict__ i_org, const uint64_t* __restrict_
     my_first = post + 1;
     while ((i_org[my_first] >> 32) == (my_org >> 32)) ++my_first;  // same read: not a hit
   }
-  const uint64_t my_off = valid ? hit_off[i] : 0;
-  const uint64_t base = __shfl_sync(0xFFFFFFFFu, my_off, 0);
-  uint32_t rel = valid ? static_cast<uint32_t>(my_off - base) : 0;
-  uint32_t run = valid ? rel + my_cnt : 0;
-  for (int d = 1; d < 32; d <<= 1) {
-    const uint32_t o = __shfl_up_sync(0xFFFFFFFFu, run, d);
-    if (lane >= d && o > run) run = o;
-  }
-  if (!valid) rel = run;
-  const uint32_t total = __shfl_sync(0xFFFFFFFFu, run, 31);
-  for (uint32_t t0 = 0; t0 < total; t0 += 32) {
-    const uint32_t t = t0 + lane;
-    uint32_t q = 0;
-#pragma unroll
-    for (uint32_t step = 16; step > 0; step >>= 1) {
-      const uint32_t r = __shfl_sync(0xFFFFFFFFu, rel, q + step);
-      if (r <= t) q += step;
-    }
-    const uint32_t qrel = __shfl_sync(0xFFFFFFFFu, rel, q);
-    const uint32_t qfirst = __shfl_sync(0xFFFFFFFFu, my_first, q);
-    const uint64_t lo = __shfl_sync(0xFFFFFFFFu, my_org, q);
-    if (t < total) {
-      const uint64_t o = i_org[qfirst + (t - qrel)];
-      const uint64_t lhs_pos = static_cast<uint32_t>(lo) >> 1;
-      const uint64_t rhs_id = o >> 32;
-      const uint64_t strand = (lo & 1) == (o & 1);
-      const uint64_t rhs_pos = static_cast<uint32_t>(o) >> 1;
-      const uint64_t diagonal =
-          !strand ? rhs_pos + lhs_pos : rhs_pos - lhs_pos + (3ULL << 30);
-      h_grp[base + t] = (((rhs_id << 1) | strand) << 32) | diagonal;
-      h_pos[base + t] = (lhs_pos << 32) | rhs_pos;
-    }
-  }
+  ExpandWarp(i_org, threadIdx.x & 31, my_cnt, my_first, my_org, valid ? hit_off[i] : 0,
+             HitStore{h_grp, h_pos});
 }
 
 // per-read offsets out of per-record offsets
@@ -1482,6 +1301,219 @@ void JoinSweep(Ctx& c, uint32_t first) {
   c.j_first = first;
 }
 
+struct HitCounts {
+  uint64_t n_q = 0, n_hits = 0;  // query records, seed hits
+};
+
+// Per-read hit ranges of the range's nr reads: read_hit_off[i] = hit_off[read_off[i] -
+// q_begin] for i in [0, nr], on the device and in h_rho.
+void ReadHitRanges(Ctx& c, const uint64_t* hit_off, const uint64_t* read_off, uint64_t q_begin,
+                   uint32_t nr, uint64_t* read_hit_off, std::vector<uint64_t>& h_rho) {
+  GatherU64<<<CeilDiv(nr + 1ULL, kThreads), kThreads, 0, c.stream>>>(
+      hit_off, read_off, q_begin, nr + 1ULL, read_hit_off);
+  RVN_LAUNCH_CHECK();
+  ++c.launches;
+  RVN_CUDA(cudaMemcpyAsync(h_rho.data(), read_hit_off, (nr + 1ULL) * sizeof(uint64_t),
+                           cudaMemcpyDeviceToHost, c.stream));
+  RVN_CUDA(cudaStreamSynchronize(c.stream));
+}
+
+// Stage-1 hits of reads [first, last) inside the index batch, by the self-join: the
+// sweep if the slots are stale, then this range's slice of the slots is scanned and
+// expanded into c.h_grp / c.h_pos.
+HitCounts JoinHits(Ctx& c, uint32_t first, uint32_t last, uint64_t* read_hit_off,
+                   std::vector<uint64_t>& h_rho) {
+  const uint32_t nr = last - first;
+  HitCounts h;
+  const bool sweep = c.j_gen != c.i_gen || c.j_occurrence != c.occurrence || first < c.j_first;
+  if (sweep && !(c.qt_valid && c.qt_first <= first && c.i_last <= c.qt_last)) {
+    EnsureThresholds(c, first, c.i_last);  // (its sketch and micromize time are not probe's)
+  }
+  TimerBegin(c, "probe");
+  if (sweep) JoinSweep(c, first);
+  const uint64_t b0 = first - c.j_first;
+  const uint64_t q_begin = c.h_j_off[b0];
+  h.n_q = c.h_j_off[b0 + nr] - q_begin;
+  const uint64_t* packed = c.j_packed.get() + q_begin;
+  uint64_t* hit_off = c.m_hit_off.reserve(h.n_q + 2);
+  if (h.n_q > 0) {
+    uint32_t* cnt = c.m_cnt.reserve(h.n_q + 1);
+    UnpackJoin<<<CeilDiv(h.n_q, kThreads), kThreads, 0, c.stream>>>(packed, h.n_q, cnt);
+    RVN_LAUNCH_CHECK();
+    ++c.launches;
+    ExclusiveScanU32(c, cnt, hit_off, h.n_q);
+    h.n_hits = ReadU64(c, hit_off + h.n_q);
+  } else {
+    RVN_CUDA(cudaMemsetAsync(hit_off, 0, sizeof(uint64_t), c.stream));
+  }
+  TimerEnd(c);
+  TimerBegin(c, "expand");
+  uint64_t* hg = c.h_grp.reserve(h.n_hits + 1);
+  uint64_t* hp = c.h_pos.reserve(h.n_hits + 1);
+  if (h.n_hits > 0) {
+    ExpandJoinKernel<<<CeilDiv(h.n_q, kThreads), kThreads, 0, c.stream>>>(
+        c.i_org.get(), packed, h.n_q, hit_off, hg, hp);
+    RVN_LAUNCH_CHECK();
+    ++c.launches;
+  }
+  ReadHitRanges(c, hit_off, c.j_off.get() + b0, q_begin, nr, read_hit_off, h_rho);
+  TimerEnd(c);
+  c.r_filt_off.reserve(nr + 2ULL);
+  for (uint32_t i = 0; i <= nr; ++i) c.r_filt_off.get()[i] = 0;
+  return h;
+}
+
+// Positions of the over-frequent query minimizers (filt) of the range's nr reads, in
+// sketch order: c.r_filtered, and per-read offsets into it in c.r_filt_off.
+void FilteredPositions(Ctx& c, const uint8_t* filt, const uint64_t* qo, uint64_t q_begin,
+                       uint64_t n_q, const uint64_t* read_off, uint32_t nr) {
+  uint32_t* f32 = c.m_first.get();  // `first` is dead after ExpandKernel
+  FilteredFlagsToU32<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(
+      filt, n_q, f32);
+  uint64_t* fpos = c.m_filt_off.reserve(n_q + 2);
+  ExclusiveScanU32(c, f32, fpos, n_q);
+  const uint64_t n_filtered = ReadU64(c, fpos + n_q);
+  uint32_t* fout = c.m_filtered.reserve(n_filtered + 1);
+  ScatterFiltered<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(
+      filt, fpos, qo, q_begin, n_q, fout);
+  RVN_LAUNCH_CHECK();
+  c.launches += 2;
+  // per-read offsets of the filtered list
+  uint64_t* froff = c.m_ovl_off.reserve(nr + 2ULL);
+  GatherU64<<<CeilDiv(nr + 1ULL, kThreads), kThreads, 0, c.stream>>>(
+      fpos, read_off, q_begin, nr + 1ULL, froff);
+  RVN_LAUNCH_CHECK();
+  ++c.launches;
+  uint32_t* hf = c.r_filtered.reserve(n_filtered + 1);
+  RVN_CUDA(cudaMemcpyAsync(hf, fout, n_filtered * sizeof(uint32_t),
+                           cudaMemcpyDeviceToHost, c.stream));
+  RVN_CUDA(cudaMemcpyAsync(c.r_filt_off.get(), froff,
+                           (nr + 1ULL) * sizeof(uint64_t),
+                           cudaMemcpyDeviceToHost, c.stream));
+  RVN_CUDA(cudaStreamSynchronize(c.stream));
+}
+
+// Hits of reads [first, last) by probing the index with their query records (the
+// micromizers with minhash, else the full sketch) into c.h_grp / c.h_pos, and the
+// filtered positions if wanted (stage 2).
+HitCounts ProbeHits(Ctx& c, uint32_t first, uint32_t last, bool avoid_equal,
+                    bool avoid_symmetric, bool minhash, bool want_filtered,
+                    uint64_t* read_hit_off, std::vector<uint64_t>& h_rho) {
+  const uint32_t nr = last - first;
+  HitCounts h;
+  // ---- query records ----
+  const uint64_t *qo, *d_read_off;
+  ValView qv;  // query values: u32 for full sketches of k <= 15, else u64
+  const std::vector<uint64_t>* h_read_off;
+  uint64_t off_base_read;  // index of `first` inside the offsets arrays
+  if (minhash) {
+    if (!(c.q_valid && c.q_first <= first && last <= c.q_last)) {
+      EnsureMicromizers(c, first, last);
+    }
+    qv = ValView{c.q_val.get(), c.q_is32 ? 1 : 0};
+    qo = c.q_org.get();
+    d_read_off = c.q_off.get();
+    h_read_off = &c.h_q_off;
+    off_base_read = first - c.q_first;
+  } else {
+    if (!(c.s_valid && c.s_first <= first && last <= c.s_last)) {
+      EnsureSketch(c, first, last);
+    }
+    qv = ValView{c.s_val.get(), c.s_is32 ? 1 : 0};
+    qo = c.s_org.get();
+    d_read_off = c.s_off.get();
+    h_read_off = &c.h_s_off;
+    off_base_read = first - c.s_first;
+  }
+  const uint64_t q_begin = (*h_read_off)[off_base_read];
+  const uint64_t n_q = (*h_read_off)[off_base_read + nr] - q_begin;
+  h.n_q = n_q;
+
+  IndexView ix{ValView{c.i_val.get(), c.i_is32 ? 1 : 0}, c.i_org.get(), c.i_bucket.get(), c.i_n,
+               c.i_shift, c.occurrence, c.i_limit};
+
+  // ---- probe + expand ----
+  TimerBegin(c, "probe");
+  uint32_t* cnt = c.m_cnt.reserve(n_q + 1);
+  uint32_t* frst = c.m_first.reserve(n_q + 1);
+  uint8_t* filt = c.m_filt.reserve(n_q + 1);
+  uint64_t* hit_off = c.m_hit_off.reserve(n_q + 2);
+  // kept postings = a suffix of the run (or the whole run): see ProbeSuffix
+  const bool suffix = (avoid_equal && avoid_symmetric && c.i_sorted_ids) ||
+                      (!avoid_equal && !avoid_symmetric);
+  if (n_q > 0) {
+    if (suffix && n_q >= (1u << 16) && n_q < 0xFFFFFFFFULL) {
+      // sort the queries by value, probe in that order, results back by index
+      uint64_t* k1 = c.m_sq_key.reserve(n_q + 2);
+      uint64_t* k2 = c.m_sq_key2.reserve(n_q);
+      uint32_t* v1 = c.m_sq_idx.reserve(n_q);
+      uint32_t* v2 = c.m_sq_idx2.reserve(n_q);
+      IotaU32<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(v1, n_q);
+      // FULL value order: consecutive probes then walk consecutive buckets, values
+      // and postings (the reads of a warp fall into a few hundred bytes instead of
+      // one 32-byte sector per probe per array)
+      const int hi_bit = static_cast<int>(2 * c.prm.k);
+      int w_q;
+      ValView sorted_qv;
+      if (qv.is32) {
+        const uint32_t* src = static_cast<const uint32_t*>(qv.p) + q_begin;
+        uint32_t* a32 = reinterpret_cast<uint32_t*>(k1);
+        uint32_t* b32 = a32 + n_q + (n_q & 1);  // second half of k1 (8-byte aligned)
+        w_q = RadixSortPairs(c, src, a32, b32, v1, v2, v1, n_q, 0, hi_bit);
+        sorted_qv = ValView{w_q < 0 ? src : (w_q == 0 ? a32 : b32), 1};
+      } else {
+        const uint64_t* src = static_cast<const uint64_t*>(qv.p) + q_begin;
+        w_q = RadixSortPairs(c, src, k1, k2, v1, v2, v1, n_q, 0, hi_bit);
+        sorted_qv = ValView{w_q < 0 ? src : (w_q == 0 ? k1 : k2), 0};
+      }
+      const uint32_t* sorted_qi = w_q == 0 ? v2 : v1;
+      // (a key buffer the sort did not end in receives the packed results)
+      uint64_t* packed = (qv.is32 || w_q == 0) ? k2 : k1;
+      ProbeSortedKernel<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(
+          ix, sorted_qv, sorted_qi, qo, q_begin, n_q, avoid_equal, packed);
+      UnpackProbe<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(packed, n_q, cnt, frst, filt);
+      c.launches += (2 * c.prm.k + 7) / 8 + 5;
+    } else if (suffix) {
+      ProbeSuffixKernel<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(
+          ix, qv, qo, q_begin, n_q, avoid_equal, cnt, frst, filt);
+    } else {
+      ProbeKernel<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(
+          ix, qv, qo, q_begin, n_q, avoid_equal, avoid_symmetric, cnt, frst, filt);
+    }
+    RVN_LAUNCH_CHECK();
+    ++c.launches;
+    ExclusiveScanU32(c, cnt, hit_off, n_q);
+    h.n_hits = ReadU64(c, hit_off + n_q);
+  } else {
+    RVN_CUDA(cudaMemsetAsync(hit_off, 0, sizeof(uint64_t), c.stream));
+  }
+  TimerEnd(c);
+  TimerBegin(c, "expand");
+  uint64_t* hg = c.h_grp.reserve(h.n_hits + 1);
+  uint64_t* hp = c.h_pos.reserve(h.n_hits + 1);
+  if (h.n_hits > 0) {
+    if (suffix) {
+      ExpandWarpKernel<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(
+          ix, qo, q_begin, n_q, cnt, frst, hit_off, hg, hp);
+    } else {
+      ExpandKernel<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(
+          ix, qv, qo, q_begin, n_q, avoid_equal, avoid_symmetric, cnt, frst,
+          hit_off, hg, hp);
+    }
+    RVN_LAUNCH_CHECK();
+    ++c.launches;
+  }
+  ReadHitRanges(c, hit_off, d_read_off + off_base_read, q_begin, nr, read_hit_off, h_rho);
+  TimerEnd(c);
+
+  c.r_filt_off.reserve(nr + 2ULL);
+  for (uint32_t i = 0; i <= nr; ++i) c.r_filt_off.get()[i] = 0;
+  if (want_filtered && n_q > 0) {
+    FilteredPositions(c, filt, qo, q_begin, n_q, d_read_off + off_base_read, nr);
+  }
+  return h;
+}
+
 }  // namespace
 
 // Chains hits that are already grouped by query read: hits of read i of the
@@ -1744,201 +1776,20 @@ void MapRange(Ctx& c, uint32_t first, uint32_t last, bool avoid_equal,
   c.r_valid = false;
   const uint32_t nr = last - first;
 
-  // ---- stage 1 with the query reads inside the index batch: self-join ----
+  // ---- seed hits: self-join for stage 1 with the query reads inside the index
+  // batch, else probes of the index ----
   const bool join = c.self_join && minhash && avoid_equal && avoid_symmetric && !want_filtered &&
                     c.i_from_sketch && c.i_sorted_ids && c.ids_identity && first >= c.i_first &&
                     last <= c.i_last;
-  uint64_t n_q = 0, n_hits = 0;
-  uint64_t *hg = nullptr, *hp = nullptr;
   uint64_t* read_hit_off = c.m_read_hit_off.reserve(nr + 2ULL);
-  std::vector<uint64_t> h_rho(nr + 1ULL);
-  if (join) {
-    const bool sweep = c.j_gen != c.i_gen || c.j_occurrence != c.occurrence || first < c.j_first;
-    if (sweep && !(c.qt_valid && c.qt_first <= first && c.i_last <= c.qt_last)) {
-      EnsureThresholds(c, first, c.i_last);  // (its sketch and micromize time are not probe's)
-    }
-    TimerBegin(c, "probe");
-    if (sweep) JoinSweep(c, first);
-    const uint64_t b0 = first - c.j_first;
-    const uint64_t q_begin = c.h_j_off[b0];
-    n_q = c.h_j_off[b0 + nr] - q_begin;
-    const uint64_t* packed = c.j_packed.get() + q_begin;
-    uint64_t* hit_off = c.m_hit_off.reserve(n_q + 2);
-    if (n_q > 0) {
-      uint32_t* cnt = c.m_cnt.reserve(n_q + 1);
-      UnpackJoin<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(packed, n_q, cnt);
-      RVN_LAUNCH_CHECK();
-      ++c.launches;
-      ExclusiveScanU32(c, cnt, hit_off, n_q);
-      n_hits = ReadU64(c, hit_off + n_q);
-    } else {
-      RVN_CUDA(cudaMemsetAsync(hit_off, 0, sizeof(uint64_t), c.stream));
-    }
-    TimerEnd(c);
-    TimerBegin(c, "expand");
-    hg = c.h_grp.reserve(n_hits + 1);
-    hp = c.h_pos.reserve(n_hits + 1);
-    if (n_hits > 0) {
-      ExpandJoinKernel<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(
-          c.i_org.get(), packed, n_q, hit_off, hg, hp);
-      RVN_LAUNCH_CHECK();
-      ++c.launches;
-    }
-    GatherU64<<<CeilDiv(nr + 1ULL, kThreads), kThreads, 0, c.stream>>>(
-        hit_off, c.j_off.get() + b0, q_begin, nr + 1ULL, read_hit_off);
-    RVN_LAUNCH_CHECK();
-    ++c.launches;
-    RVN_CUDA(cudaMemcpyAsync(h_rho.data(), read_hit_off, (nr + 1ULL) * sizeof(uint64_t),
-                             cudaMemcpyDeviceToHost, c.stream));
-    RVN_CUDA(cudaStreamSynchronize(c.stream));
-    TimerEnd(c);
-    c.r_filt_off.reserve(nr + 2ULL);
-    for (uint32_t i = 0; i <= nr; ++i) c.r_filt_off.get()[i] = 0;
-  } else {
-  // ---- query records ----
-  const uint64_t *qo, *d_read_off;
-  ValView qv;  // query values: u32 for full sketches of k <= 15, else u64
-  const std::vector<uint64_t>* h_read_off;
-  uint64_t off_base_read;  // index of `first` inside the offsets arrays
-  if (minhash) {
-    if (!(c.q_valid && c.q_first <= first && last <= c.q_last)) {
-      EnsureMicromizers(c, first, last);
-    }
-    qv = ValView{c.q_val.get(), c.q_is32 ? 1 : 0};
-    qo = c.q_org.get();
-    d_read_off = c.q_off.get();
-    h_read_off = &c.h_q_off;
-    off_base_read = first - c.q_first;
-  } else {
-    if (!(c.s_valid && c.s_first <= first && last <= c.s_last)) {
-      EnsureSketch(c, first, last);
-    }
-    qv = ValView{c.s_val.get(), c.s_is32 ? 1 : 0};
-    qo = c.s_org.get();
-    d_read_off = c.s_off.get();
-    h_read_off = &c.h_s_off;
-    off_base_read = first - c.s_first;
-  }
-  const uint64_t q_begin = (*h_read_off)[off_base_read];
-  n_q = (*h_read_off)[off_base_read + nr] - q_begin;
-
-  IndexView ix{ValView{c.i_val.get(), c.i_is32 ? 1 : 0}, c.i_org.get(), c.i_bucket.get(), c.i_n,
-               c.i_shift, c.occurrence, c.i_limit};
-
-  // ---- probe + expand ----
-  TimerBegin(c, "probe");
-  uint32_t* cnt = c.m_cnt.reserve(n_q + 1);
-  uint32_t* frst = c.m_first.reserve(n_q + 1);
-  uint8_t* filt = c.m_filt.reserve(n_q + 1);
-  uint64_t* hit_off = c.m_hit_off.reserve(n_q + 2);
-  // kept postings = a suffix of the run (or the whole run): see ProbeSuffixKernel
-  const bool suffix = (avoid_equal && avoid_symmetric && c.i_sorted_ids) ||
-                      (!avoid_equal && !avoid_symmetric);
-  if (n_q > 0) {
-    if (suffix && n_q >= (1u << 16) && n_q < 0xFFFFFFFFULL) {
-      // sort the queries by value, probe in that order, results back by index
-      uint64_t* k1 = c.m_sq_key.reserve(n_q + 2);
-      uint64_t* k2 = c.m_sq_key2.reserve(n_q);
-      uint32_t* v1 = c.m_sq_idx.reserve(n_q);
-      uint32_t* v2 = c.m_sq_idx2.reserve(n_q);
-      IotaU32<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(v1, n_q);
-      // FULL value order: consecutive probes then walk consecutive buckets, values
-      // and postings (the reads of a warp fall into a few hundred bytes instead of
-      // one 32-byte sector per probe per array)
-      const int hi_bit = static_cast<int>(2 * c.prm.k);
-      int w_q;
-      ValView sorted_qv;
-      if (qv.is32) {
-        const uint32_t* src = static_cast<const uint32_t*>(qv.p) + q_begin;
-        uint32_t* a32 = reinterpret_cast<uint32_t*>(k1);
-        uint32_t* b32 = a32 + n_q + (n_q & 1);  // second half of k1 (8-byte aligned)
-        w_q = RadixSortPairs(c, src, a32, b32, v1, v2, v1, n_q, 0, hi_bit);
-        sorted_qv = ValView{w_q < 0 ? src : (w_q == 0 ? a32 : b32), 1};
-      } else {
-        const uint64_t* src = static_cast<const uint64_t*>(qv.p) + q_begin;
-        w_q = RadixSortPairs(c, src, k1, k2, v1, v2, v1, n_q, 0, hi_bit);
-        sorted_qv = ValView{w_q < 0 ? src : (w_q == 0 ? k1 : k2), 0};
-      }
-      const uint32_t* sorted_qi = w_q == 0 ? v2 : v1;
-      // (a key buffer the sort did not end in receives the packed results)
-      uint64_t* packed = (qv.is32 || w_q == 0) ? k2 : k1;
-      ProbeSortedKernel<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(
-          ix, sorted_qv, sorted_qi, qo, q_begin, n_q, avoid_equal, packed);
-      UnpackProbe<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(packed, n_q, cnt, frst, filt);
-      c.launches += (2 * c.prm.k + 7) / 8 + 5;
-    } else if (suffix) {
-      ProbeSuffixKernel<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(
-          ix, qv, qo, q_begin, n_q, avoid_equal, cnt, frst, filt);
-    } else {
-      ProbeKernel<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(
-          ix, qv, qo, q_begin, n_q, avoid_equal, avoid_symmetric, cnt, frst, filt);
-    }
-    RVN_LAUNCH_CHECK();
-    ++c.launches;
-    ExclusiveScanU32(c, cnt, hit_off, n_q);
-    n_hits = ReadU64(c, hit_off + n_q);
-  } else {
-    RVN_CUDA(cudaMemsetAsync(hit_off, 0, sizeof(uint64_t), c.stream));
-  }
-  TimerEnd(c);
-  TimerBegin(c, "expand");
-  hg = c.h_grp.reserve(n_hits + 1);
-  hp = c.h_pos.reserve(n_hits + 1);
-  if (n_hits > 0) {
-    if (suffix) {
-      ExpandWarpKernel<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(
-          ix, qo, q_begin, n_q, cnt, frst, hit_off, hg, hp);
-    } else {
-      ExpandKernel<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(
-          ix, qv, qo, q_begin, n_q, avoid_equal, avoid_symmetric, cnt, frst,
-          hit_off, hg, hp);
-    }
-    RVN_LAUNCH_CHECK();
-    ++c.launches;
-  }
-  // per-read hit ranges
-  GatherU64<<<CeilDiv(nr + 1ULL, kThreads), kThreads, 0, c.stream>>>(
-      hit_off, d_read_off + off_base_read, q_begin, nr + 1ULL, read_hit_off);
-  RVN_LAUNCH_CHECK();
-  ++c.launches;
-  RVN_CUDA(cudaMemcpyAsync(h_rho.data(), read_hit_off,
-                           (nr + 1ULL) * sizeof(uint64_t),
-                           cudaMemcpyDeviceToHost, c.stream));
-  RVN_CUDA(cudaStreamSynchronize(c.stream));
-  TimerEnd(c);
-
-  // ---- filtered positions (stage 2 only) ----
-  c.r_filt_off.reserve(nr + 2ULL);
-  for (uint32_t i = 0; i <= nr; ++i) c.r_filt_off.get()[i] = 0;
-  uint64_t n_filtered = 0;
-  if (want_filtered && n_q > 0) {
-    uint32_t* f32 = c.m_first.get();  // `first` is dead after ExpandKernel
-    FilteredFlagsToU32<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(
-        filt, n_q, f32);
-    uint64_t* fpos = c.m_filt_off.reserve(n_q + 2);
-    ExclusiveScanU32(c, f32, fpos, n_q);
-    n_filtered = ReadU64(c, fpos + n_q);
-    uint32_t* fout = c.m_filtered.reserve(n_filtered + 1);
-    ScatterFiltered<<<CeilDiv(n_q, kThreads), kThreads, 0, c.stream>>>(
-        filt, fpos, qo, q_begin, n_q, fout);
-    RVN_LAUNCH_CHECK();
-    c.launches += 2;
-    // per-read offsets of the filtered list
-    uint64_t* froff = c.m_ovl_off.reserve(nr + 2ULL);
-    GatherU64<<<CeilDiv(nr + 1ULL, kThreads), kThreads, 0, c.stream>>>(
-        fpos, d_read_off + off_base_read, q_begin, nr + 1ULL, froff);
-    RVN_LAUNCH_CHECK();
-    ++c.launches;
-    uint32_t* hf = c.r_filtered.reserve(n_filtered + 1);
-    RVN_CUDA(cudaMemcpyAsync(hf, fout, n_filtered * sizeof(uint32_t),
-                             cudaMemcpyDeviceToHost, c.stream));
-    RVN_CUDA(cudaMemcpyAsync(c.r_filt_off.get(), froff,
-                             (nr + 1ULL) * sizeof(uint64_t),
-                             cudaMemcpyDeviceToHost, c.stream));
-    RVN_CUDA(cudaStreamSynchronize(c.stream));
-  }
-
-  }  // (probe path)
+  std::vector<uint64_t> h_rho(nr + 1ULL);  // read_hit_off on the host
+  const HitCounts h =
+      join ? JoinHits(c, first, last, read_hit_off, h_rho)
+           : ProbeHits(c, first, last, avoid_equal, avoid_symmetric, minhash, want_filtered,
+                       read_hit_off, h_rho);
+  const uint64_t n_q = h.n_q, n_hits = h.n_hits;
+  const uint64_t* hg = c.h_grp.get();
+  const uint64_t* hp = c.h_pos.get();
 
   if (c.keep_hits) {
     uint64_t* g = c.r_hit_grp.reserve(n_hits + 1);
