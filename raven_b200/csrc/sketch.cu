@@ -322,8 +322,45 @@ SketchKernel(const uint64_t* __restrict__ words,
 // valid windows that contain it (every such minimum is <= hash(q)). About a
 // quarter of the instructions of the generic kernel; same tiles, same look-back,
 // same output order.
+// The records of a tile are compacted in shared memory in output order (values in
+// place over the tile's hashes, origins as 16-bit (q - q0) << 1 | strand) and the
+// whole CTA writes them with aligned 16-byte stores: each warp store fills whole
+// 32-byte sectors instead of a third of ten.
 // ---------------------------------------------------------------------------
 constexpr int kFastGroup = 4;  // consecutive tiles per CTA: one look-back for all
+
+// the n records of one tile, compacted in shared memory in output order, by the CTA
+__device__ __forceinline__ void StoreTileRecords(const uint32_t* __restrict__ sh_val,
+                                                 const uint16_t* __restrict__ sh_org,
+                                                 uint32_t n, uint64_t org_base,
+                                                 uint32_t* __restrict__ out_val,
+                                                 uint64_t* __restrict__ out_org) {
+  {  // values: 4 a store; a head up to the first 16-byte boundary and a tail
+    const uint32_t head =
+        min(n, static_cast<uint32_t>((16 - (reinterpret_cast<uintptr_t>(out_val) & 15)) & 15) / 4);
+    const uint32_t nvec = (n - head) / 4;
+    uint4* vp = reinterpret_cast<uint4*>(out_val + head);
+    for (uint32_t i = threadIdx.x; i < nvec; i += kSketchThreads) {
+      const uint32_t* s = sh_val + head + 4 * i;
+      vp[i] = make_uint4(s[0], s[1], s[2], s[3]);
+    }
+    const uint32_t tail = head + 4 * nvec;
+    if (threadIdx.x < head) out_val[threadIdx.x] = sh_val[threadIdx.x];
+    if (threadIdx.x < n - tail) out_val[tail + threadIdx.x] = sh_val[tail + threadIdx.x];
+  }
+  {  // origins: 2 a store
+    const uint32_t head = min(n, (reinterpret_cast<uintptr_t>(out_org) & 15) ? 1u : 0u);
+    const uint32_t nvec = (n - head) / 2;
+    ulonglong2* op = reinterpret_cast<ulonglong2*>(out_org + head);
+    for (uint32_t i = threadIdx.x; i < nvec; i += kSketchThreads) {
+      const uint16_t* s = sh_org + head + 2 * i;
+      op[i] = make_ulonglong2(org_base + s[0], org_base + s[1]);
+    }
+    const uint32_t tail = head + 2 * nvec;
+    if (threadIdx.x < head) out_org[0] = org_base + sh_org[0];
+    if (threadIdx.x < n - tail) out_org[tail + threadIdx.x] = org_base + sh_org[tail + threadIdx.x];
+  }
+}
 
 template <int W>
 __global__ void __launch_bounds__(kSketchThreads, 4)
@@ -341,25 +378,71 @@ SketchFastKernel(const uint64_t* __restrict__ words, const uint64_t* __restrict_
   constexpr int N = ITEMS + 2 * H;  // hashes a thread looks at
   constexpr int kSlots = kSketchTile + 2 * H;
   constexpr int G = kFastGroup;
+  constexpr uint32_t kTileWords = (kSlots + 31 + 31) / 32 + 3;
   static_assert(kSketchTile == ITEMS * kSketchThreads, "8 positions per thread");
   static_assert(W >= 2 && W <= 8, "window of 2..8 k-mers");
-  __shared__ uint64_t sh_words[(kSlots + 31 + 31) / 32 + 3];
+  static_assert(kSketchTile <= 1u << 15, "16-bit staged origins");
+  // packed words of every tile of the group, staged together up front
+  __shared__ uint64_t sh_words[G][kTileWords];
   // hashes of every tile of the group (they are the output values; a register copy
-  // would cost occupancy): slot j of tile g = position q0 - H + j
+  // would cost occupancy): slot j of tile g = position q0 - H + j. At the write-out
+  // slot e holds the value of the tile's e-th record.
   __shared__ __align__(16) uint32_t sh_hash_all[kFastGroup][kSlots + 8];
-  __shared__ uint32_t sh_scan[34];
+  __shared__ uint16_t sh_org[kSketchTile];  // origins of one tile's records, in order
+  __shared__ uint64_t sh_scan[34];
+  // per tile of the group: read length in k-mers, first position, read id, staged words
+  __shared__ int32_t sh_L[G], sh_q0[G];
+  __shared__ uint32_t sh_id[G], sh_wlo[G], sh_wn[G], sh_wvalid[G];
+  __shared__ const uint64_t* sh_wsrc[G];
   __shared__ uint32_t sh_group;
   __shared__ uint64_t sh_excl;
 
   // ticket: the group of G consecutive tiles this CTA sketches (tiles of one launch
-  // are ordered by (read, position), so a group may span reads)
-  if (threadIdx.x == 0) sh_group = atomicAdd(ticket, 1u);
+  // are ordered by (read, position), so a group may span reads). One lane per tile
+  // then looks up its read, so the G chains of dependent loads overlap.
+  if (threadIdx.x < 32) {
+    uint32_t grp = 0;
+    if (threadIdx.x == 0) grp = atomicAdd(ticket, 1u);
+    grp = __shfl_sync(0xFFFFFFFFu, grp, 0);
+    const uint64_t t = static_cast<uint64_t>(grp) * G + threadIdx.x;
+    if (threadIdx.x < G && t < n_tiles) {
+      const uint64_t tile_base = tile_off[first_read];
+      const bool one_read = last_read - first_read == 1;  // e.g. an external query: no table
+      const uint32_t r = one_read ? first_read : tile_read[tile_base + t];
+      const int32_t L = static_cast<int32_t>(lens[r] - k + 1);  // k-mer positions, >= W
+      const int32_t q0 = static_cast<int32_t>((tile_base + t - tile_off[r]) * kSketchTile);
+      const int32_t q1 = min(q0 + static_cast<int32_t>(kSketchTile), L);
+      const uint64_t wb = woff[r];
+      const uint32_t nwords = static_cast<uint32_t>(woff[r + 1] - wb);
+      // words of positions [q0 - H, q1 + H) (+ k - 1 bases), one spare for the funnel
+      const uint32_t w_lo = static_cast<uint32_t>(max(q0 - H, 0)) >> 5;
+      const uint32_t w_hi = ((static_cast<uint32_t>(min(q1 + H, L)) - 1 + k - 1) >> 5) + 2;
+      sh_L[threadIdx.x] = L;
+      sh_q0[threadIdx.x] = q0;
+      sh_id[threadIdx.x] = ids[r];
+      sh_wlo[threadIdx.x] = w_lo;
+      sh_wn[threadIdx.x] = w_hi - w_lo;
+      sh_wvalid[threadIdx.x] = nwords > w_lo ? nwords - w_lo : 0;
+      sh_wsrc[threadIdx.x] = words + wb + w_lo;
+    }
+    if (threadIdx.x == 0) sh_group = grp;
+  }
   __syncthreads();
   const uint32_t group = sh_group;
   const uint64_t t_first = static_cast<uint64_t>(group) * G;
   const int g_count = static_cast<int>(min(static_cast<uint64_t>(G), n_tiles - t_first));
-  const uint64_t tile_base = tile_off[first_read];
-  const bool one_read = last_read - first_read == 1;  // e.g. an external query: no table
+
+  // ---- stage the packed words of all tiles at once ----
+  constexpr uint32_t kStageIters = (G * kTileWords + kSketchThreads - 1) / kSketchThreads;
+#pragma unroll
+  for (uint32_t it = 0; it < kStageIters; ++it) {
+    const uint32_t idx = it * kSketchThreads + threadIdx.x;
+    const uint32_t g = idx / kTileWords, j = idx - g * kTileWords;
+    if (g < static_cast<uint32_t>(g_count) && j < sh_wn[g]) {
+      sh_words[g][j] = j < sh_wvalid[g] ? __ldg(sh_wsrc[g] + j) : 0ULL;
+    }
+  }
+  __syncthreads();
 
   const uint32_t mask = (1u << (2 * k)) - 1u;
   const uint32_t rshift = 32 - 2 * k;
@@ -373,44 +456,29 @@ SketchFastKernel(const uint64_t* __restrict__ words, const uint64_t* __restrict_
     return fw == rv ? kBad : h;  // palindromic k-mers never enter a window
   };
 
-  uint32_t flags[G], strands[G], ex[G], tot[G], rd[G];
-  int32_t qa_of[G];
+  uint32_t flags[G], strands[G];
 
+  // ---- canonical hashes of every tile ----
 #pragma unroll
   for (int g = 0; g < G; ++g) {
-    flags[g] = strands[g] = ex[g] = tot[g] = rd[g] = 0;
-    qa_of[g] = 0;
+    strands[g] = 0;
     if (g < g_count) {  // (uniform over the CTA)
-      const uint64_t t = t_first + g;
-      const uint32_t r = one_read ? first_read : tile_read[tile_base + t];
-      rd[g] = r;
-      const int32_t L = static_cast<int32_t>(lens[r] - k + 1);  // k-mer positions, >= W
-      const int32_t q0 = static_cast<int32_t>((tile_base + t - tile_off[r]) * kSketchTile);
+      const int32_t L = sh_L[g];
+      const int32_t q0 = sh_q0[g];
       const int32_t q1 = min(q0 + static_cast<int32_t>(kSketchTile), L);
+      const uint32_t w_lo = sh_wlo[g];
+      const uint64_t* sh_w = sh_words[g];
       uint32_t* sh_hash = sh_hash_all[g];
-
-      // ---- stage the packed words of positions [q0 - H, q1 + H) (+ k - 1 bases) ----
-      const uint64_t* rw = words + woff[r];
-      const uint32_t nwords = static_cast<uint32_t>(woff[r + 1] - woff[r]);
-      const int32_t p_lo = max(q0 - H, 0);
-      const uint32_t w_lo = static_cast<uint32_t>(p_lo) >> 5;
-      const uint32_t w_hi = ((static_cast<uint32_t>(min(q1 + H, L)) - 1 + k - 1) >> 5) + 2;
-      __syncthreads();  // the previous tile is done with sh_words
-      for (uint32_t i = w_lo + threadIdx.x; i < w_hi; i += kSketchThreads) {
-        sh_words[i - w_lo] = i < nwords ? __ldg(rw + i) : 0ULL;
-      }
-      __syncthreads();
 
       // ---- own positions: 8 consecutive k-mers out of one 64-bit funnel ----
       const int32_t qa = q0 + static_cast<int32_t>(threadIdx.x) * ITEMS;
-      qa_of[g] = qa;
       {
         const uint32_t wi = (static_cast<uint32_t>(qa) >> 5) - w_lo;
         const uint32_t sh = (static_cast<uint32_t>(qa) & 31) << 1;
         uint64_t lo = 0;
         if (qa < q1) {
-          lo = sh_words[wi] >> sh;
-          if (sh) lo |= sh_words[wi + 1] << (64 - sh);
+          lo = sh_w[wi] >> sh;
+          if (sh) lo |= sh_w[wi + 1] << (64 - sh);
         }
         const uint32_t lo_lo = static_cast<uint32_t>(lo), lo_hi = static_cast<uint32_t>(lo >> 32);
         uint32_t st_bits = 0;
@@ -434,22 +502,34 @@ SketchFastKernel(const uint64_t* __restrict__ words, const uint64_t* __restrict_
         if (p >= 0 && p < L) {
           const uint32_t wi = (static_cast<uint32_t>(p) >> 5) - w_lo;
           const uint32_t sh = (static_cast<uint32_t>(p) & 31) << 1;
-          uint64_t lo = sh_words[wi] >> sh;
-          if (sh) lo |= sh_words[wi + 1] << (64 - sh);
+          uint64_t lo = sh_w[wi] >> sh;
+          if (sh) lo |= sh_w[wi + 1] << (64 - sh);
           uint32_t st;
           h = hash_of(static_cast<uint32_t>(lo), &st);
         }
         sh_hash[left ? threadIdx.x : H + kSketchTile + threadIdx.x - H] = h;
       }
-      __syncthreads();
+    }
+  }
+  __syncthreads();
 
-      // ---- select ----
+  // ---- select; one scan counts the records of all tiles (16 bits a tile) ----
+  static_assert(kSketchTile < (1u << 16) && G <= 4, "tile counts packed in a u64");
+  uint64_t packed = 0;
+#pragma unroll
+  for (int g = 0; g < G; ++g) {
+    flags[g] = 0;
+    if (g < g_count) {
+      const int32_t L = sh_L[g];
+      const int32_t q0 = sh_q0[g];
+      const int32_t q1 = min(q0 + static_cast<int32_t>(kSketchTile), L);
+      const int32_t qa = q0 + static_cast<int32_t>(threadIdx.x) * ITEMS;
       // (every window of an interior tile lies inside the read: no bounds tests)
       const bool interior = q0 >= H && q0 + static_cast<int32_t>(kSketchTile) + H <= L;
       uint32_t fl = 0;
       if (qa < q1) {
         uint32_t h[N];
-        const uint32_t* src = sh_hash + threadIdx.x * ITEMS;  // slot of position qa - H
+        const uint32_t* src = sh_hash_all[g] + threadIdx.x * ITEMS;  // slot of position qa - H
 #pragma unroll
         for (int j = 0; j < N; ++j) h[j] = src[j];
         // minimum of the window starting at slot j (positions qa - H + j .. + W - 1),
@@ -473,14 +553,14 @@ SketchFastKernel(const uint64_t* __restrict__ words, const uint64_t* __restrict_
         }
       }
       flags[g] = fl;
-      uint32_t total;
-      ex[g] = BlockExclusiveSum<uint32_t, kSketchThreads>(__popc(fl), sh_scan, &total);
-      tot[g] = total;
+      packed |= static_cast<uint64_t>(__popc(fl)) << (16 * g);
     }
   }
+  uint64_t totals;
+  const uint64_t ex_packed = BlockExclusiveSum<uint64_t, kSketchThreads>(packed, sh_scan, &totals);
   uint32_t group_total = 0;
 #pragma unroll
-  for (int g = 0; g < G; ++g) group_total += tot[g];
+  for (int g = 0; g < G; ++g) group_total += static_cast<uint32_t>(totals >> (16 * g)) & 0xFFFFu;
 
   // ---- output offset of the group: decoupled look-back by the first warp ----
   if (threadIdx.x < 32) {
@@ -517,32 +597,50 @@ SketchFastKernel(const uint64_t* __restrict__ words, const uint64_t* __restrict_
       uint64_t run = excl;
       for (int g = 0; g < g_count; ++g) {
         tile_out[t_first + g] = run;
-        run += tot[g];
+        run += static_cast<uint32_t>(totals >> (16 * g)) & 0xFFFFu;
       }
       if (t_first + g_count == n_tiles) tile_out[n_tiles] = run;
       sh_excl = excl;
     }
   }
   __syncthreads();
+
+  // ---- write-out, tile by tile: compact in shared memory, then store coalesced ----
   uint64_t base = sh_excl;
 #pragma unroll
   for (int g = 0; g < G; ++g) {
     if (g < g_count) {
-      uint64_t dst = base + ex[g];
-      const uint64_t id = static_cast<uint64_t>(ids[rd[g]]) << 32;
-      const uint32_t* own = sh_hash_all[g] + H + threadIdx.x * ITEMS;
+      const uint32_t n = static_cast<uint32_t>(totals >> (16 * g)) & 0xFFFFu;
+      uint32_t* sh_val = sh_hash_all[g];
+      // the value of record e moves to slot e <= its own slot: every thread reads its
+      // values before any is overwritten (the barrier also ends the previous tile's
+      // stores, which read sh_org)
+      uint32_t v[ITEMS];
+      const uint32_t* own = sh_val + H + threadIdx.x * ITEMS;
+#pragma unroll
+      for (int i = 0; i < ITEMS; ++i) v[i] = own[i];
+      __syncthreads();
+      uint32_t e = static_cast<uint32_t>(ex_packed >> (16 * g)) & 0xFFFFu;
 #pragma unroll
       for (int i = 0; i < ITEMS; ++i) {
         if ((flags[g] >> i) & 1u) {
-          if (dst < out_cap) {
-            out_val[dst] = own[i];
-            out_org[dst] = id | (static_cast<uint64_t>(static_cast<uint32_t>(qa_of[g] + i)) << 1) |
-                           ((strands[g] >> i) & 1u);
-          }
-          ++dst;
+          sh_val[e] = v[i];
+          sh_org[e] =
+              static_cast<uint16_t>((threadIdx.x * ITEMS + i) << 1 | ((strands[g] >> i) & 1u));
+          ++e;
         }
       }
-      base += tot[g];
+      __syncthreads();
+      // past out_cap the pass only counts (the host repeats it with the exact size)
+      const uint64_t room = base < out_cap ? out_cap - base : 0;
+      const uint32_t n_out = static_cast<uint32_t>(min(static_cast<uint64_t>(n), room));
+      if (n_out > 0) {
+        // origin = id << 32 | q << 1 | strand = (id << 32 | q0 << 1) + staged origin
+        const uint64_t org_base = (static_cast<uint64_t>(sh_id[g]) << 32) |
+                                  (static_cast<uint64_t>(static_cast<uint32_t>(sh_q0[g])) << 1);
+        StoreTileRecords(sh_val, sh_org, n_out, org_base, out_val + base, out_org + base);
+      }
+      base += n;
     }
   }
 }
@@ -560,23 +658,113 @@ __global__ void GatherReadOffsets(const uint64_t* __restrict__ tile_off,
 // ---- micromizers: the len/k smallest values of a read's sketch, ties by
 // position, back in position order ("minhash", SURVEY.md App. A.2) ----
 constexpr int kMicroThreads = 256;
+constexpr int kMicroBits = 10;                          // radix digit of the selection
+constexpr uint32_t kMicroBins = 1u << kMicroBits;
+constexpr size_t kMicroStageBytes = 40 << 10;           // largest on-chip copy of a sketch
+
+// The micromizers of one read whose sketch has more than m records, by the CTA.
+// src: the read's values, in shared memory or (a sketch too long for it) in global
+// memory; each is its own inlined copy, so on-chip reads compile to shared loads.
+template <typename ValT, bool kWrite>
+__device__ __forceinline__ void SelectMicromizers(
+    const ValT* __restrict__ src, const uint64_t* __restrict__ org, uint32_t cnt, uint32_t m,
+    uint32_t k, uint64_t ob, ValT* __restrict__ q_val, uint64_t* __restrict__ q_org,
+    uint64_t* __restrict__ thr_val, uint32_t* __restrict__ thr_pos, uint32_t* hist,
+    uint32_t* sh_scan, uint64_t* sh_scan64, uint32_t* sh_pick) {
+  // ---- radix select of the value with ascending rank m-1 ----
+  // (every thread owns 4 consecutive digits of the histogram's scan)
+  static_assert(kMicroBins == 4 * kMicroThreads, "4 digits a thread");
+  uint64_t prefix = 0, prefix_mask = 0;
+  uint32_t want = m - 1;
+  for (int shift = static_cast<int>((2 * k + kMicroBits - 1) / kMicroBits - 1) * kMicroBits;
+       shift >= 0; shift -= kMicroBits) {
+    reinterpret_cast<uint4*>(hist)[threadIdx.x] = make_uint4(0, 0, 0, 0);
+    __syncthreads();  // (the first: the values are on chip)
+    for (uint32_t i = threadIdx.x; i < cnt; i += kMicroThreads) {
+      const uint64_t v = src[i];
+      if ((v & prefix_mask) == prefix) {
+        atomicAdd(&hist[(v >> shift) & (kMicroBins - 1)], 1u);
+      }
+    }
+    __syncthreads();
+    {  // the digit whose cumulative count first exceeds `want`: one block scan
+      const uint4 h = reinterpret_cast<const uint4*>(hist)[threadIdx.x];
+      uint32_t tot;
+      uint32_t run = BlockExclusiveSum<uint32_t, kMicroThreads>(h.x + h.y + h.z + h.w, sh_scan,
+                                                                &tot);
+      const uint32_t hc[4] = {h.x, h.y, h.z, h.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        if (run <= want && want < run + hc[j]) {
+          sh_pick[0] = 4 * threadIdx.x + j;
+          sh_pick[1] = want - run;
+        }
+        run += hc[j];
+      }
+    }
+    __syncthreads();
+    prefix |= static_cast<uint64_t>(sh_pick[0]) << shift;
+    prefix_mask |= static_cast<uint64_t>(kMicroBins - 1) << shift;
+    want = sh_pick[1];
+  }
+  const uint64_t T = prefix;
+  const uint32_t need_eq = want + 1;  // first need_eq records equal to T
+
+  // ---- ordered compaction: every thread walks its own run of records ----
+  // (an odd run length keeps the shared-memory reads of a warp free of conflicts)
+  const uint32_t run_len = ((cnt + kMicroThreads - 1) / kMicroThreads) | 1u;
+  const uint32_t lo = min(threadIdx.x * run_len, cnt), hi = min(lo + run_len, cnt);
+  uint32_t n_eq = 0, n_lt = 0;
+  for (uint32_t i = lo; i < hi; ++i) {
+    const uint64_t v = src[i];
+    n_eq += v == T;
+    n_lt += v < T;
+  }
+  uint64_t tot;
+  const uint64_t before = BlockExclusiveSum<uint64_t, kMicroThreads>(
+      static_cast<uint64_t>(n_eq) << 32 | n_lt, sh_scan64, &tot);
+  uint32_t eq_run = static_cast<uint32_t>(before >> 32);
+  uint32_t lt_run = static_cast<uint32_t>(before);
+  // (thresholds only: just the thread that holds the last kept tie walks again)
+  if (kWrite || (eq_run < need_eq && need_eq <= eq_run + n_eq)) {
+    for (uint32_t i = lo; i < hi; ++i) {
+      const uint64_t v = src[i];
+      const bool is_eq = v == T, is_lt = v < T;
+      if (kWrite && (is_lt || (is_eq && eq_run < need_eq))) {
+        const uint64_t d = ob + lt_run + min(eq_run, need_eq);
+        q_val[d] = static_cast<ValT>(v);
+        q_org[d] = org[i];
+      }
+      if (is_eq && eq_run + 1 == need_eq) {  // the last tie that is kept
+        *thr_val = T;
+        *thr_pos = (static_cast<uint32_t>(org[i]) >> 1) + 1;
+      }
+      lt_run += is_lt;
+      eq_run += is_eq;
+    }
+  }
+}
 
 // Besides (kWrite) the micromizers themselves, the selection rule of every read is
 // left behind as a pair (thr_val, thr_pos): record (value, position) of the read is
 // one of its micromizers iff value < thr_val || (value == thr_val && position <
 // thr_pos) - what the stage-1 self-join over the index asks of every posting.
+// A read's values are copied to shared memory once (dynamic, stage_cap of them) and
+// selected there; a sketch longer than that is selected from global memory.
 template <typename ValT, bool kWrite>
 __global__ void __launch_bounds__(kMicroThreads)
 MicromizeKernel(const ValT* __restrict__ s_val,
                 const uint64_t* __restrict__ s_org,
                 const uint64_t* __restrict__ s_off,  // per read of the sketch
                 uint32_t s_first, const uint64_t* __restrict__ q_off,
-                uint32_t q_first, uint32_t k,
+                uint32_t q_first, uint32_t k, uint32_t stage_cap,
                 ValT* __restrict__ q_val, uint64_t* __restrict__ q_org,
                 uint64_t* __restrict__ thr_val, uint32_t* __restrict__ thr_pos) {
-  __shared__ uint32_t hist[256];
+  extern __shared__ __align__(16) unsigned char micro_smem[];
+  __shared__ __align__(16) uint32_t hist[kMicroBins];
   __shared__ uint32_t sh_scan[34];
-  __shared__ uint32_t sh_digit, sh_want;
+  __shared__ uint64_t sh_scan64[34];
+  __shared__ uint32_t sh_pick[2];  // digit and remaining rank of a radix round
   __shared__ unsigned long long sh_max;
 
   const uint32_t r = q_first + blockIdx.x;
@@ -614,72 +802,34 @@ MicromizeKernel(const ValT* __restrict__ s_val,
     return;
   }
 
-  // radix select of the value with ascending rank m-1
-  uint64_t prefix = 0, prefix_mask = 0;
-  uint32_t want = m - 1;
-  for (int shift = static_cast<int>((2 * k + 7) / 8 - 1) * 8; shift >= 0;
-       shift -= 8) {
-    hist[threadIdx.x] = 0;
-    __syncthreads();
-    for (uint32_t i = threadIdx.x; i < cnt; i += kMicroThreads) {
-      const uint64_t v = val[i];
-      if ((v & prefix_mask) == prefix) {
-        atomicAdd(&hist[(v >> shift) & 255], 1u);
+  if (cnt <= stage_cap) {
+    // the values on chip: 16-byte loads after a head up to the first boundary
+    ValT* sh = reinterpret_cast<ValT*>(micro_smem);
+    constexpr uint32_t V = 16 / sizeof(ValT);
+    const uint32_t head = min(
+        cnt, static_cast<uint32_t>((16 - (reinterpret_cast<uintptr_t>(val) & 15)) & 15) /
+                 static_cast<uint32_t>(sizeof(ValT)));
+    const uint32_t nvec = (cnt - head) / V;
+    const uint4* vp = reinterpret_cast<const uint4*>(val + head);
+    for (uint32_t i = threadIdx.x; i < nvec; i += kMicroThreads) {
+      const uint4 x = __ldg(vp + i);
+      if (sizeof(ValT) == 4) {
+        sh[head + 4 * i] = x.x;
+        sh[head + 4 * i + 1] = x.y;
+        sh[head + 4 * i + 2] = x.z;
+        sh[head + 4 * i + 3] = x.w;
+      } else {
+        sh[head + 2 * i] = static_cast<ValT>(static_cast<uint64_t>(x.y) << 32 | x.x);
+        sh[head + 2 * i + 1] = static_cast<ValT>(static_cast<uint64_t>(x.w) << 32 | x.z);
       }
     }
-    __syncthreads();
-    {  // the digit whose cumulative count first exceeds `want`: one block scan
-      static_assert(kMicroThreads == 256, "one thread per digit");
-      const uint32_t h = hist[threadIdx.x];
-      uint32_t tot;
-      const uint32_t ex = BlockExclusiveSum<uint32_t, kMicroThreads>(h, sh_scan, &tot);
-      if (ex <= want && want < ex + h) {
-        sh_digit = threadIdx.x;
-        sh_want = want - ex;
-      }
-    }
-    __syncthreads();
-    prefix |= static_cast<uint64_t>(sh_digit) << shift;
-    prefix_mask |= 255ULL << shift;
-    want = sh_want;
-    __syncthreads();
-  }
-  const uint64_t T = prefix;
-  const uint32_t need_eq = want + 1;  // first need_eq records equal to T
-
-  // ordered compaction, one chunk of kMicroThreads records at a time
-  uint32_t kept = 0, eq_seen = 0;
-  for (uint32_t base = 0; base < cnt; base += kMicroThreads) {
-    const uint32_t i = base + threadIdx.x;
-    uint64_t v = 0, o = 0;
-    uint32_t is_eq = 0, is_lt = 0;
-    if (i < cnt) {
-      v = val[i];
-      o = org[i];
-      is_eq = v == T;
-      is_lt = v < T;
-    }
-    uint32_t tot;
-    const uint32_t packed = BlockExclusiveSum<uint32_t, kMicroThreads>(
-        is_eq << 16 | is_lt, sh_scan, &tot);
-    const uint32_t eq_before = eq_seen + (packed >> 16);
-    const uint32_t lt_before = packed & 0xFFFF;
-    const uint32_t eq_kept_before =
-        min(eq_before, need_eq) - min(eq_seen, need_eq);
-    const bool keep = is_lt || (is_eq && eq_before < need_eq);
-    if (kWrite && keep) {
-      const uint64_t d = ob + kept + lt_before + eq_kept_before;
-      q_val[d] = static_cast<ValT>(v);
-      q_org[d] = o;
-    }
-    if (is_eq && eq_before + 1 == need_eq) {  // the last tie that is kept
-      thr_val[blockIdx.x] = T;
-      thr_pos[blockIdx.x] = (static_cast<uint32_t>(o) >> 1) + 1;
-    }
-    if (!kWrite && eq_seen + (tot >> 16) >= need_eq) break;  // (uniform) nothing left to learn
-    const uint32_t eq_tot = tot >> 16, lt_tot = tot & 0xFFFF;
-    kept += lt_tot + (min(eq_seen + eq_tot, need_eq) - min(eq_seen, need_eq));
-    eq_seen += eq_tot;
+    if (threadIdx.x < head) sh[threadIdx.x] = val[threadIdx.x];
+    for (uint32_t i = head + V * nvec + threadIdx.x; i < cnt; i += kMicroThreads) sh[i] = val[i];
+    SelectMicromizers<ValT, kWrite>(sh, org, cnt, m, k, ob, q_val, q_org, thr_val + blockIdx.x,
+                                    thr_pos + blockIdx.x, hist, sh_scan, sh_scan64, sh_pick);
+  } else {
+    SelectMicromizers<ValT, kWrite>(val, org, cnt, m, k, ob, q_val, q_org, thr_val + blockIdx.x,
+                                    thr_pos + blockIdx.x, hist, sh_scan, sh_scan64, sh_pick);
   }
 }
 
@@ -854,6 +1004,18 @@ void Micromize(Ctx& c, uint32_t first, uint32_t last, bool write) {
     c.h_q_off[i + 1] = c.h_q_off[i] + (m < cnt ? m : cnt);
   }
   const uint64_t total = c.h_q_off[nr];
+  // shared memory for the longest sketch that is selected (len/k < its length), up to
+  // kMicroStageBytes; longer ones are selected from global memory
+  const size_t val_bytes = c.s_is32 ? 4 : 8;
+  uint64_t longest = 0;
+  for (uint32_t i = 0; i < nr; ++i) {
+    const uint32_t r = first + i;
+    const uint64_t cnt = c.h_s_off[r - c.s_first + 1] - c.h_s_off[r - c.s_first];
+    if (c.h_q_off[i + 1] - c.h_q_off[i] < cnt) longest = std::max(longest, cnt);
+  }
+  const uint32_t stage_cap =
+      static_cast<uint32_t>(std::min<uint64_t>(longest, kMicroStageBytes / val_bytes));
+  const size_t smem = stage_cap * val_bytes;
   uint64_t* qoff = c.q_off.reserve(nr + 1ULL);
   RVN_CUDA(cudaMemcpyAsync(qoff, c.h_q_off.data(),
                            (nr + 1ULL) * sizeof(uint64_t),
@@ -870,20 +1032,22 @@ void Micromize(Ctx& c, uint32_t first, uint32_t last, bool write) {
       auto* sv = reinterpret_cast<const uint32_t*>(c.s_val.get());
       auto* q32 = reinterpret_cast<uint32_t*>(qv);
       if (write) {
-        MicromizeKernel<uint32_t, true><<<nr, kMicroThreads, 0, c.stream>>>(
-            sv, c.s_org.get(), c.s_off.get(), c.s_first, qoff, first, c.prm.k, q32, qo, tv, tp);
+        MicromizeKernel<uint32_t, true><<<nr, kMicroThreads, smem, c.stream>>>(
+            sv, c.s_org.get(), c.s_off.get(), c.s_first, qoff, first, c.prm.k, stage_cap, q32, qo,
+            tv, tp);
       } else {
-        MicromizeKernel<uint32_t, false><<<nr, kMicroThreads, 0, c.stream>>>(
-            sv, c.s_org.get(), c.s_off.get(), c.s_first, qoff, first, c.prm.k, q32, qo, tv, tp);
+        MicromizeKernel<uint32_t, false><<<nr, kMicroThreads, smem, c.stream>>>(
+            sv, c.s_org.get(), c.s_off.get(), c.s_first, qoff, first, c.prm.k, stage_cap, q32, qo,
+            tv, tp);
       }
     } else if (write) {
-      MicromizeKernel<uint64_t, true><<<nr, kMicroThreads, 0, c.stream>>>(
-          c.s_val.get(), c.s_org.get(), c.s_off.get(), c.s_first, qoff, first, c.prm.k, qv, qo,
-          tv, tp);
+      MicromizeKernel<uint64_t, true><<<nr, kMicroThreads, smem, c.stream>>>(
+          c.s_val.get(), c.s_org.get(), c.s_off.get(), c.s_first, qoff, first, c.prm.k, stage_cap,
+          qv, qo, tv, tp);
     } else {
-      MicromizeKernel<uint64_t, false><<<nr, kMicroThreads, 0, c.stream>>>(
-          c.s_val.get(), c.s_org.get(), c.s_off.get(), c.s_first, qoff, first, c.prm.k, qv, qo,
-          tv, tp);
+      MicromizeKernel<uint64_t, false><<<nr, kMicroThreads, smem, c.stream>>>(
+          c.s_val.get(), c.s_org.get(), c.s_off.get(), c.s_first, qoff, first, c.prm.k, stage_cap,
+          qv, qo, tv, tp);
     }
     RVN_LAUNCH_CHECK();
     ++c.launches;
