@@ -8,21 +8,17 @@
 //           (first posting, count) or "filtered" if count > occurrence
 //   expand  hits (ram "Match": group = (rhs_id<<1|same_strand)<<32|diagonal,
 //           positions = lhs_pos<<32|rhs_pos) written per query read
-//   chain   ONE CTA PER QUERY READ, hits resident in shared memory:
-//           bitonic sort by (group, positions) -> diagonal-band intervals by
-//           binary searches + block scans -> second sort by (band, positions)
-//           -> one thread per band runs ram's patience/LIS with its exact
-//           binary-search predicate, gap split and covered-bases test ->
-//           overlaps written through a reserved slab, then re-ordered by
-//           query id so that the output order equals the reference's.
-//   Reads whose hits do not fit in shared memory take the same code path
-//   over a global-memory scratch slab.
+//   chain   each read's hits split by (rhs_id, strand) pair, each pair chained
+//           on chip by one thread or one CTA by its size, large reads whole by a
+//           CTA over global memory; ram's per-band rules are chain.cuh's. The
+//           overlaps are re-ordered into the reference's output order.
 //
 // The chain result is a pure function of the MULTISET of hits of a query
 // (both reference sorts are total orders here: equal (group, positions)
 // pairs cannot occur), so hit generation order is free (DESIGN.md).
 #include <algorithm>
 
+#include "chain.cuh"
 #include "engine.cuh"
 #include "seed.cuh"
 
@@ -348,31 +344,34 @@ __global__ void ScatterFiltered(const uint8_t* __restrict__ filt,
 // chaining
 // ---------------------------------------------------------------------------
 
-struct ChainParams {
-  uint32_t k, bandwidth, chain, matches, gap;
-};
-
-// sorts (A[i], B[i]) pairs ascending by (A, B); npad is a power of two
-template <int THREADS>
-__device__ void BitonicSortPairs(uint64_t* A, uint64_t* B, uint32_t npad) {
+// Bitonic sorting network of the CTA over npad slots (a power of two), ascending:
+// exchange(i, j, up) orders slots i < j, the smaller into i when `up`, else into j.
+template <int THREADS, typename Exchange>
+__device__ __forceinline__ void BitonicSort(uint32_t npad, Exchange exchange) {
   for (uint32_t size = 2; size <= npad; size <<= 1) {
     for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
       for (uint32_t t = threadIdx.x; t < (npad >> 1); t += THREADS) {
         const uint32_t i = 2 * t - (t & (stride - 1));
-        const uint32_t j = i + stride;
-        const bool up = (i & size) == 0;
-        const uint64_t ai = A[i], aj = A[j], bi = B[i], bj = B[j];
-        const bool gt = ai > aj || (ai == aj && bi > bj);
-        if (gt == up) {
-          A[i] = aj;
-          A[j] = ai;
-          B[i] = bj;
-          B[j] = bi;
-        }
+        exchange(i, i + stride, (i & size) == 0);
       }
       __syncthreads();
     }
   }
+}
+
+// sorts (A[i], B[i]) pairs ascending by (A, B); npad is a power of two
+template <int THREADS>
+__device__ void BitonicSortPairs(uint64_t* A, uint64_t* B, uint32_t npad) {
+  BitonicSort<THREADS>(npad, [=](uint32_t i, uint32_t j, bool up) {
+    const uint64_t ai = A[i], aj = A[j], bi = B[i], bj = B[j];
+    const bool gt = ai > aj || (ai == aj && bi > bj);
+    if (gt == up) {
+      A[i] = aj;
+      A[j] = ai;
+      B[i] = bj;
+      B[j] = bi;
+    }
+  });
 }
 
 // Everything a CTA needs to chain the hits of one query read. IdxT = u16 for
@@ -386,6 +385,26 @@ struct ChainWork {
   IdxT* IB;      // n/4+1  band begin
   IdxT* IE;      // n/4+1  band end
   uint32_t* CNT; // n/4+1  overlaps per band
+  // the index arrays for n hits from idx on, CNT at the next 4-byte boundary
+  __device__ __forceinline__ void PlaceIndices(IdxT* idx, uint32_t n) {
+    const uint32_t nb = n / 4 + 1;
+    LB = idx;
+    PD = LB + (n + nb + 2);
+    IB = PD + (n + 1);
+    IE = IB + nb;
+    CNT = reinterpret_cast<uint32_t*>((reinterpret_cast<uintptr_t>(IE + nb) + 3) & ~uintptr_t(3));
+  }
+};
+
+// BandLis storage of ChainRead: tail(n) at minimal[n], then the chain from minimal[0] on
+template <typename IdxT>
+struct ArrayLis {
+  IdxT *minimal, *predecessor;
+  __device__ uint32_t tail(uint32_t n) const { return minimal[n]; }
+  __device__ void set_tail(uint32_t n, uint32_t v) const { minimal[n] = static_cast<IdxT>(v); }
+  __device__ void set_chain(uint32_t x, uint32_t v) const { minimal[x] = static_cast<IdxT>(v); }
+  __device__ uint32_t pred(uint32_t x) const { return predecessor[x]; }
+  __device__ void set_pred(uint32_t x, uint32_t v) const { predecessor[x] = static_cast<IdxT>(v); }
 };
 
 template <typename IdxT, int THREADS>
@@ -504,89 +523,20 @@ __device__ uint32_t ChainRead(const ChainWork<IdxT>& wk, uint32_t n,
   __syncthreads();
   BitonicSortPairs<THREADS>(G, P, npad);
 
-  // 5. one thread per band: LIS + gap split + covered bases
+  // 5. one thread per band: ram's chain rules (chain.cuh), counting the overlaps
   IdxT* MINI = wk.LB;  // re-used: per band (len + 1) entries at IB[b] + b
   for (uint32_t b = threadIdx.x; b < nb; b += THREADS) {
-    const uint32_t jb = wk.IB[b], ie = wk.IE[b];
-    const uint32_t len = ie - jb;
+    const uint32_t jb = wk.IB[b];
+    const uint64_t* Pb = P + jb;
+    const ArrayLis<IdxT> lis{MINI + jb + b, wk.PD + jb};
+    const bool strand = G[jb] & 1;
+    const uint32_t longest =
+        BandLis(wk.IE[b] - jb, strand, cp.chain, [&](uint32_t t) { return Pb[t]; }, lis);
     uint32_t emitted = 0;
-    uint32_t longest = 0;
-    if (len >= cp.chain) {
-      const uint64_t* Pb = P + jb;
-      IdxT* minimal = MINI + jb + b;
-      IdxT* pred = wk.PD + jb;
-      const bool strand = G[jb] & 1;
-      minimal[0] = 0;
-      for (uint32_t t = 0; t < len; ++t) {
-        const uint32_t cl = static_cast<uint32_t>(Pb[t] >> 32);
-        const uint32_t cr = static_cast<uint32_t>(Pb[t]);
-        uint32_t lo = 1, hi = longest;
-        while (lo <= hi) {
-          const uint32_t mid = lo + (hi - lo) / 2;
-          const uint64_t tail = Pb[minimal[mid]];
-          const uint32_t tl = static_cast<uint32_t>(tail >> 32);
-          const uint32_t tr = static_cast<uint32_t>(tail);
-          if (tl < cl && (strand ? tr < cr : tr > cr)) {
-            lo = mid + 1;
-          } else {
-            hi = mid - 1;
-          }
-        }
-        pred[t] = minimal[lo - 1];
-        minimal[lo] = static_cast<IdxT>(t);
-        longest = max(longest, lo);
-      }
-      if (longest >= cp.chain) {
-        // unroll the chain into minimal[0 .. longest)
-        uint32_t j = minimal[longest];
-        for (uint32_t i = 0; i < longest; ++i) {
-          const uint32_t pj = pred[j];
-          minimal[longest - 1 - i] = static_cast<IdxT>(j);
-          j = pj;
-        }
-      } else {
-        longest = 0;
-      }
-    }
-    // count the overlaps this band emits (walk repeated when writing)
-    if (longest) {
-      const uint64_t* Pb = P + jb;
-      const IdxT* idx = MINI + jb + b;
-      const bool strand = G[jb] & 1;
-      for (uint32_t kk = 1, l = 0; kk <= longest; ++kk) {
-        const uint32_t prev = static_cast<uint32_t>(Pb[idx[kk - 1]] >> 32);
-        const uint32_t cur =
-            kk < longest ? static_cast<uint32_t>(Pb[idx[kk]] >> 32) : 0xFFFFFFFFu;
-        if (cur - prev > cp.gap) {
-          if (kk - l >= cp.chain) {
-            uint32_t lm = 0, lb_ = 0, le = 0, rm = 0, rb_ = 0, re = 0;
-            for (uint32_t m = l; m < kk; ++m) {
-              const uint64_t pp = Pb[idx[m]];
-              const uint32_t lp = static_cast<uint32_t>(pp >> 32);
-              if (lp > le) {
-                lm += le - lb_;
-                lb_ = lp;
-              }
-              le = lp + cp.k;
-              uint32_t rp = static_cast<uint32_t>(pp);
-              rp = strand ? rp : (1U << 31) - (rp + cp.k - 1);
-              if (rp > re) {
-                rm += re - rb_;
-                rb_ = rp;
-              }
-              re = rp + cp.k;
-            }
-            lm += le - lb_;
-            rm += re - rb_;
-            if (min(lm, rm) >= cp.matches) ++emitted;
-          }
-          l = kk;
-        }
-      }
-    }
+    ForEachChainOverlap(longest, strand, cp, [&](uint32_t x) { return Pb[lis.minimal[x]]; },
+                        [&](uint64_t, uint64_t, uint32_t) { ++emitted; });
     wk.CNT[b] = emitted;
-    // stash the chain length where the writer finds it
-    wk.IE[b] = static_cast<IdxT>(longest);
+    wk.IE[b] = static_cast<IdxT>(longest);  // the chain length, for the writer
   }
   __syncthreads();
 
@@ -622,56 +572,16 @@ __device__ uint32_t ChainRead(const ChainWork<IdxT>& wk, uint32_t n,
       uint64_t* kdst = ovl_key ? ovl_key + base + carry + ex : nullptr;
       uint32_t seq = carry + ex;
       const uint32_t jb = wk.IB[b];
-      const uint32_t longest = wk.IE[b];
       const uint64_t* Pb = P + jb;
-      const IdxT* idx = MINI + jb + b;
+      const IdxT* chain = MINI + jb + b;
       const bool strand = G[jb] & 1;
       const uint32_t rhs_id = static_cast<uint32_t>(G[jb] & 0xFFFFFFFFu) >> 1;
-      for (uint32_t kk = 1, l = 0; kk <= longest; ++kk) {
-        const uint32_t prev = static_cast<uint32_t>(Pb[idx[kk - 1]] >> 32);
-        const uint32_t cur =
-            kk < longest ? static_cast<uint32_t>(Pb[idx[kk]] >> 32) : 0xFFFFFFFFu;
-        if (cur - prev > cp.gap) {
-          if (kk - l >= cp.chain) {
-            uint32_t lm = 0, lb_ = 0, le = 0, rm = 0, rb_ = 0, re = 0;
-            for (uint32_t m = l; m < kk; ++m) {
-              const uint64_t pp = Pb[idx[m]];
-              const uint32_t lp = static_cast<uint32_t>(pp >> 32);
-              if (lp > le) {
-                lm += le - lb_;
-                lb_ = lp;
-              }
-              le = lp + cp.k;
-              uint32_t rp = static_cast<uint32_t>(pp);
-              rp = strand ? rp : (1U << 31) - (rp + cp.k - 1);
-              if (rp > re) {
-                rm += re - rb_;
-                rb_ = rp;
-              }
-              re = rp + cp.k;
-            }
-            lm += le - lb_;
-            rm += re - rb_;
-            if (min(lm, rm) >= cp.matches) {
-              const uint64_t pf = Pb[idx[l]], pl = Pb[idx[kk - 1]];
-              rvn_overlap o;
-              o.lhs_id = lhs_id;
-              o.lhs_begin = static_cast<uint32_t>(pf >> 32);
-              o.lhs_end = cp.k + static_cast<uint32_t>(pl >> 32);
-              o.rhs_id = rhs_id;
-              o.rhs_begin = strand ? static_cast<uint32_t>(pf)
-                                   : static_cast<uint32_t>(pl);
-              o.rhs_end = cp.k + (strand ? static_cast<uint32_t>(pl)
-                                         : static_cast<uint32_t>(pf));
-              o.score = min(lm, rm);
-              o.strand = strand;
-              *dst++ = o;
-              if (kdst) *kdst++ = key_hi | seq++;
-            }
-          }
-          l = kk;
-        }
-      }
+      ForEachChainOverlap(wk.IE[b], strand, cp, [&](uint32_t x) { return Pb[chain[x]]; },
+                          [&](uint64_t first, uint64_t last, uint32_t score) {
+                            *dst++ = MakeOverlap(lhs_id, rhs_id, strand, cp.k, first, last,
+                                                 score);
+                            if (kdst) *kdst++ = key_hi | seq++;
+                          });
     }
     carry += tot;
   }
@@ -697,12 +607,9 @@ constexpr uint32_t kThreadPairMax = 48;   // larger (rhs, strand) pairs get a CT
 //               emission order).
 //  GroupChainKernel  ONE THREAD PER PAIR over all pairs of all reads, largest
 //               pairs first (size-sorted, so the lanes of a warp carry similar
-//               work and nothing waits at a barrier): (diagonal, positions)
-//               order by binary insertion, the reference's window loop, per
-//               band the position order, ram's patience/LIS recurrence with
-//               its exact probe sequence, gap split, covered bases. Overlaps go
-//               to a global list keyed (pair index, sequence number) and are
-//               put back in emission order by a radix sort of the keys.
+//               work and nothing waits at a barrier): ChainPairSerial (chain.cuh).
+//               Overlaps go to a global list keyed (pair index, sequence number)
+//               and are put back in emission order by a radix sort of the keys.
 // ---------------------------------------------------------------------------
 struct GroupDesc {
   uint32_t hit_off, cnt, gid, lhs_id;
@@ -837,20 +744,13 @@ SplitKernel(const uint64_t* __restrict__ h_grp, const uint64_t* __restrict__ h_p
     sh_hbase = atomicAdd(&totals[1], static_cast<unsigned long long>(nh));
   }
   __syncthreads();
-  for (uint32_t size = 2; size <= gpad; size <<= 1) {
-    for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
-      for (uint32_t t = threadIdx.x; t < (gpad >> 1); t += THREADS) {
-        const uint32_t i = 2 * t - (t & (stride - 1));
-        const uint32_t j = i + stride;
-        const uint64_t a = GL[i], c2 = GL[j];
-        if ((a > c2) == ((i & size) == 0)) {
-          GL[i] = c2;
-          GL[j] = a;
-        }
-      }
-      __syncthreads();
+  BitonicSort<THREADS>(gpad, [=](uint32_t i, uint32_t j, bool up) {
+    const uint64_t a = GL[i], c2 = GL[j];
+    if ((a > c2) == up) {
+      GL[i] = c2;
+      GL[j] = a;
     }
-  }
+  });
   const uint64_t gbase = sh_gbase, hbase = sh_hbase;
   const uint32_t lhs_id = lhs_ids[r];
   for (uint32_t q = threadIdx.x; q < ng; q += THREADS) {
@@ -883,135 +783,11 @@ SplitKernel(const uint64_t* __restrict__ h_grp, const uint64_t* __restrict__ h_p
   }
 }
 
-// A pair's hits live in shared memory, interleaved across the CTA's threads
-// (element i of thread t at [i * T + t]): every thread walks its own column,
-// same-index accesses of a warp are conflict-free, and no barrier is needed.
-struct Column {
-  uint64_t* P;  // positions column (already offset by the thread index)
-  uint32_t* D;  // diagonal column; per band re-used as (minimal, predecessor) u16 pairs
-  uint32_t T;   // column stride = threads per CTA
-  __device__ __forceinline__ uint64_t& p(uint32_t i) const { return P[i * T]; }
-  __device__ __forceinline__ uint32_t& d(uint32_t i) const { return D[i * T]; }
-};
-
-// one band [jb, ie) of a pair: position order, LIS, gap split, emit
-__device__ __forceinline__ void BandChain(const Column& c, uint32_t jb, uint32_t ie,
-                                          bool strand, uint32_t lhs_id,
-                                          uint32_t rhs_id, const ChainParams& cp,
-                                          uint64_t key_hi, uint32_t* seq,
-                                          rvn_overlap* __restrict__ out,
-                                          uint64_t* __restrict__ out_key,
-                                          unsigned long long* __restrict__ out_cnt,
-                                          uint64_t out_cap) {
-  const uint32_t len = ie - jb;
-  if (len < cp.chain) return;
-  for (uint32_t a = 1; a < len; ++a) {  // binary insertion sort by positions
-    const uint64_t pv = c.p(jb + a);
-    if (c.p(jb + a - 1) <= pv) continue;
-    uint32_t lo = 0, hi = a - 1;  // first element > pv lies in [lo, hi]
-    while (lo < hi) {
-      const uint32_t mid = (lo + hi) >> 1;
-      if (c.p(jb + mid) > pv) {
-        hi = mid;
-      } else {
-        lo = mid + 1;
-      }
-    }
-    for (uint32_t b = a; b > lo; --b) c.p(jb + b) = c.p(jb + b - 1);
-    c.p(jb + lo) = pv;
-  }
-  // the band's diagonals are dead: word x of the band now holds
-  // minimal[x + 1] (low half) and predecessor[x] (high half); minimal[0] = 0
-  auto mini_get = [&](uint32_t x) -> uint32_t { return c.d(jb + x) & 0xFFFFu; };
-  auto mini_set = [&](uint32_t x, uint32_t v) {
-    c.d(jb + x) = (c.d(jb + x) & 0xFFFF0000u) | v;
-  };
-  auto pred_get = [&](uint32_t x) -> uint32_t { return c.d(jb + x) >> 16; };
-  auto pred_set = [&](uint32_t x, uint32_t v) {
-    c.d(jb + x) = (c.d(jb + x) & 0xFFFFu) | (v << 16);
-  };
-  uint32_t longest = 0;
-  for (uint32_t t = 0; t < len; ++t) {
-    const uint64_t cur = c.p(jb + t);
-    const uint32_t cl = static_cast<uint32_t>(cur >> 32);
-    const uint32_t cr = static_cast<uint32_t>(cur);
-    uint32_t lo = 1, hi = longest;
-    while (lo <= hi) {
-      const uint32_t mid = lo + (hi - lo) / 2;
-      const uint64_t tail = c.p(jb + mini_get(mid - 1));
-      const uint32_t tl = static_cast<uint32_t>(tail >> 32);
-      const uint32_t tr = static_cast<uint32_t>(tail);
-      if (tl < cl && (strand ? tr < cr : tr > cr)) {
-        lo = mid + 1;
-      } else {
-        hi = mid - 1;
-      }
-    }
-    pred_set(t, lo > 1 ? mini_get(lo - 2) : 0u);
-    mini_set(lo - 1, t);
-    longest = max(longest, lo);
-  }
-  if (longest < cp.chain) return;
-  {
-    uint32_t j = mini_get(longest - 1);
-    for (uint32_t i = 0; i < longest; ++i) {
-      const uint32_t pj = pred_get(j);
-      mini_set(longest - 1 - i, j);
-      j = pj;
-    }
-  }
-  for (uint32_t kk = 1, l = 0; kk <= longest; ++kk) {
-    const uint32_t prev = static_cast<uint32_t>(c.p(jb + mini_get(kk - 1)) >> 32);
-    const uint32_t cur = kk < longest
-                             ? static_cast<uint32_t>(c.p(jb + mini_get(kk)) >> 32)
-                             : 0xFFFFFFFFu;
-    if (cur - prev > cp.gap) {
-      if (kk - l >= cp.chain) {
-        uint32_t lm = 0, lb_ = 0, le = 0, rm = 0, rb_ = 0, re = 0;
-        for (uint32_t m = l; m < kk; ++m) {
-          const uint64_t pp = c.p(jb + mini_get(m));
-          const uint32_t lp = static_cast<uint32_t>(pp >> 32);
-          if (lp > le) {
-            lm += le - lb_;
-            lb_ = lp;
-          }
-          le = lp + cp.k;
-          uint32_t rp = static_cast<uint32_t>(pp);
-          rp = strand ? rp : (1U << 31) - (rp + cp.k - 1);
-          if (rp > re) {
-            rm += re - rb_;
-            rb_ = rp;
-          }
-          re = rp + cp.k;
-        }
-        lm += le - lb_;
-        rm += re - rb_;
-        if (min(lm, rm) >= cp.matches) {
-          const uint64_t pf = c.p(jb + mini_get(l)), pl = c.p(jb + mini_get(kk - 1));
-          rvn_overlap o;
-          o.lhs_id = lhs_id;
-          o.lhs_begin = static_cast<uint32_t>(pf >> 32);
-          o.lhs_end = cp.k + static_cast<uint32_t>(pl >> 32);
-          o.rhs_id = rhs_id;
-          o.rhs_begin = strand ? static_cast<uint32_t>(pf) : static_cast<uint32_t>(pl);
-          o.rhs_end = cp.k + (strand ? static_cast<uint32_t>(pl)
-                                     : static_cast<uint32_t>(pf));
-          o.score = min(lm, rm);
-          o.strand = strand;
-          const unsigned long long slot = atomicAdd(out_cnt, 1ULL);
-          if (slot < out_cap) {
-            out[slot] = o;
-            out_key[slot] = key_hi | (*seq)++;
-          }
-        }
-      }
-      l = kk;
-    }
-  }
-}
-
-// thread t of the launch handles pair order[first + t]; every pair of this
-// launch has at most m_cap hits (the launch is one size class)
+// thread t of the launch handles pair order[first + t]; every pair of this launch has at
+// most m_cap hits (the launch is one size class). A pair's hits live in shared memory,
+// interleaved across the CTA's threads (element i of thread t at [i * T + t]): every
+// thread walks its own column, same-index accesses of a warp are conflict-free, and no
+// barrier is needed.
 __global__ void GroupChainKernel(const GroupDesc* __restrict__ desc,
                                  const uint32_t* __restrict__ order, uint64_t first,
                                  uint64_t last, uint32_t m_cap,
@@ -1031,61 +807,19 @@ __global__ void GroupChainKernel(const GroupDesc* __restrict__ desc,
   c.T = T;
   const uint32_t g = order[t];
   const GroupDesc d = desc[g];
-  const uint32_t m = d.cnt;
-  for (uint32_t i = 0; i < m; ++i) {
+  for (uint32_t i = 0; i < d.cnt; ++i) {
     c.p(i) = g_pos[d.hit_off + i];
     c.d(i) = g_diag[d.hit_off + i];
   }
-  for (uint32_t a = 1; a < m; ++a) {  // binary insertion by (diagonal, positions)
-    const uint32_t dv = c.d(a);
-    const uint64_t pv = c.p(a);
-    uint32_t lo = 0, hi = a;  // first element > (dv, pv) lies in [lo, hi]
-    while (lo < hi) {
-      const uint32_t mid = (lo + hi) >> 1;
-      const uint32_t dm = c.d(mid);
-      if (dm > dv || (dm == dv && c.p(mid) > pv)) {
-        hi = mid;
-      } else {
-        lo = mid + 1;
-      }
-    }
-    for (uint32_t b = a; b > lo; --b) {
-      c.d(b) = c.d(b - 1);
-      c.p(b) = c.p(b - 1);
-    }
-    c.d(lo) = dv;
-    c.p(lo) = pv;
-  }
-  // the reference's window loop; index m plays the stop dummy
-  const bool strand = d.gid & 1;
-  const uint32_t rhs_id = d.gid >> 1;
   const uint64_t key_hi = static_cast<uint64_t>(g) << 16;
   uint32_t seq = 0;
-  bool open = false;
-  uint32_t ob = 0, oe = 0;
-  for (uint32_t i = 1, j = 0; i <= m; ++i) {
-    if (i == m || c.d(i) - c.d(j) > cp.bandwidth) {
-      if (i - j >= 4) {
-        if (open && oe > j) {
-          oe = i;
-        } else {
-          if (open) {
-            BandChain(c, ob, oe, strand, d.lhs_id, rhs_id, cp, key_hi, &seq, out,
-                      out_key, out_cnt, out_cap);
-          }
-          ob = j;
-          oe = i;
-          open = true;
-        }
-      }
-      ++j;
-      while (j < i && (i == m || c.d(i) - c.d(j) > cp.bandwidth)) ++j;
+  ChainPairSerial(c, d.cnt, d.gid, d.lhs_id, cp, [&](const rvn_overlap& o) {
+    const unsigned long long slot = atomicAdd(out_cnt, 1ULL);
+    if (slot < out_cap) {
+      out[slot] = o;
+      out_key[slot] = key_hi | seq++;
     }
-  }
-  if (open) {
-    BandChain(c, ob, oe, strand, d.lhs_id, rhs_id, cp, key_hi, &seq, out, out_key,
-              out_cnt, out_cap);
-  }
+  });
 }
 
 // One CTA per (query, rhs, strand) pair with more than kThreadPairMax hits - the
@@ -1116,16 +850,10 @@ PairChainKernel(const GroupDesc* __restrict__ desc, const uint32_t* __restrict__
   const uint32_t g = order[first + blockIdx.x];
   const GroupDesc d = desc[g];
   const uint32_t n = d.cnt;
-  const uint32_t ncap = npad - 1, nbmax = ncap / 4 + 1;
   ChainWork<uint16_t> wk;
   wk.G = reinterpret_cast<uint64_t*>(smem);
   wk.P = wk.G + npad;
-  wk.LB = reinterpret_cast<uint16_t*>(wk.P + npad);
-  wk.PD = wk.LB + (ncap + nbmax + 2);
-  wk.IB = wk.PD + (ncap + 1);
-  wk.IE = wk.IB + nbmax;
-  wk.CNT = reinterpret_cast<uint32_t*>(
-      (reinterpret_cast<uintptr_t>(wk.IE + nbmax) + 3) & ~uintptr_t(3));
+  wk.PlaceIndices(reinterpret_cast<uint16_t*>(wk.P + npad), npad - 1);
   // padding beyond the pair's hits sorts last (all ones), like the reference's dummy
   uint32_t np2 = 8;
   while (np2 < n + 1) np2 <<= 1;
@@ -1228,12 +956,7 @@ ChainKernelGlobal(const uint64_t* __restrict__ h_grp,
   ChainWork<uint32_t> wk;
   wk.G = slab64 + slab64_off[blockIdx.x];
   wk.P = wk.G + npad;
-  const uint32_t nbmax = n / 4 + 1;
-  wk.LB = slab32 + slab32_off[blockIdx.x];
-  wk.PD = wk.LB + (n + nbmax + 2);
-  wk.IB = wk.PD + (n + 1);
-  wk.IE = wk.IB + nbmax;
-  wk.CNT = wk.IE + nbmax;
+  wk.PlaceIndices(slab32 + slab32_off[blockIdx.x], n);
 
   for (uint32_t i = threadIdx.x; i < npad; i += kThreads) {
     wk.G[i] = i < n ? h_grp[hb + i] : ~0ULL;
@@ -1514,6 +1237,277 @@ HitCounts ProbeHits(Ctx& c, uint32_t first, uint32_t last, bool avoid_equal,
   return h;
 }
 
+// read size classes of the split path: n hits take the first class with n + 1 <= bound
+constexpr uint32_t kSplitBounds[] = {256, 512, 1024, 2048, 4096, 8192, 65536};
+constexpr int kSplitClasses = sizeof(kSplitBounds) / sizeof(kSplitBounds[0]);
+// pair size classes, descending: one launch chains the pairs with
+// kPairBounds[b + 1] < hits <= kPairBounds[b]; a CTA per pair (PairChainKernel, shared
+// memory by class) above kThreadPairMax, a thread per pair from there on
+// (GroupChainKernel: shared memory per CTA = threads x class bound x 12 B)
+constexpr uint32_t kPairBounds[] = {8191, 4095, 2047, 1023, 511, 255, 127, 63,
+                                    kThreadPairMax, 32, 24, 16, 8};
+constexpr uint32_t kPairClasses = sizeof(kPairBounds) / sizeof(kPairBounds[0]);
+constexpr uint32_t kFirstThreadClass = 8;
+static_assert(kPairBounds[kFirstThreadClass] == kThreadPairMax,
+              "pairs of up to kThreadPairMax hits get a thread each");
+constexpr int kGroupSmemLimit = 200 * 1024;        // GroupChainKernel's dynamic shared memory
+constexpr uint64_t kGroupSmemBudget = 196 * 1024;  // what one of its CTAs may take
+
+struct ReadRoutes {
+  std::vector<uint32_t> split[kSplitClasses];  // the split path, by size class
+  std::vector<uint32_t> global;                // the global-memory path (ChainKernelGlobal)
+};
+
+// Where each read is chained: reads beyond kChainSmemCap hits, and all reads when
+// chain < 1, on the global-memory path, the others on the split path. Reads of fewer
+// than 4 hits form no band and go nowhere (their ovl_loc stays 0).
+ReadRoutes ClassifyReads(const std::vector<uint64_t>& h_rho, uint32_t nr, bool split_ok) {
+  ReadRoutes r;
+  for (uint32_t i = 0; i < nr; ++i) {
+    const uint64_t n = h_rho[i + 1] - h_rho[i];
+    if (n < 4) continue;
+    if (n > kChainSmemCap || !split_ok) {
+      r.global.push_back(i);
+      continue;
+    }
+    int k = 0;
+    while (kSplitBounds[k] < n + 1) ++k;
+    r.split[k].push_back(i);
+  }
+  return r;
+}
+
+// the split path's pairs: descriptors, and their hits pair-contiguous
+struct PairSplit {
+  const uint32_t* d_list;  // the split reads on the device, largest size class first
+  uint32_t n_reads;
+  GroupDesc* desc;
+  uint32_t *dcnt, *didx, *g_diag;
+  uint64_t *g_pos, *group_loc;
+  uint64_t n_groups;
+};
+
+// Splits the hits of the split path's reads by pair (SplitKernel, one launch per size
+// class, largest first). The reads SplitKernel hands back - more distinct pairs than
+// its table holds, or a pair of more than kPairMaxHits hits - join routes.global in
+// read order. counter[1] and [2] count the pairs and their hits.
+PairSplit SplitPairs(Ctx& c, const uint64_t* hg, const uint64_t* hp,
+                     const uint64_t* read_hit_off, const uint32_t* lhs_ids, ReadRoutes& routes,
+                     uint32_t nr, uint64_t n_hits, uint64_t n_q, uint64_t* counter) {
+  PairSplit s{};
+  std::vector<uint32_t> list;
+  for (int k = kSplitClasses - 1; k >= 0; --k) {
+    list.insert(list.end(), routes.split[k].begin(), routes.split[k].end());
+  }
+  s.n_reads = static_cast<uint32_t>(list.size());
+  uint32_t* d_list = c.m_first.reserve(std::max<size_t>(list.size(), n_q) + 1);
+  s.d_list = d_list;
+  uint32_t* d_fb = c.m_fallback.reserve(nr + 4ULL);
+  RVN_CUDA(cudaMemsetAsync(d_fb, 0, 2 * sizeof(uint32_t), c.stream));
+  if (list.empty()) return s;
+  RVN_CUDA(cudaMemcpyAsync(d_list, list.data(), list.size() * sizeof(uint32_t),
+                           cudaMemcpyHostToDevice, c.stream));
+  RVN_CUDA(cudaStreamSynchronize(c.stream));  // (list goes out of scope)
+
+  const uint64_t max_groups = n_hits / 4 + 1;
+  s.desc = reinterpret_cast<GroupDesc*>(c.m_desc.reserve(max_groups * (sizeof(GroupDesc) / 4)));
+  s.dcnt = c.m_desc_cnt.reserve(max_groups);
+  s.didx = c.m_desc_idx.reserve(max_groups);
+  s.g_diag = c.m_gdiag.reserve(n_hits + 1);
+  s.g_pos = c.m_gpos.reserve(n_hits + 1);
+  c.m_desc_cnt2.reserve(max_groups);  // (ChainPairs' sort buffers)
+  c.m_desc_idx2.reserve(max_groups);
+  s.group_loc = c.m_group_loc.reserve(nr + 1ULL);
+  // counters: [0] overlaps (global-memory path), [1] pairs, [2] kept hits,
+  // [3] overlaps of the pairs
+  RVN_CUDA(cudaMemsetAsync(counter, 0, 4 * sizeof(uint64_t), c.stream));
+  auto* ctr = reinterpret_cast<unsigned long long*>(counter);
+  size_t off = 0;
+  for (int k = kSplitClasses - 1; k >= 0; --k) {  // largest class first
+    const unsigned cnt = static_cast<unsigned>(routes.split[k].size());
+    if (cnt == 0) continue;
+    const size_t smem = MakeSplitLayout(kSplitBounds[k] - 1).bytes;
+    const uint32_t* lst = d_list + off;
+    off += cnt;
+    const bool wide = kSplitBounds[k] > 2048;
+    auto kern = wide ? SplitKernel<256, 2> : SplitKernel<128, 8>;
+    if (wide) {
+      RVN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    static_cast<int>(MakeSplitLayout(kChainSmemCap).bytes)));
+    }
+    kern<<<cnt, wide ? 256 : 128, smem, c.stream>>>(hg, hp, read_hit_off, lhs_ids, lst, ctr + 1,
+                                                    s.desc, s.dcnt, s.didx, s.g_diag, s.g_pos,
+                                                    s.group_loc, d_fb + 2, d_fb);
+    RVN_LAUNCH_CHECK();
+    ++c.launches;
+  }
+  // pair count, reads handed back
+  uint64_t* hpin = c.pin64.reserve(8);
+  RVN_CUDA(cudaMemcpyAsync(hpin, counter, 4 * sizeof(uint64_t), cudaMemcpyDeviceToHost,
+                           c.stream));
+  std::vector<uint32_t> fb(2);
+  RVN_CUDA(cudaMemcpyAsync(fb.data(), d_fb, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost,
+                           c.stream));
+  RVN_CUDA(cudaStreamSynchronize(c.stream));
+  s.n_groups = hpin[1];
+  const uint32_t nfb = fb[0];
+  if (nfb) {
+    fb.resize(nfb);
+    RVN_CUDA(cudaMemcpyAsync(fb.data(), d_fb + 2, nfb * sizeof(uint32_t),
+                             cudaMemcpyDeviceToHost, c.stream));
+    RVN_CUDA(cudaStreamSynchronize(c.stream));
+    std::sort(fb.begin(), fb.end());
+    routes.global.insert(routes.global.end(), fb.begin(), fb.end());
+  }
+  if (s.n_groups >= 0xFFFFFFFFULL) throw LimitError("2^32 or more seed pairs");
+  // GroupDesc::hit_off is 32 bits wide
+  if (hpin[2] >= 0xFFFFFFFFULL) throw LimitError("2^32 or more chained seed hits in one flush");
+  return s;
+}
+
+// Chains every pair, largest first (a stable descending radix sort of the pair sizes,
+// so that the lanes of a warp get pairs of similar size), one launch per size class of
+// kPairBounds. The overlaps land in c.m_ovl_tmp in any order, keyed (pair index,
+// sequence number) in c.m_okey; returns their number.
+uint64_t ChainPairs(Ctx& c, const PairSplit& s, const ChainParams& cp, uint64_t ovl_cap,
+                    uint64_t* counter) {
+  uint32_t* dcnt2 = c.m_desc_cnt2.get();
+  uint32_t* didx2 = c.m_desc_idx2.get();
+  const int w_desc = RadixSortPairs(c, s.dcnt, dcnt2, s.dcnt, s.didx, didx2, s.didx, s.n_groups,
+                                    0, 13, /*descending=*/true);
+  const uint32_t* sorted_cnt = w_desc == 0 ? dcnt2 : s.dcnt;
+  const uint32_t* sorted_idx = w_desc == 0 ? didx2 : s.didx;
+  rvn_overlap* tmp_ovl = c.m_ovl_tmp.reserve(ovl_cap);
+  uint64_t* key = c.m_okey.reserve(ovl_cap);
+  uint32_t* d_bounds = c.m_bounds.reserve(kPairClasses);
+  uint64_t* d_starts = c.m_starts.reserve(kPairClasses + 1);
+  RVN_CUDA(cudaMemcpyAsync(d_bounds, kPairBounds, sizeof(kPairBounds), cudaMemcpyHostToDevice,
+                           c.stream));
+  SizeClassStarts<<<1, 32, 0, c.stream>>>(sorted_cnt, s.n_groups, d_bounds, kPairClasses,
+                                          d_starts);
+  uint64_t h_starts[kPairClasses + 1];
+  RVN_CUDA(cudaMemcpyAsync(h_starts, d_starts, kPairClasses * sizeof(uint64_t),
+                           cudaMemcpyDeviceToHost, c.stream));
+  RVN_CUDA(cudaStreamSynchronize(c.stream));
+  h_starts[kPairClasses] = s.n_groups;
+  h_starts[0] = 0;  // (no pair of the split path has more than kPairMaxHits hits)
+  RVN_CUDA(cudaFuncSetAttribute(GroupChainKernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                kGroupSmemLimit));
+  RVN_CUDA(cudaFuncSetAttribute(PairChainKernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                static_cast<int>(PairChainSmem(kPairMaxHits + 1))));
+  auto* ctr = reinterpret_cast<unsigned long long*>(counter);
+  for (uint32_t b = 0; b < kPairClasses; ++b) {
+    const uint64_t lo = h_starts[b], hi = h_starts[b + 1];
+    if (hi <= lo) continue;
+    if (b < kFirstThreadClass) {
+      const uint32_t npad = kPairBounds[b] + 1;
+      PairChainKernel<<<static_cast<unsigned>(hi - lo), kPairThreads, PairChainSmem(npad),
+                        c.stream>>>(s.desc, sorted_idx, lo, npad, s.g_diag, s.g_pos, cp, tmp_ovl,
+                                    key, ctr + 3, ovl_cap);
+    } else {
+      uint32_t threads = 128;
+      while (threads > 8 && 12ULL * kPairBounds[b] * threads > kGroupSmemBudget) threads >>= 1;
+      const size_t smem = 12ULL * kPairBounds[b] * threads;
+      GroupChainKernel<<<CeilDiv(hi - lo, threads), threads, smem, c.stream>>>(
+          s.desc, sorted_idx, lo, hi, kPairBounds[b], s.g_diag, s.g_pos, cp, tmp_ovl, key,
+          ctr + 3, ovl_cap);
+    }
+    RVN_LAUNCH_CHECK();
+    ++c.launches;
+  }
+  const uint64_t n_ovl = ReadU64(c, counter + 3);
+  if (n_ovl > ovl_cap) throw LimitError("overlap slab overflow");
+  if (n_ovl >= 0xFFFFFFFFULL) throw LimitError("2^32 or more overlaps");
+  return n_ovl;
+}
+
+// Puts the n_ovl overlaps of ChainPairs in emission order = (pair index, sequence
+// number) at the front of raw, and points each split read's ovl_loc at its own.
+void OrderPairOverlaps(Ctx& c, const PairSplit& s, uint64_t n_ovl, uint64_t ovl_cap,
+                       rvn_overlap* raw, uint64_t* loc) {
+  uint64_t* key = c.m_okey.get();
+  uint64_t* key2 = c.m_okey2.reserve(ovl_cap);
+  uint32_t* oidx = c.m_oidx.reserve(ovl_cap);
+  uint32_t* oidx2 = c.m_oidx2.reserve(ovl_cap);
+  IotaU32<<<CeilDiv(n_ovl, kThreads), kThreads, 0, c.stream>>>(oidx, n_ovl);
+  int key_bits = 17;
+  while (key_bits < 64 && (1ULL << (key_bits - 16)) < s.n_groups) ++key_bits;
+  const int w_ovl = RadixSortPairs(c, key, key2, key, oidx, oidx2, oidx, n_ovl, 0, key_bits);
+  const uint64_t* sorted_key = w_ovl == 0 ? key2 : key;
+  const uint32_t* sorted_oidx = w_ovl == 0 ? oidx2 : oidx;
+  GatherOverlapsByIndex<<<CeilDiv(n_ovl * 2, kThreads), kThreads, 0, c.stream>>>(
+      c.m_ovl_tmp.get(), sorted_oidx, n_ovl, raw);
+  LocateReadOverlaps<<<CeilDiv(s.n_reads, kThreads), kThreads, 0, c.stream>>>(
+      sorted_key, n_ovl, s.d_list, s.n_reads, s.group_loc, 0, loc);
+  RVN_LAUNCH_CHECK();
+  c.launches += 3;
+}
+
+// Chains the listed reads whole on the global-memory path (ChainKernelGlobal, a CTA
+// per read over a scratch slab), appending to raw behind what counter[0] holds.
+void ChainWholeReads(Ctx& c, const std::vector<uint32_t>& reads, const uint64_t* hg,
+                     const uint64_t* hp, const uint64_t* read_hit_off,
+                     const std::vector<uint64_t>& h_rho, const uint32_t* lhs_ids,
+                     const ChainParams& cp, rvn_overlap* raw, uint64_t* counter,
+                     uint64_t ovl_cap, uint64_t* loc) {
+  if (reads.empty()) return;
+  std::vector<uint64_t> off64(reads.size() + 1, 0), off32(reads.size() + 1, 0);
+  for (size_t i = 0; i < reads.size(); ++i) {
+    const uint64_t n = h_rho[reads[i] + 1] - h_rho[reads[i]];
+    if (n >= 0x7FFFFFFFULL) throw LimitError("a query has 2^31 or more hits");
+    uint64_t npad = 8;
+    while (npad < n + 1) npad <<= 1;
+    const uint64_t nbmax = n / 4 + 1;
+    off64[i + 1] = off64[i] + 2 * npad;
+    off32[i + 1] = off32[i] + (n + nbmax + 2) + (n + 1) + 3 * nbmax + 4;
+  }
+  uint64_t* slab64 = c.m_scratch64.reserve(off64.back() + 2 * (reads.size() + 1) + 8);
+  uint32_t* slab32 = c.m_scratch32.reserve(off32.back() + reads.size() + 8);
+  // offsets and the read list ride at the tail of the slabs
+  uint64_t* d_off64 = slab64 + off64.back();
+  uint64_t* d_off32 = d_off64 + reads.size() + 1;
+  uint32_t* d_reads = slab32 + off32.back();
+  RVN_CUDA(cudaMemcpyAsync(d_off64, off64.data(), (reads.size() + 1) * 8,
+                           cudaMemcpyHostToDevice, c.stream));
+  RVN_CUDA(cudaMemcpyAsync(d_off32, off32.data(), (reads.size() + 1) * 8,
+                           cudaMemcpyHostToDevice, c.stream));
+  RVN_CUDA(cudaMemcpyAsync(d_reads, reads.data(), reads.size() * 4, cudaMemcpyHostToDevice,
+                           c.stream));
+  ChainKernelGlobal<<<static_cast<unsigned>(reads.size()), kThreads, 0, c.stream>>>(
+      hg, hp, read_hit_off, lhs_ids, d_reads, d_off64, d_off32, slab64, slab32, cp, raw,
+      reinterpret_cast<unsigned long long*>(counter), ovl_cap, loc);
+  RVN_LAUNCH_CHECK();
+  ++c.launches;
+  RVN_CUDA(cudaStreamSynchronize(c.stream));  // host vectors go out of scope
+}
+
+// Moves every read's overlaps from where raw holds them (ovl_loc) to query order in
+// c.m_ovl / c.m_ovl_off; returns their number.
+uint64_t ApplyQueryOrder(Ctx& c, const rvn_overlap* raw, const uint64_t* loc, uint32_t nr,
+                         uint64_t ovl_cap) {
+  uint32_t* ocnt = c.m_cnt.reserve(nr + 1ULL);
+  uint64_t* ooff = c.m_ovl_off.reserve(nr + 2ULL);
+  uint64_t n_ovl = 0;
+  if (nr > 0) {
+    OverlapCounts<<<CeilDiv(nr, kThreads), kThreads, 0, c.stream>>>(loc, nr, ocnt);
+    RVN_LAUNCH_CHECK();
+    ++c.launches;
+    ExclusiveScanU32(c, ocnt, ooff, nr);
+    n_ovl = ReadU64(c, ooff + nr);
+  } else {
+    RVN_CUDA(cudaMemsetAsync(ooff, 0, sizeof(uint64_t), c.stream));
+  }
+  if (n_ovl > ovl_cap) throw LimitError("overlap slab overflow");
+  rvn_overlap* ordered = c.m_ovl.reserve(n_ovl + 1);
+  if (n_ovl > 0) {
+    ReorderOverlaps<<<CeilDiv(nr, kThreads / 32), kThreads, 0, c.stream>>>(raw, loc, ooff, nr,
+                                                                          ordered);
+    RVN_LAUNCH_CHECK();
+    ++c.launches;
+  }
+  return n_ovl;
+}
+
 }  // namespace
 
 // Chains hits that are already grouped by query read: hits of read i of the
@@ -1532,239 +1526,23 @@ uint64_t ChainGroupedHits(Ctx& c, const uint64_t* hg, const uint64_t* hp,
   RVN_CUDA(cudaMemsetAsync(counter, 0, sizeof(uint64_t), c.stream));
   RVN_CUDA(cudaMemsetAsync(loc, 0, (nr + 1ULL) * sizeof(uint64_t), c.stream));
 
-  // ---- fast path: split by (rhs, strand) pair, then one thread per pair ----
-  static const uint32_t kBounds[] = {256, 512, 1024, 2048, 4096, 8192, 65536};
-  constexpr int kClasses = sizeof(kBounds) / sizeof(kBounds[0]);
-  std::vector<uint32_t> cls[kClasses];
-  std::vector<uint32_t> big;
-  const bool fast_ok = c.prm.chain >= 1;
-  for (uint32_t i = 0; i < nr; ++i) {
-    const uint64_t n = h_rho[i + 1] - h_rho[i];
-    if (n < 4) continue;  // cannot form a band; ovl_loc stays 0
-    if (n > kChainSmemCap || !fast_ok) {
-      big.push_back(i);
-      continue;
+  ReadRoutes routes = ClassifyReads(h_rho, nr, c.prm.chain >= 1);
+  const PairSplit s =
+      SplitPairs(c, hg, hp, read_hit_off, lhs_ids, routes, nr, n_hits, n_q, counter);
+  if (s.n_reads) {
+    uint64_t n_pair_ovl = 0;
+    if (s.n_groups) {
+      n_pair_ovl = ChainPairs(c, s, cp, ovl_cap, counter);
+      if (n_pair_ovl) OrderPairOverlaps(c, s, n_pair_ovl, ovl_cap, raw, loc);
     }
-    int k = 0;
-    while (kBounds[k] < n + 1) ++k;
-    cls[k].push_back(i);
+    // the global-memory path appends behind the pairs' overlaps
+    RVN_CUDA(cudaMemcpyAsync(counter, &n_pair_ovl, sizeof(uint64_t), cudaMemcpyHostToDevice,
+                             c.stream));
+    RVN_CUDA(cudaStreamSynchronize(c.stream));
   }
-  uint64_t n_fast_ovl = 0;
-  {
-    size_t total = 0;
-    for (auto& v : cls) total += v.size();
-    uint32_t* d_list = c.m_first.reserve(std::max<size_t>(total, n_q) + 1);
-    uint32_t* d_fb = c.m_fallback.reserve(nr + 4ULL);
-    RVN_CUDA(cudaMemsetAsync(d_fb, 0, 2 * sizeof(uint32_t), c.stream));
-    std::vector<uint32_t> flat;
-    flat.reserve(total);
-    for (int k = kClasses - 1; k >= 0; --k) {
-      flat.insert(flat.end(), cls[k].begin(), cls[k].end());
-    }
-    if (total) {
-      RVN_CUDA(cudaMemcpyAsync(d_list, flat.data(), total * sizeof(uint32_t),
-                               cudaMemcpyHostToDevice, c.stream));
-      RVN_CUDA(cudaStreamSynchronize(c.stream));  // flat goes out of scope
-
-      const uint64_t max_groups = n_hits / 4 + 1;
-      GroupDesc* desc = reinterpret_cast<GroupDesc*>(
-          c.m_desc.reserve(max_groups * (sizeof(GroupDesc) / 4)));
-      uint32_t* dcnt = c.m_desc_cnt.reserve(max_groups);
-      uint32_t* didx = c.m_desc_idx.reserve(max_groups);
-      uint32_t* dcnt2 = c.m_desc_cnt2.reserve(max_groups);
-      uint32_t* didx2 = c.m_desc_idx2.reserve(max_groups);
-      uint32_t* g_diag = c.m_gdiag.reserve(n_hits + 1);
-      uint64_t* g_pos = c.m_gpos.reserve(n_hits + 1);
-      uint64_t* group_loc = c.m_group_loc.reserve(nr + 1ULL);
-      // counters: [0] overlaps (generic path), [1] pairs, [2] kept hits,
-      // [3] overlaps of the fast path
-      RVN_CUDA(cudaMemsetAsync(counter, 0, 4 * sizeof(uint64_t), c.stream));
-      auto* ctr = reinterpret_cast<unsigned long long*>(counter);
-
-      size_t off = 0;
-      for (int k = kClasses - 1; k >= 0; --k) {  // largest class first
-        const unsigned cnt = static_cast<unsigned>(cls[k].size());
-        if (cnt == 0) continue;
-        const size_t smem = MakeSplitLayout(kBounds[k] - 1).bytes;
-        const uint32_t* lst = d_list + off;
-        off += cnt;
-        if (kBounds[k] > 2048) {
-          auto kern = SplitKernel<256, 2>;
-          RVN_CUDA(cudaFuncSetAttribute(
-              kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-              static_cast<int>(MakeSplitLayout(kChainSmemCap).bytes)));
-          kern<<<cnt, 256, smem, c.stream>>>(hg, hp, read_hit_off, lhs_ids, lst,
-                                             ctr + 1, desc, dcnt, didx, g_diag, g_pos,
-                                             group_loc, d_fb + 2, d_fb);
-        } else {
-          auto kern = SplitKernel<128, 8>;
-          kern<<<cnt, 128, smem, c.stream>>>(hg, hp, read_hit_off, lhs_ids, lst,
-                                             ctr + 1, desc, dcnt, didx, g_diag, g_pos,
-                                             group_loc, d_fb + 2, d_fb);
-        }
-        RVN_LAUNCH_CHECK();
-        ++c.launches;
-      }
-      // pair count, reads handed back (pair table full / a pair beyond kPairMaxHits)
-      uint64_t* hpin = c.pin64.reserve(8);
-      RVN_CUDA(cudaMemcpyAsync(hpin, counter, 4 * sizeof(uint64_t),
-                               cudaMemcpyDeviceToHost, c.stream));
-      std::vector<uint32_t> fb(2);
-      RVN_CUDA(cudaMemcpyAsync(fb.data(), d_fb, 2 * sizeof(uint32_t),
-                               cudaMemcpyDeviceToHost, c.stream));
-      RVN_CUDA(cudaStreamSynchronize(c.stream));
-      const uint64_t n_groups = hpin[1];
-      const uint32_t nfb = fb[0];
-      if (nfb) {
-        fb.resize(nfb);
-        RVN_CUDA(cudaMemcpyAsync(fb.data(), d_fb + 2, nfb * sizeof(uint32_t),
-                                 cudaMemcpyDeviceToHost, c.stream));
-        RVN_CUDA(cudaStreamSynchronize(c.stream));
-        std::sort(fb.begin(), fb.end());
-        big.insert(big.end(), fb.begin(), fb.end());
-      }
-      if (n_groups >= 0xFFFFFFFFULL) throw LimitError("2^32 or more seed pairs");
-      // GroupDesc::hit_off is 32 bits wide
-      if (hpin[2] >= 0xFFFFFFFFULL) throw LimitError("2^32 or more chained seed hits in one flush");
-
-      if (n_groups) {
-        // largest pairs first: lanes of a warp get pairs of similar size
-        // (stable descending radix sort on the 13 count bits, radix.cu)
-        const int w_desc = RadixSortPairs(c, dcnt, dcnt2, dcnt, didx, didx2, didx, n_groups, 0, 13,
-                                          /*descending=*/true);
-        const uint32_t* sorted_cnt = w_desc == 0 ? dcnt2 : dcnt;
-        const uint32_t* sorted_idx = w_desc == 0 ? didx2 : didx;
-        rvn_overlap* tmp_ovl = c.m_ovl_tmp.reserve(ovl_cap);
-        uint64_t* key = c.m_okey.reserve(ovl_cap);
-        uint64_t* key2 = c.m_okey2.reserve(ovl_cap);
-        uint32_t* oidx = c.m_oidx.reserve(ovl_cap);
-        uint32_t* oidx2 = c.m_oidx2.reserve(ovl_cap);
-        // One launch per size class of the (descending) pair order. Pairs with more
-        // than kThreadPairMax hits get a CTA each (PairChainKernel, shared memory
-        // by class); the many small ones a thread each (GroupChainKernel: shared
-        // memory per CTA = threads x class bound x 12 B).
-        static const uint32_t kGB[] = {8191, 4095, 2047, 1023, 511, 255, 127, 63,
-                                       kThreadPairMax, 32, 24, 16, 8};
-        constexpr uint32_t kNB = sizeof(kGB) / sizeof(kGB[0]);
-        constexpr uint32_t kFirstThreadClass = 8;  // kGB[8] == kThreadPairMax
-        uint32_t* d_bounds = c.m_bounds.reserve(kNB);
-        uint64_t* d_starts = c.m_starts.reserve(kNB + 1);
-        RVN_CUDA(cudaMemcpyAsync(d_bounds, kGB, sizeof(kGB), cudaMemcpyHostToDevice,
-                                 c.stream));
-        SizeClassStarts<<<1, 32, 0, c.stream>>>(sorted_cnt, n_groups, d_bounds, kNB, d_starts);
-        uint64_t h_starts[kNB + 1];
-        RVN_CUDA(cudaMemcpyAsync(h_starts, d_starts, kNB * sizeof(uint64_t),
-                                 cudaMemcpyDeviceToHost, c.stream));
-        RVN_CUDA(cudaStreamSynchronize(c.stream));
-        h_starts[kNB] = n_groups;
-        h_starts[0] = 0;  // (a read has at most kChainSmemCap = 8191 hits on this path)
-        RVN_CUDA(cudaFuncSetAttribute(GroupChainKernel,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      200 * 1024));
-        RVN_CUDA(cudaFuncSetAttribute(PairChainKernel,
-                                      cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      static_cast<int>(PairChainSmem(8192))));
-        for (uint32_t b = 0; b < kNB; ++b) {
-          // pairs with bound[b+1] < count <= bound[b]
-          const uint64_t lo = h_starts[b], hi = h_starts[b + 1];
-          if (hi <= lo) continue;
-          if (b < kFirstThreadClass) {
-            const uint32_t npad = kGB[b] + 1;
-            PairChainKernel<<<static_cast<unsigned>(hi - lo), kPairThreads, PairChainSmem(npad),
-                              c.stream>>>(desc, sorted_idx, lo, npad, g_diag, g_pos, cp, tmp_ovl,
-                                          key, ctr + 3, ovl_cap);
-          } else {
-            uint32_t threads = 128;
-            while (threads > 8 && 12ULL * kGB[b] * threads > 196 * 1024) threads >>= 1;
-            const size_t smem = 12ULL * kGB[b] * threads;
-            GroupChainKernel<<<CeilDiv(hi - lo, threads), threads, smem, c.stream>>>(
-                desc, sorted_idx, lo, hi, kGB[b], g_diag, g_pos, cp, tmp_ovl, key, ctr + 3,
-                ovl_cap);
-          }
-          RVN_LAUNCH_CHECK();
-          ++c.launches;
-        }
-        n_fast_ovl = ReadU64(c, counter + 3);
-        if (n_fast_ovl > ovl_cap) throw LimitError("overlap slab overflow");
-        if (n_fast_ovl >= 0xFFFFFFFFULL) throw LimitError("2^32 or more overlaps");
-        if (n_fast_ovl) {
-          // emission order = (pair index, sequence number)
-          IotaU32<<<CeilDiv(n_fast_ovl, kThreads), kThreads, 0, c.stream>>>(
-              oidx, n_fast_ovl);
-          int key_bits = 17;
-          while (key_bits < 64 && (1ULL << (key_bits - 16)) < n_groups) ++key_bits;
-          const int w_ovl = RadixSortPairs(c, key, key2, key, oidx, oidx2, oidx, n_fast_ovl, 0,
-                                           key_bits);
-          const uint64_t* sorted_key = w_ovl == 0 ? key2 : key;
-          const uint32_t* sorted_oidx = w_ovl == 0 ? oidx2 : oidx;
-          GatherOverlapsByIndex<<<CeilDiv(n_fast_ovl * 2, kThreads), kThreads, 0,
-                                  c.stream>>>(tmp_ovl, sorted_oidx, n_fast_ovl, raw);
-          LocateReadOverlaps<<<CeilDiv(total, kThreads), kThreads, 0, c.stream>>>(
-              sorted_key, n_fast_ovl, d_list, static_cast<uint32_t>(total),
-              group_loc, 0, loc);
-          RVN_LAUNCH_CHECK();
-          c.launches += 3;
-        }
-      }
-      // the generic kernel appends behind the fast path's overlaps
-      RVN_CUDA(cudaMemcpyAsync(counter, &n_fast_ovl, sizeof(uint64_t),
-                               cudaMemcpyHostToDevice, c.stream));
-      RVN_CUDA(cudaStreamSynchronize(c.stream));
-    }
-  }
-  if (!big.empty()) {
-    std::vector<uint64_t> off64(big.size() + 1, 0), off32(big.size() + 1, 0);
-    for (size_t i = 0; i < big.size(); ++i) {
-      const uint64_t n = h_rho[big[i] + 1] - h_rho[big[i]];
-      if (n >= 0x7FFFFFFFULL) throw LimitError("a query has 2^31 or more hits");
-      uint64_t npad = 8;
-      while (npad < n + 1) npad <<= 1;
-      const uint64_t nbmax = n / 4 + 1;
-      off64[i + 1] = off64[i] + 2 * npad;
-      off32[i + 1] = off32[i] + (n + nbmax + 2) + (n + 1) + 3 * nbmax + 4;
-    }
-    uint64_t* slab64 = c.m_scratch64.reserve(off64.back() + 2 * (big.size() + 1) + 8);
-    uint32_t* slab32 = c.m_scratch32.reserve(off32.back() + big.size() + 8);
-    // offsets and the read list ride at the tail of the slabs
-    uint64_t* d_off64 = slab64 + off64.back();
-    uint64_t* d_off32 = d_off64 + big.size() + 1;
-    uint32_t* d_big = slab32 + off32.back();
-    RVN_CUDA(cudaMemcpyAsync(d_off64, off64.data(), (big.size() + 1) * 8,
-                             cudaMemcpyHostToDevice, c.stream));
-    RVN_CUDA(cudaMemcpyAsync(d_off32, off32.data(), (big.size() + 1) * 8,
-                             cudaMemcpyHostToDevice, c.stream));
-    RVN_CUDA(cudaMemcpyAsync(d_big, big.data(), big.size() * 4,
-                             cudaMemcpyHostToDevice, c.stream));
-    ChainKernelGlobal<<<static_cast<unsigned>(big.size()), kThreads, 0,
-                        c.stream>>>(
-        hg, hp, read_hit_off, lhs_ids, d_big, d_off64, d_off32, slab64, slab32, cp,
-        raw, reinterpret_cast<unsigned long long*>(counter), ovl_cap, loc);
-    RVN_LAUNCH_CHECK();
-    ++c.launches;
-    RVN_CUDA(cudaStreamSynchronize(c.stream));  // host vectors go out of scope
-  }
-
-  // ---- query order ----
-  uint32_t* ocnt = c.m_cnt.reserve(nr + 1ULL);
-  uint64_t* ooff = c.m_ovl_off.reserve(nr + 2ULL);
-  uint64_t n_ovl = 0;
-  if (nr > 0) {
-    OverlapCounts<<<CeilDiv(nr, kThreads), kThreads, 0, c.stream>>>(loc, nr, ocnt);
-    RVN_LAUNCH_CHECK();
-    ++c.launches;
-    ExclusiveScanU32(c, ocnt, ooff, nr);
-    n_ovl = ReadU64(c, ooff + nr);
-  } else {
-    RVN_CUDA(cudaMemsetAsync(ooff, 0, sizeof(uint64_t), c.stream));
-  }
-  if (n_ovl > ovl_cap) throw LimitError("overlap slab overflow");
-  rvn_overlap* ordered = c.m_ovl.reserve(n_ovl + 1);
-  if (n_ovl > 0) {
-    ReorderOverlaps<<<CeilDiv(nr, kThreads / 32), kThreads, 0, c.stream>>>(
-        raw, loc, ooff, nr, ordered);
-    RVN_LAUNCH_CHECK();
-    ++c.launches;
-  }
+  ChainWholeReads(c, routes.global, hg, hp, read_hit_off, h_rho, lhs_ids, cp, raw, counter,
+                  ovl_cap, loc);
+  const uint64_t n_ovl = ApplyQueryOrder(c, raw, loc, nr, ovl_cap);
   TimerEnd(c);
   return n_ovl;
 }
