@@ -183,6 +183,8 @@ int rvn_edit_distance_batch(rvn_ctx* ctx, uint64_t n_pairs, const uint32_t* lhs_
  * 1260 >> 4 bins; begin/end then stay 0 / bins like the reference's fields); else
  * [begin[i], end[i]) is the valid region in bins and median[i] the element of rank
  * size/2 of it. The caller zeroes the bins outside the region like UpdateValidRegion.
+ * After a windowed call (option "stage1_window") the piles are in host memory and pass
+ * through the device in chunks of reads; the outputs are the same.
  * RVN_ERR_STATE if another call has replaced the device piles since. */
 int rvn_stage1_pile_regions(rvn_ctx* ctx, uint32_t coverage, uint32_t* begin, uint32_t* end,
                             uint16_t* median, uint8_t* invalid);
@@ -208,6 +210,16 @@ int rvn_align_breaking_points(rvn_ctx* ctx, uint64_t n_pairs, const uint32_t* q_
                               const uint32_t* t_begin, const uint32_t* t_len, uint32_t window,
                               const uint64_t* bp_off, int32_t* distance,
                               uint32_t* breaking_points);
+
+/* The estimates behind option "stage1_window" -1 (auto) for a stage-1 call over the
+ * uploaded reads with these arguments (0 = the defaults, as in
+ * rvn_find_overlaps_and_create_piles), in bytes: device memory of a resident pass, device
+ * memory of a windowed pass, pinned host memory of a windowed pass. Auto runs windowed
+ * only when the resident estimate exceeds the free device memory (plus the buffers the
+ * context already holds), max_overlaps <= 65536 and both windowed estimates fit. */
+int rvn_stage1_footprint(rvn_ctx* ctx, uint64_t max_overlaps, uint64_t index_batch_bases,
+                         uint64_t query_batch_bases, uint64_t* resident,
+                         uint64_t* windowed_device, uint64_t* windowed_host);
 
 /* raven::FindOverlapsAndCreatePiles over the uploaded read set: index batches
  * of >= index_batch_bases (reference: 1<<32), query flushes of >=
@@ -281,8 +293,18 @@ int rvn_get_stats(rvn_ctx* ctx, rvn_stats* out);
  * rvn_reads_upload* returns while the packed bases still travel - in chunks, on a
  * copy stream - and the sketch kernel of the next call starts on the reads that
  * have arrived; the caller must keep `words` unchanged until the next call on the
- * context has returned; meant for pinned host memory); "reset_stats".
- * Unknown name -> RVN_ERR_INVALID. */
+ * context has returned; meant for pinned host memory); "stage1_window" (where
+ * rvn_find_overlaps_and_create_piles keeps the piles and overlap lists of all reads:
+ * 0 = on the device for the whole pass; 1 = windowed: in pinned host memory, and
+ * each flush brings only the reads it touches - its queries and the current index
+ * batch - to the device, so the device holds the packed bases, one index batch and
+ * one window; -1 = auto, the default: windowed only when an estimate of the
+ * resident pass exceeds the free device memory and the windowed pass fits
+ * (rvn_stage1_footprint), else resident. Results are identical in every
+ * mode; a windowed pass takes max_overlaps <= 65536 and leaves phase
+ * "stage1_window" in rvn_get_timings); "stage1_window_budget" (bytes: replaces the
+ * free device memory in the auto decision, 0 = the free memory); "reset_stats".
+ * Unknown name or value out of range -> RVN_ERR_INVALID. */
 int rvn_set_option(rvn_ctx* ctx, const char* name, int64_t value);
 
 /* Device time (ms, CUDA events on the context's stream) of the phases of the

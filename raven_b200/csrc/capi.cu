@@ -3,6 +3,9 @@
 // (RavenLib/src/construct.cc:14-121).
 #include <algorithm>
 #include <cstring>
+#include <memory>
+
+#include <unistd.h>
 
 #include "engine.cuh"
 
@@ -17,6 +20,12 @@ namespace {
 template <typename F>
 int Guard(rvn_ctx* ctx, F&& f, bool sketches_first = false) {
   if (!ctx) return RVN_ERR_INVALID;
+  // buffers allocated during the call are charged to this context
+  struct Owner {
+    uint64_t* prev;
+    explicit Owner(uint64_t* o) : prev(g_devbuf_owner) { g_devbuf_owner = o; }
+    ~Owner() { g_devbuf_owner = prev; }
+  } owner(&ctx->c.held_bytes);
   try {
     RVN_CUDA(cudaSetDevice(ctx->c.device));
     // an asynchronous upload in flight: calls that begin with the sketch kernel
@@ -61,9 +70,235 @@ void CheckRange(const Ctx& c, uint32_t first, uint32_t last) {
   }
 }
 
+// The reference's schedule (construct.cc:36-112): index batches [j, end) of >= ib
+// bases, and per batch the flushes of its queries - every read up to the end of
+// the batch - per >= qb bases (the truncation rule makes the flush boundaries
+// observable).
+struct Batch {
+  uint32_t j, end;
+  std::vector<std::pair<uint32_t, uint32_t>> flushes;  // [k0, k1)
+};
+
+std::vector<Batch> Schedule(const Ctx& c, uint64_t ib, uint64_t qb) {
+  std::vector<Batch> out;
+  const uint32_t n = c.n_reads;
+  uint64_t bases = 0;
+  for (uint32_t i = 0, j = 0; i < n; ++i) {
+    bases += c.h_len[i];
+    if (i != n - 1 && bases < ib) continue;
+    bases = 0;
+    Batch b{j, i + 1, {}};
+    for (uint32_t k = 0, k0 = 0; k < i + 1; ++k) {
+      bases += c.h_len[k];
+      if (k != i && bases < qb) continue;
+      bases = 0;
+      b.flushes.emplace_back(k0, k + 1);
+      k0 = k + 1;
+    }
+    out.push_back(std::move(b));
+    j = i + 1;
+  }
+  return out;
+}
+
+// Largest max_overlaps a windowed pass takes: it keeps that many records per read.
+constexpr uint64_t kWindowMaxOverlaps = 1ULL << 16;
+// Device working set of one index batch (sketch, tiers, bare keys, bucket table,
+// self-join slots, one flush's hits, with the buffers' headroom) per base of the
+// batch: a C2 pass (one 1.98 Gbp batch) holds 43.6 GB in all (DESIGN.md §3, §5).
+constexpr double kBatchBytesPerBase = 21.0;
+
+// Estimated memory of a stage-1 pass over the uploaded reads, in bytes.
+struct Footprint {
+  double resident = 0;         // device, resident pass
+  double windowed_device = 0;  // device, windowed pass
+  double windowed_host = 0;    // pinned host, windowed pass
+};
+
+// Both modes hold the reads (packed bases, offsets, lengths, ids, pile offsets)
+// and the working set of the largest index batch. On top of that:
+// - resident: all piles (u16 per bin) and their difference array (i32 per bin and
+//   read), and the lists in two copies plus the staging list and its sort keys.
+//   A list keeps at most kmax records; the estimate also takes one overlap per
+//   other read as the most a list gathers, since the compact lists only hold what
+//   was kept.
+// - windowed, on the device: the same per slot of the largest window, with kmax
+//   (at least 1) records per list row; on the host: the rows, counts and piles of
+//   all reads.
+// off: pile offsets of the reads (len >> 4 bins each, n + 1 entries)
+Footprint Stage1Footprint(const Ctx& c, const std::vector<uint64_t>& off,
+                          const std::vector<Batch>& batches, uint64_t kmax) {
+  const uint32_t n = c.n_reads;
+  const double bins = static_cast<double>(off[n]);
+  const double stride = static_cast<double>(std::max<uint64_t>(kmax, 1));
+  const double list_bytes = 3.0 * sizeof(rvn_overlap) + 8.0;  // per record
+  uint64_t batch_bases = 0;
+  double window = 0;  // device bytes of the largest window
+  for (const Batch& b : batches) {
+    uint64_t bases = 0;
+    for (uint32_t r = b.j; r < b.end; ++r) bases += c.h_len[r];
+    batch_bases = std::max(batch_bases, bases);
+    for (const auto& f : b.flushes) {
+      const uint32_t a0 = std::min(f.first, b.j), a1 = std::min(f.second, b.j);
+      const double slots = (b.end - b.j) + (a1 - a0);
+      const double wbins = static_cast<double>((off[b.end] - off[b.j]) + (off[a1] - off[a0]));
+      window = std::max(window, 6.0 * wbins + 4.0 * slots + slots * stride * list_bytes);
+    }
+  }
+  const double reads = 8.0 * c.n_words + 32.0 * n + kBatchBytesPerBase * batch_bases;
+  const double kept = std::min(static_cast<double>(kmax), n > 0 ? n - 1.0 : 0.0);
+  Footprint f;
+  f.resident = reads + 6.0 * bins + 4.0 * n + n * kept * list_bytes;
+  f.windowed_device = reads + window;
+  f.windowed_host = n * stride * sizeof(rvn_overlap) + 4.0 * n + 2.0 * bins;
+  return f;
+}
+
+// Option "stage1_window" -1 (auto): windowed only when the resident estimate exceeds
+// the device memory a pass can use and the windowed pass itself fits: it takes
+// kmax, its own device estimate fits the same memory and its host rows fit the
+// host's free physical memory. Otherwise resident, as before the option existed.
+// Usable device memory: the free memory plus the buffers this context already
+// holds, since a pass re-uses them ("stage1_window_budget" replaces both when it is
+// not 0).
+bool UseWindow(Ctx& c, const std::vector<Batch>& batches, uint64_t kmax) {
+  if (c.stage1_window >= 0) return c.stage1_window != 0;
+  if (kmax > kWindowMaxOverlaps) return false;
+  const Footprint f = Stage1Footprint(c, c.st_pile_off, batches, kmax);
+  double budget = static_cast<double>(c.stage1_window_budget);
+  if (budget == 0) {
+    size_t free_b = 0, total_b = 0;
+    RVN_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    budget = static_cast<double>(free_b) + static_cast<double>(c.held_bytes);
+  }
+  if (f.resident <= budget) return false;
+  const double host_free = static_cast<double>(sysconf(_SC_AVPHYS_PAGES)) *
+                           static_cast<double>(sysconf(_SC_PAGESIZE));
+  return f.windowed_device <= budget && f.windowed_host <= host_free;
+}
+
+// Windowed stage 1: the piles (c.st_pile) and kept lists of all reads stay on the
+// host, the lists in rows of kmax records plus a count per read (c.w_rows, c.w_cnt).
+// A flush brings the reads it touches - its Window - to the device: the index
+// batch's piles and lists stay there for the whole batch, those of the flush's
+// queries before the batch come and go with the flush. Same kernels as the
+// resident pass, on window slots; results land in st_ovl / st_ovl_off / st_pile.
+class WindowedStage1 {
+ public:
+  WindowedStage1(Ctx& c, uint64_t kmax, uint64_t total_bins)
+      : c_(c), kmax_(kmax), stride_(std::max<uint64_t>(kmax, 1)) {
+    if (kmax > kWindowMaxOverlaps) {
+      throw LimitError("windowed stage 1 keeps max_overlaps records per read: at most 65536");
+    }
+    const uint64_t n = c.n_reads;
+    rows_ = c.w_rows.reserve(n * stride_ + 1);
+    cnt_ = c.w_cnt.reserve(n + 1);
+    std::memset(cnt_, 0, (n + 1) * sizeof(uint32_t));
+    pile_ = c.st_pile.reserve(total_bins + 1);
+    std::memset(pile_, 0, (total_bins + 1) * sizeof(uint16_t));
+  }
+
+  // reads of [j, end) have neither piles nor lists yet: the batch part starts empty
+  void BeginBatch(const Batch& b) {
+    const std::vector<uint64_t>& off = c_.st_pile_off;
+    j_ = b.j;
+    end_ = b.end;
+    nb_ = end_ - j_;
+    bb_ = off[end_] - off[j_];
+    uint64_t max_a = 0, max_a_bins = 0;
+    for (const auto& f : b.flushes) {
+      const uint32_t a0 = std::min(f.first, j_), a1 = std::min(f.second, j_);
+      max_a = std::max<uint64_t>(max_a, a1 - a0);
+      max_a_bins = std::max(max_a_bins, off[a1] - off[a0]);
+    }
+    // sized once per batch: growing a buffer does not keep its contents
+    const uint64_t slots = nb_ + max_a;
+    c_.g_list[0].reserve(slots * stride_ + 1);
+    c_.g_list[1].reserve(slots * stride_ + 1);
+    c_.g_cnt.reserve(slots + 1);
+    c_.g_kept.reserve(slots + 1);
+    c_.w_row_off.reserve(slots + 2);
+    c_.w_pile_off.reserve(slots + 2);
+    c_.p_data.reserve(bb_ + max_a_bins + 1);
+    RVN_CUDA(cudaMemsetAsync(c_.g_cnt.get(), 0, nb_ * sizeof(uint32_t), c_.stream));
+    RVN_CUDA(cudaMemsetAsync(c_.p_data.get(), 0, bb_ * sizeof(uint16_t), c_.stream));
+  }
+
+  // the overlaps MapRange left in c.m_ovl for the queries [k0, k1)
+  void Flush(uint32_t k0, uint32_t k1) {
+    if (c_.r_n_ovl == 0) return;
+    const std::vector<uint64_t>& off = c_.st_pile_off;
+    const Window w{j_, end_, std::min(k0, j_), std::min(k1, j_)};
+    const uint32_t na = w.a1 - w.a0;
+    const uint64_t a_bins = off[w.a1] - off[w.a0];
+    TimerBegin(c_, "stage1_window");
+    Move(w, cudaMemcpyHostToDevice);
+    WindowTables(c_, w, c_.p_off.get(), stride_, c_.w_row_off.get(), c_.w_pile_off.get());
+    TimerEnd(c_);
+    PileAddLayersDevice(c_, c_.p_data.get(), c_.w_pile_off.get(), bb_ + a_bins, w,
+                        c_.m_ovl.get(), c_.r_n_ovl);
+    GatherFlush(c_, c_.m_ovl.get(), c_.m_ovl_off.get(), c_.r_n_ovl, k0, k1, kmax_, w,
+                c_.w_row_off.get(), stride_);
+    if (na) {
+      TimerBegin(c_, "stage1_window");
+      Move(w, cudaMemcpyDeviceToHost);
+      TimerEnd(c_);
+    }
+  }
+
+  // the batch part goes back to the host
+  void EndBatch() {
+    TimerBegin(c_, "stage1_window");
+    Move(Window{j_, end_, 0, 0}, cudaMemcpyDeviceToHost, /*batch=*/true);
+    TimerEnd(c_);
+  }
+
+  // compact lists, as the resident pass leaves them
+  void Fetch() {
+    RVN_CUDA(cudaStreamSynchronize(c_.stream));
+    const uint32_t n = c_.n_reads;
+    uint64_t* ooff = c_.st_ovl_off.reserve(n + 1ULL);
+    ooff[0] = 0;
+    for (uint32_t r = 0; r < n; ++r) ooff[r + 1] = ooff[r] + cnt_[r];
+    rvn_overlap* o = c_.st_ovl.reserve(ooff[n] + 1);
+    for (uint32_t r = 0; r < n; ++r) {
+      std::memcpy(o + ooff[r], rows_ + r * stride_, cnt_[r] * sizeof(rvn_overlap));
+    }
+  }
+
+ private:
+  // the query part of `w` (or the batch part) between its host home and the device
+  void Move(const Window& w, cudaMemcpyKind kind, bool batch = false) {
+    const uint32_t r0 = batch ? w.b0 : w.a0, r1 = batch ? w.b1 : w.a1;
+    if (r1 == r0) return;
+    const uint64_t slot0 = batch ? 0 : nb_;
+    const uint64_t bin0 = batch ? 0 : bb_;
+    const std::vector<uint64_t>& off = c_.st_pile_off;
+    const bool up = kind == cudaMemcpyHostToDevice;
+    auto copy = [&](void* dev, void* host, uint64_t bytes) {
+      if (bytes) {
+        RVN_CUDA(cudaMemcpyAsync(up ? dev : host, up ? host : dev, bytes, kind, c_.stream));
+      }
+    };
+    copy(c_.g_cnt.get() + slot0, cnt_ + r0, (r1 - r0) * sizeof(uint32_t));
+    copy(c_.g_list[c_.g_cur].get() + slot0 * stride_, rows_ + r0 * stride_,
+         (r1 - r0) * stride_ * sizeof(rvn_overlap));
+    copy(c_.p_data.get() + bin0, pile_ + off[r0], (off[r1] - off[r0]) * sizeof(uint16_t));
+  }
+
+  Ctx& c_;
+  const uint64_t kmax_, stride_;
+  rvn_overlap* rows_;
+  uint32_t* cnt_;
+  uint16_t* pile_;
+  uint32_t j_ = 0, end_ = 0, nb_ = 0;
+  uint64_t bb_ = 0;
+};
+
 // raven::FindOverlapsAndCreatePiles, same batch / flush schedule as the
 // reference; every step runs on the GPU (Minimize, Filter, Map, AddLayers,
-// gather, truncation); the host only drives the schedule.
+// gather, truncation); the host only drives the schedule (and, windowed, keeps
+// the piles and lists of the reads a flush does not touch).
 void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
             uint64_t qb) {
   if (ib == 0) ib = 1ULL << 32;
@@ -76,6 +311,7 @@ void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
     throw StateError("stage 1 needs read ids equal to their index");
   }
   c.st_valid = false;
+  c.st_piles_on_device = false;
   c.own_mod = 1;
   c.own_rem = 0;
   // a stage-1 pass owns its intermediates: nothing is carried over from an
@@ -92,9 +328,15 @@ void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
     c.st_pile_off[i + 1] = c.st_pile_off[i] + (c.h_len[i] >> 4);
   }
   const uint64_t total_bins = c.st_pile_off[n];
-  uint16_t* d_pile = c.p_data.reserve(total_bins + 1);
+  const std::vector<Batch> batches = Schedule(c, ib, qb);
+  const bool windowed = UseWindow(c, batches, kmax);
+  c.st_windowed = false;
+  uint16_t* d_pile = nullptr;
+  if (!windowed) {
+    d_pile = c.p_data.reserve(total_bins + 1);
+    RVN_CUDA(cudaMemsetAsync(d_pile, 0, (total_bins + 1) * sizeof(uint16_t), c.stream));
+  }
   uint64_t* d_poff = c.p_off.reserve(n + 1ULL);
-  RVN_CUDA(cudaMemsetAsync(d_pile, 0, (total_bins + 1) * sizeof(uint16_t), c.stream));
   if (!c.p_off_uploaded) {  // (an asynchronous upload has sent them ahead of the bases)
     RVN_CUDA(cudaMemcpyAsync(d_poff, c.st_pile_off.data(), (n + 1ULL) * 8,
                              cudaMemcpyHostToDevice, c.stream));
@@ -102,52 +344,52 @@ void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
 
   GatherReset(c);
   c.st_mapped = 0;
+  std::unique_ptr<WindowedStage1> win;
+  if (windowed) win.reset(new WindowedStage1(c, kmax, total_bins));
 
-  uint64_t bases = 0;
   uint64_t tmax = 0;  // largest micromizer value of the reads sketched so far
-  for (uint32_t i = 0, j = 0; i < n; ++i) {
-    bases += c.h_len[i];
-    if (i != n - 1 && bases < ib) continue;
-    bases = 0;
-
+  for (const Batch& b : batches) {
     // Queries are micromizers only (construct.cc:62): no record above the largest
     // micromizer value of any read so far can be hit - those are counted for the
     // occurrence threshold but stay out of the index (index.cu, tiers)
     uint64_t limit = ~0ULL;
     if (!minhash) {
-      tmax = std::max(tmax, MaxMicromizerValue(c, j, i + 1));
+      tmax = std::max(tmax, MaxMicromizerValue(c, b.j, b.end));
       limit = tmax;
     }
-    BuildIndex(c, j, i + 1, minhash, limit);
+    BuildIndex(c, b.j, b.end, minhash, limit);
     FilterIndex(c, freq);
+    if (win) win->BeginBatch(b);
 
-    // every read up to the end of this index batch is a query, flushed per
-    // >= qb bases exactly like the reference (the truncation rule makes the
-    // flush boundaries observable)
-    for (uint32_t k = 0, k0 = 0; k < i + 1; ++k) {
-      bases += c.h_len[k];
-      if (k != i && bases < qb) continue;
-      bases = 0;
-
-      MapRange(c, k0, k + 1, true, true, true, false, /*fetch=*/false);
-      PileAddLayersDevice(c, d_pile, d_poff, c.st_pile_off.data(), n,
-                          c.m_ovl.get(), c.r_n_ovl);
-      GatherFlush(c, c.m_ovl.get(), c.m_ovl_off.get(), c.r_n_ovl, k0, k + 1, kmax);
+    for (const auto& f : b.flushes) {
+      MapRange(c, f.first, f.second, true, true, true, false, /*fetch=*/false);
+      if (win) {
+        win->Flush(f.first, f.second);
+      } else {
+        PileAddLayersDevice(c, d_pile, d_poff, total_bins, Window::All(n), c.m_ovl.get(),
+                            c.r_n_ovl);
+        GatherFlush(c, c.m_ovl.get(), c.m_ovl_off.get(), c.r_n_ovl, f.first, f.second, kmax,
+                    Window::All(n));
+      }
       c.st_mapped += c.r_n_ovl;
-      k0 = k + 1;
     }
-    j = i + 1;
+    if (win) win->EndBatch();
   }
 
-  GatherFetch(c);
-  RVN_CUDA(cudaMemcpyAsync(c.st_pile.reserve(total_bins + 1), d_pile, total_bins * sizeof(uint16_t),
-                           cudaMemcpyDeviceToHost, c.stream));
+  if (win) {
+    win->Fetch();
+  } else {
+    GatherFetch(c);
+    RVN_CUDA(cudaMemcpyAsync(c.st_pile.reserve(total_bins + 1), d_pile,
+                             total_bins * sizeof(uint16_t), cudaMemcpyDeviceToHost, c.stream));
+  }
   RVN_CUDA(cudaStreamSynchronize(c.stream));
   TimerCollect(c);
   c.stats.kernel_launches = c.launches - launches0;
   c.stats.occurrence = c.occurrence;
   c.st_valid = true;
-  c.st_piles_on_device = true;
+  c.st_windowed = windowed;
+  c.st_piles_on_device = !windowed;
 }
 
 }  // namespace
@@ -486,7 +728,7 @@ RVN_API int rvn_pile_add_layers(rvn_ctx* ctx, uint16_t* data,
                              cudaMemcpyHostToDevice, c.stream));
     RVN_CUDA(cudaMemcpyAsync(o, overlaps, n_overlaps * sizeof(rvn_overlap),
                              cudaMemcpyHostToDevice, c.stream));
-    PileAddLayersDevice(c, d, off, bin_off, n_piles, o, n_overlaps);
+    PileAddLayersDevice(c, d, off, bins, Window::All(n_piles), o, n_overlaps);
     RVN_CUDA(cudaMemcpyAsync(data, d, bins * 2, cudaMemcpyDeviceToHost, c.stream));
     RVN_CUDA(cudaStreamSynchronize(c.stream));
     TimerCollect(c);
@@ -544,6 +786,24 @@ RVN_API int rvn_find_overlaps_and_create_piles(rvn_ctx* ctx, double frequency,
   return Guard(ctx, [&](Ctx& c) {
     Stage1(c, frequency, max_overlaps, minhash != 0, index_batch_bases,
            query_batch_bases);
+  }, /*sketches_first=*/true);
+}
+
+RVN_API int rvn_stage1_footprint(rvn_ctx* ctx, uint64_t max_overlaps,
+                                 uint64_t index_batch_bases, uint64_t query_batch_bases,
+                                 uint64_t* resident, uint64_t* windowed_device,
+                                 uint64_t* windowed_host) {
+  return Guard(ctx, [&](Ctx& c) {
+    const uint32_t n = c.n_reads;
+    std::vector<uint64_t> off(n + 1ULL, 0);
+    for (uint32_t i = 0; i < n; ++i) off[i + 1] = off[i] + (c.h_len[i] >> 4);
+    const Footprint f = Stage1Footprint(
+        c, off, Schedule(c, index_batch_bases ? index_batch_bases : 1ULL << 32,
+                         query_batch_bases ? query_batch_bases : 1ULL << 30),
+        max_overlaps);
+    if (resident) *resident = static_cast<uint64_t>(f.resident);
+    if (windowed_device) *windowed_device = static_cast<uint64_t>(f.windowed_device);
+    if (windowed_host) *windowed_host = static_cast<uint64_t>(f.windowed_host);
   }, /*sketches_first=*/true);
 }
 
@@ -759,6 +1019,11 @@ RVN_API int rvn_set_option(rvn_ctx* ctx, const char* name, int64_t value) {
       c.bare_cluster = 0;  // (chosen again at the next build)
     } else if (name && std::strcmp(name, "tier_min_records") == 0) {
       c.tier_min_records = value < 0 ? 0 : static_cast<uint64_t>(value);
+    } else if (name && std::strcmp(name, "stage1_window") == 0) {
+      if (value < -1 || value > 1) throw InvalidArgument("stage1_window: -1 (auto), 0 or 1");
+      c.stage1_window = value;
+    } else if (name && std::strcmp(name, "stage1_window_budget") == 0) {
+      c.stage1_window_budget = value < 0 ? 0 : static_cast<uint64_t>(value);
     } else if (name && std::strcmp(name, "reset_stats") == 0) {
       std::memset(&c.stats, 0, sizeof(c.stats));
       c.launches = 0;

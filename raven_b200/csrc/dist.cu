@@ -725,9 +725,9 @@ void DistStage1Add(Ctx& c, const rvn_overlap* d_ovl, uint64_t n_ovl, uint32_t n_
     if (e > b) {
       RelativeOffsets<<<CeilDiv(k + 2 - k0, kThreads), kThreads, 0, c.stream>>>(qoff, k0,
                                                                               k + 2 - k0, d_rel);
-      PileAddLayersDevice(c, c.p_data.get(), c.p_off.get(), c.st_pile_off.data(), n, merged + b,
-                          e - b);
-      GatherFlush(c, merged + b, d_rel, e - b, k0, k + 1, kmax);
+      PileAddLayersDevice(c, c.p_data.get(), c.p_off.get(), c.st_pile_off[n], Window::All(n),
+                          merged + b, e - b);
+      GatherFlush(c, merged + b, d_rel, e - b, k0, k + 1, kmax, Window::All(n));
     }
     k0 = k + 1;
   }

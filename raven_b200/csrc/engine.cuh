@@ -27,6 +27,22 @@ constexpr uint32_t kSketchTile = 2048;
 constexpr uint32_t kSketchThreads = 256;
 constexpr uint32_t kMaxWindow = 256;  // w limit (halo staged in shared memory)
 
+// The reads one stage-1 flush touches, as dense slots: the index batch [b0, b1)
+// first, then the flush's queries [a0, a1) that lie before it (a1 <= b0, possibly
+// empty). Piles, list counts and offsets of a flush are indexed by slot. The
+// resident layout is the window of all n reads, where slot == id.
+struct Window {
+  uint32_t b0 = 0, b1 = 0, a0 = 0, a1 = 0;
+  static Window All(uint32_t n) { return Window{0, n, 0, 0}; }
+  __host__ __device__ __forceinline__ uint32_t size() const { return (b1 - b0) + (a1 - a0); }
+  __host__ __device__ __forceinline__ uint32_t Slot(uint32_t id) const {
+    return id >= b0 ? id - b0 : (b1 - b0) + (id - a0);
+  }
+  __host__ __device__ __forceinline__ uint32_t Id(uint32_t s) const {
+    return s < b1 - b0 ? b0 + s : a0 + (s - (b1 - b0));
+  }
+};
+
 struct PhaseTimer {
   std::vector<const char*> names;
   std::vector<float> ms;
@@ -35,6 +51,8 @@ struct PhaseTimer {
 };
 
 struct Ctx {
+  // device bytes held by this context's buffers (first member: it outlives them)
+  uint64_t held_bytes = 0;
   int device = 0;
   int sms = 132;  // multiprocessors of `device` (grid caps of the grid-stride kernels)
   cudaStream_t stream = nullptr;
@@ -187,6 +205,18 @@ struct Ctx {
   DevBuf<uint32_t> g_cnt, g_kept, g_key, g_idx, g_key2, g_idx2, g_rhs_cnt,
       g_total_cnt;
 
+  // ---- windowed stage 1 (capi.cu): piles and lists of all reads on the host,
+  // a flush's window of them on the device ----
+  // option "stage1_window": 0 resident, 1 windowed, -1 (default) windowed only when
+  // the resident estimate exceeds the free device memory ("stage1_window_budget"
+  // replaces that free memory when it is not 0)
+  int64_t stage1_window = -1;
+  uint64_t stage1_window_budget = 0;
+  bool st_windowed = false;  // the last stage-1 call ran windowed
+  PinBuf<rvn_overlap> w_rows;  // kmax records per read
+  PinBuf<uint32_t> w_cnt;      // kept records per read
+  DevBuf<uint64_t> w_pile_off, w_row_off;  // per slot (+1) of the current window
+
   // ---- POA (poa.cu) ----
   DevBuf<uint32_t> po_win_first, po_seq_begin, po_seq_end, po_cons_len, po_cov, po_list;
   DevBuf<uint64_t> po_seq_off, po_d_cons_off;
@@ -314,9 +344,18 @@ uint64_t ChainGroupedHits(Ctx& c, const uint64_t* hg, const uint64_t* hp,
 
 // ---- gather.cu ----
 void GatherReset(Ctx& c);
+// one flush over the reads of window `w` (lists, counts and offsets by slot).
+// row_off null: the lists are compact (c.g_off) and are re-compacted; otherwise
+// every slot owns a fixed row of row_stride records at row_off[slot] and the lists
+// stay in their rows
 void GatherFlush(Ctx& c, const rvn_overlap* ovl, const uint64_t* q_ovl_off,
-                 uint64_t m, uint32_t k0, uint32_t k1, uint64_t kmax);
+                 uint64_t m, uint32_t k0, uint32_t k1, uint64_t kmax, const Window& w,
+                 const uint64_t* row_off = nullptr, uint64_t row_stride = 0);
 void GatherFetch(Ctx& c);
+// the window tables: row_off[s] = s * stride, pile_off[s] = first bin of slot s
+// in a pile buffer that holds the window's piles in slot order (both nw + 1)
+void WindowTables(Ctx& c, const Window& w, const uint64_t* d_poff, uint64_t stride,
+                  uint64_t* row_off, uint64_t* pile_off);
 
 // ---- dist.cu ---- key-partitioned index, reads owned by id mod parts
 // which: 0 = full minimizers, 1 = micromizers; records of reads [first,last)
@@ -357,10 +396,10 @@ void EditDistanceBatch(Ctx& c, uint64_t n, const uint32_t* lhs_read, const uint3
                        const uint8_t* strand, const int32_t* limit, int32_t* out);
 
 // ---- pile.cu ----
-// data: device u16 bins, off: device u64 offsets (n_piles + 1)
-void PileAddLayersDevice(Ctx& c, uint16_t* d_data, const uint64_t* d_off,
-                         const uint64_t* h_off, uint32_t n_piles,
-                         const rvn_overlap* d_ovl, uint64_t n_ovl);
+// data: device u16 bins of the piles of window `w` in slot order, off: their device
+// u64 offsets (w.size() + 1), `bins` of them in all
+void PileAddLayersDevice(Ctx& c, uint16_t* d_data, const uint64_t* d_off, uint64_t bins,
+                         const Window& w, const rvn_overlap* d_ovl, uint64_t n_ovl);
 
 // ---- poa.cu ---- racon window consensus over a flat batch of windows
 void PoaBatch(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first,

@@ -40,34 +40,36 @@ __device__ __forceinline__ uint32_t OverlapLength(const rvn_overlap& o) {
   return a > b ? a : b;  // overlap_utils.cc:10-12
 }
 
-__global__ void RhsKeys(const rvn_overlap* __restrict__ ovl, uint32_t m,
+__global__ void RhsKeys(const rvn_overlap* __restrict__ ovl, uint32_t m, Window w,
                         uint32_t* __restrict__ key, uint32_t* __restrict__ idx,
                         uint32_t* __restrict__ rhs_cnt) {
   const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= m) return;
-  const uint32_t r = ovl[e].rhs_id;
+  const uint32_t r = w.Slot(ovl[e].rhs_id);
   key[e] = r;
   idx[e] = e;
   atomicAdd(&rhs_cnt[r], 1u);
 }
 
-// total[r] = kept so far + new records as rhs + new records as lhs (query block)
+// total[s] = kept so far + new records as rhs + new records as lhs (query block)
+// of the read in slot s
 __global__ void ListTotals(const uint32_t* __restrict__ old_cnt,
                            const uint32_t* __restrict__ rhs_cnt,
                            const uint64_t* __restrict__ q_ovl_off, uint32_t k0,
-                           uint32_t k1, uint32_t n, uint32_t mod, uint32_t rem,
+                           uint32_t k1, Window w, uint32_t mod, uint32_t rem,
                            uint32_t* __restrict__ total) {
-  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= n) return;
+  const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= w.size()) return;
+  const uint32_t r = w.Id(s);
   if (r % mod != rem) {  // not this context's read: its list stays empty
-    total[r] = old_cnt[r];
+    total[s] = old_cnt[s];
     return;
   }
   uint32_t lhs = 0;
   if (r >= k0 && r < k1) {
     lhs = static_cast<uint32_t>(q_ovl_off[r - k0 + 1] - q_ovl_off[r - k0]);
   }
-  total[r] = old_cnt[r] + rhs_cnt[r] + lhs;
+  total[s] = old_cnt[s] + rhs_cnt[s] + lhs;
 }
 
 // one warp per read: carry the kept records over into the staging list
@@ -87,13 +89,13 @@ __global__ void PlaceRhs(const rvn_overlap* __restrict__ ovl,
                          const uint32_t* __restrict__ sorted_idx, uint32_t m,
                          const uint64_t* __restrict__ rhs_off,
                          const uint32_t* __restrict__ old_cnt,
-                         const uint64_t* __restrict__ t_off, uint32_t mod, uint32_t rem,
-                         rvn_overlap* __restrict__ stage) {
+                         const uint64_t* __restrict__ t_off, Window w, uint32_t mod,
+                         uint32_t rem, rvn_overlap* __restrict__ stage) {
   const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= m) return;
   const rvn_overlap o = ovl[sorted_idx[p]];
-  const uint32_t r = o.rhs_id;
-  if (r % mod != rem) return;
+  if (o.rhs_id % mod != rem) return;
+  const uint32_t r = w.Slot(o.rhs_id);
   const uint64_t rank = p - rhs_off[r];
   stage[t_off[r] + old_cnt[r] + rank] = ReverseOverlap(o);
 }
@@ -102,14 +104,14 @@ __global__ void PlaceLhs(const rvn_overlap* __restrict__ ovl, uint32_t m,
                          const uint64_t* __restrict__ q_ovl_off, uint32_t k0,
                          const uint32_t* __restrict__ rhs_cnt,
                          const uint32_t* __restrict__ old_cnt,
-                         const uint64_t* __restrict__ t_off, uint32_t mod, uint32_t rem,
-                         rvn_overlap* __restrict__ stage) {
+                         const uint64_t* __restrict__ t_off, Window w, uint32_t mod,
+                         uint32_t rem, rvn_overlap* __restrict__ stage) {
   const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= m) return;
   const rvn_overlap o = ovl[e];
-  const uint32_t r = o.lhs_id;
-  if (r % mod != rem) return;
-  const uint64_t rank = e - q_ovl_off[r - k0];
+  if (o.lhs_id % mod != rem) return;
+  const uint32_t r = w.Slot(o.lhs_id);
+  const uint64_t rank = e - q_ovl_off[o.lhs_id - k0];
   stage[t_off[r] + old_cnt[r] + rhs_cnt[r] + rank] = o;
 }
 
@@ -172,10 +174,12 @@ void GatherReset(Ctx& c) {
 
 // one flush of the reference's gather: `ovl` holds the m64 overlaps mapped for
 // the queries [k0, k1) in query order, q_ovl_off their per-query offsets
-// (relative to ovl, k1 - k0 + 1 entries); both on the device
+// (relative to ovl, k1 - k0 + 1 entries); both on the device. Every read an
+// overlap names lies in the window `w`; the lists of its reads are indexed by slot.
 void GatherFlush(Ctx& c, const rvn_overlap* ovl, const uint64_t* q_ovl_off,
-                 uint64_t m64, uint32_t k0, uint32_t k1, uint64_t kmax) {
-  const uint32_t n = c.n_reads;
+                 uint64_t m64, uint32_t k0, uint32_t k1, uint64_t kmax, const Window& w,
+                 const uint64_t* row_off, uint64_t row_stride) {
+  const uint32_t n = w.size();
   if (m64 == 0) return;
   if (m64 >= 0xFFFFFFFFULL) throw LimitError("2^32 or more overlaps in one flush");
   const uint32_t m = static_cast<uint32_t>(m64);
@@ -188,12 +192,13 @@ void GatherFlush(Ctx& c, const rvn_overlap* ovl, const uint64_t* q_ovl_off,
   uint32_t* rhs_cnt = c.g_rhs_cnt.reserve(n + 1ULL);
   uint64_t* rhs_off = c.g_rhs_off.reserve(n + 2ULL);
   RVN_CUDA(cudaMemsetAsync(rhs_cnt, 0, (n + 1ULL) * sizeof(uint32_t), c.stream));
-  RhsKeys<<<CeilDiv(m, kThreads), kThreads, 0, c.stream>>>(ovl, m, key, idx, rhs_cnt);
+  RhsKeys<<<CeilDiv(m, kThreads), kThreads, 0, c.stream>>>(ovl, m, w, key, idx, rhs_cnt);
   RVN_LAUNCH_CHECK();
   ++c.launches;
   int bits = 1;
   while ((1ULL << bits) < n) ++bits;
-  // stable: records of one rhs read keep their overlap-index order (radix.cu)
+  // stable: records of one rhs read keep their overlap-index order (radix.cu); slots
+  // of the index batch are in read order, and every rhs read is in the batch
   const int w_rhs = RadixSortPairs(c, key, key2, key, idx, idx2, idx, m, 0, bits);
   const uint32_t* sorted_idx = w_rhs == 0 ? idx2 : idx;
   ExclusiveScanU32(c, rhs_cnt, rhs_off, n);
@@ -202,44 +207,77 @@ void GatherFlush(Ctx& c, const rvn_overlap* ovl, const uint64_t* q_ovl_off,
   uint32_t* total = c.g_total_cnt.reserve(n + 1ULL);
   uint64_t* t_off = c.g_t_off.reserve(n + 2ULL);
   ListTotals<<<CeilDiv(n, kThreads), kThreads, 0, c.stream>>>(
-      c.g_cnt.get(), rhs_cnt, q_ovl_off, k0, k1, n, c.own_mod, c.own_rem, total);
+      c.g_cnt.get(), rhs_cnt, q_ovl_off, k0, k1, w, c.own_mod, c.own_rem, total);
   RVN_LAUNCH_CHECK();
   ++c.launches;
   ExclusiveScanU32(c, total, t_off, n);
-  const uint64_t staged = c.g_total + 2ULL * m;  // known without a read-back
+  // known without a read-back: compact lists hold g_total records, rows at most
+  // row_stride per slot
+  const uint64_t staged = (row_off ? n * row_stride : c.g_total) + 2ULL * m;
   rvn_overlap* stage = c.g_stage.reserve(staged + 1);
   uint64_t* pairs = c.g_pairs.reserve(staged + 1);
   uint32_t* kept = c.g_kept.reserve(n + 1ULL);
   const rvn_overlap* lists = c.g_list[c.g_cur].get();
+  const uint64_t* old_off = row_off ? row_off : c.g_off.get();
 
   CopyOld<<<CeilDiv(n, kThreads / 32), kThreads, 0, c.stream>>>(
-      lists, c.g_off.get(), c.g_cnt.get(), t_off, n, stage);
+      lists, old_off, c.g_cnt.get(), t_off, n, stage);
   PlaceRhs<<<CeilDiv(m, kThreads), kThreads, 0, c.stream>>>(
-      ovl, sorted_idx, m, rhs_off, c.g_cnt.get(), t_off, c.own_mod, c.own_rem, stage);
+      ovl, sorted_idx, m, rhs_off, c.g_cnt.get(), t_off, w, c.own_mod, c.own_rem, stage);
   PlaceLhs<<<CeilDiv(m, kThreads), kThreads, 0, c.stream>>>(
-      ovl, m, q_ovl_off, k0, rhs_cnt, c.g_cnt.get(), t_off, c.own_mod, c.own_rem, stage);
+      ovl, m, q_ovl_off, k0, rhs_cnt, c.g_cnt.get(), t_off, w, c.own_mod, c.own_rem, stage);
   Truncate<<<CeilDiv(n, 128), 128, 0, c.stream>>>(stage, t_off, total,
                                                    c.g_cnt.get(), n, kmax, pairs,
                                                    kept);
   RVN_LAUNCH_CHECK();
   c.launches += 4;
 
-  uint64_t* new_off = c.g_off_alt.reserve(n + 2ULL);
-  ExclusiveScanU32(c, kept, new_off, n);
-  const uint64_t new_total = ReadU64(c, new_off + n);
-  rvn_overlap* next = c.g_list[c.g_cur ^ 1].reserve(new_total + 1);
-  Compact<<<CeilDiv(n, kThreads / 32), kThreads, 0, c.stream>>>(
-      stage, t_off, total, c.g_cnt.get(), kept, pairs, kmax, new_off, n, next);
-  RVN_LAUNCH_CHECK();
-  ++c.launches;
+  if (row_off) {
+    // every list goes back to its row (the caller sized both list buffers)
+    Compact<<<CeilDiv(n, kThreads / 32), kThreads, 0, c.stream>>>(
+        stage, t_off, total, c.g_cnt.get(), kept, pairs, kmax, row_off, n,
+        c.g_list[c.g_cur ^ 1].get());
+    RVN_LAUNCH_CHECK();
+    ++c.launches;
+  } else {
+    uint64_t* new_off = c.g_off_alt.reserve(n + 2ULL);
+    ExclusiveScanU32(c, kept, new_off, n);
+    const uint64_t new_total = ReadU64(c, new_off + n);
+    rvn_overlap* next = c.g_list[c.g_cur ^ 1].reserve(new_total + 1);
+    Compact<<<CeilDiv(n, kThreads / 32), kThreads, 0, c.stream>>>(
+        stage, t_off, total, c.g_cnt.get(), kept, pairs, kmax, new_off, n, next);
+    RVN_LAUNCH_CHECK();
+    ++c.launches;
+    c.g_off.swap(c.g_off_alt);
+    c.g_total = new_total;
+  }
   // the new lists become current
   c.g_cur ^= 1;
-  std::swap(c.g_off.p, c.g_off_alt.p);
-  std::swap(c.g_off.cap, c.g_off_alt.cap);
-  std::swap(c.g_cnt.p, c.g_kept.p);
-  std::swap(c.g_cnt.cap, c.g_kept.cap);
-  c.g_total = new_total;
+  c.g_cnt.swap(c.g_kept);
   TimerEnd(c);
+}
+
+namespace {
+
+__global__ void WindowTablesKernel(Window w, const uint64_t* __restrict__ poff,
+                                   uint64_t stride, uint64_t* __restrict__ row_off,
+                                   uint64_t* __restrict__ pile_off) {
+  const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s > w.size()) return;
+  const uint32_t nb = w.b1 - w.b0;
+  row_off[s] = s * stride;
+  pile_off[s] = s <= nb ? poff[w.b0 + s] - poff[w.b0]
+                        : (poff[w.b1] - poff[w.b0]) + (poff[w.a0 + (s - nb)] - poff[w.a0]);
+}
+
+}  // namespace
+
+void WindowTables(Ctx& c, const Window& w, const uint64_t* d_poff, uint64_t stride,
+                  uint64_t* row_off, uint64_t* pile_off) {
+  WindowTablesKernel<<<CeilDiv(w.size() + 1ULL, kThreads), kThreads, 0, c.stream>>>(
+      w, d_poff, stride, row_off, pile_off);
+  RVN_LAUNCH_CHECK();
+  ++c.launches;
 }
 
 void GatherFetch(Ctx& c) {

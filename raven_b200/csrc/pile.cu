@@ -7,43 +7,45 @@
 // with a shuffle scan and adds it to the uint16 bins, saturating at 65535.
 // The running coverage is kept modulo 2^32 exactly like the reference's
 // unsigned counter, so the result is bit-identical (DESIGN.md).
+#include <algorithm>
+
 #include "engine.cuh"
 
 namespace rvn {
 
 namespace {
 
-__global__ void ScatterMarks(const rvn_overlap* __restrict__ ovl, uint64_t n,
-                             const uint64_t* __restrict__ bin_off,
-                             uint32_t n_piles, uint32_t mod, uint32_t rem,
-                             int32_t* __restrict__ diff) {
-  const uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const rvn_overlap o = ovl[i];
-  // pile p owns diff[bin_off[p] + p .. bin_off[p+1] + p]  (bins + 1 slots);
-  // only the piles this context owns (p % mod == rem) are maintained
-  if (o.lhs_id < n_piles && o.lhs_id % mod == rem) {
-    const uint64_t base = bin_off[o.lhs_id] + o.lhs_id;
-    const uint64_t bins = bin_off[o.lhs_id + 1] - bin_off[o.lhs_id];
-    const uint32_t b = (o.lhs_begin >> 4) + 1, e = (o.lhs_end >> 4) - 1;
-    if (b <= bins && e <= bins) {
-      atomicAdd(diff + base + b, 1);
-      atomicAdd(diff + base + e, -1);
-    }
-  }
-  if (o.rhs_id < n_piles && o.rhs_id % mod == rem) {
-    const uint64_t base = bin_off[o.rhs_id] + o.rhs_id;
-    const uint64_t bins = bin_off[o.rhs_id + 1] - bin_off[o.rhs_id];
-    const uint32_t b = (o.rhs_begin >> 4) + 1, e = (o.rhs_end >> 4) - 1;
-    if (b <= bins && e <= bins) {
-      atomicAdd(diff + base + b, 1);
-      atomicAdd(diff + base + e, -1);
-    }
+__device__ __forceinline__ void AddMarks(uint32_t id, uint32_t begin, uint32_t end,
+                                         const uint64_t* __restrict__ bin_off, Window w,
+                                         uint32_t mod, uint32_t rem,
+                                         int32_t* __restrict__ diff) {
+  if (id % mod != rem) return;
+  const uint32_t p = w.Slot(id);
+  if (p >= w.size()) return;
+  const uint64_t base = bin_off[p] + p;
+  const uint64_t bins = bin_off[p + 1] - bin_off[p];
+  const uint32_t b = (begin >> 4) + 1, e = (end >> 4) - 1;
+  if (b <= bins && e <= bins) {
+    atomicAdd(diff + base + b, 1);
+    atomicAdd(diff + base + e, -1);
   }
 }
 
+// pile of slot p owns diff[bin_off[p] + p .. bin_off[p+1] + p]  (bins + 1 slots);
+// only the piles this context owns (id % mod == rem) are maintained
+__global__ void ScatterMarks(const rvn_overlap* __restrict__ ovl, uint64_t n,
+                             const uint64_t* __restrict__ bin_off, Window w,
+                             uint32_t mod, uint32_t rem, int32_t* __restrict__ diff) {
+  const uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const rvn_overlap o = ovl[i];
+  AddMarks(o.lhs_id, o.lhs_begin, o.lhs_end, bin_off, w, mod, rem, diff);
+  AddMarks(o.rhs_id, o.rhs_begin, o.rhs_end, bin_off, w, mod, rem, diff);
+}
+
 // one warp per pile: inclusive scan of the differences, saturating add,
-// and the differences are cleared for the next call
+// and the differences are cleared for the next call (piles by slot: a window
+// other than all reads is only used with mod == 1)
 __global__ void __launch_bounds__(256)
 ApplyCoverage(uint16_t* __restrict__ data, const uint64_t* __restrict__ bin_off,
               uint32_t n_piles, uint32_t mod, uint32_t rem, int32_t* __restrict__ diff) {
@@ -77,25 +79,25 @@ ApplyCoverage(uint16_t* __restrict__ data, const uint64_t* __restrict__ bin_off,
 
 }  // namespace
 
-void PileAddLayersDevice(Ctx& c, uint16_t* d_data, const uint64_t* d_off,
-                         const uint64_t* h_off, uint32_t n_piles,
-                         const rvn_overlap* d_ovl, uint64_t n_ovl) {
+void PileAddLayersDevice(Ctx& c, uint16_t* d_data, const uint64_t* d_off, uint64_t bins,
+                         const Window& w, const rvn_overlap* d_ovl, uint64_t n_ovl) {
+  const uint32_t n_piles = w.size();
   if (n_piles == 0 || n_ovl == 0) return;
-  const uint64_t slots = h_off[n_piles] + n_piles;
+  const uint64_t slots = bins + n_piles;
   if (c.p_diff.cap < slots) {
     int32_t* d = c.p_diff.reserve(slots);
     RVN_CUDA(cudaMemsetAsync(d, 0, c.p_diff.cap * sizeof(int32_t), c.stream));
   }
   TimerBegin(c, "pile");
   ScatterMarks<<<CeilDiv(n_ovl, 256), 256, 0, c.stream>>>(
-      d_ovl, n_ovl, d_off, n_piles, c.own_mod, c.own_rem, c.p_diff.get());
+      d_ovl, n_ovl, d_off, w, c.own_mod, c.own_rem, c.p_diff.get());
   const uint32_t owned = CeilDiv(n_piles, c.own_mod);
   ApplyCoverage<<<CeilDiv(owned, 8), 256, 0, c.stream>>>(d_data, d_off, n_piles, c.own_mod,
                                                          c.own_rem, c.p_diff.get());
   RVN_LAUNCH_CHECK();
   c.launches += 2;
   TimerEnd(c);
-  c.stats.pile_bins += h_off[n_piles];
+  c.stats.pile_bins += bins;
 }
 
 }  // namespace rvn
@@ -185,12 +187,12 @@ __global__ void KmerComplexityKernel(const uint64_t* __restrict__ words,
 // largest r with #{x < r} <= size / 2, found bit by bit.
 __global__ void __launch_bounds__(128)
 PileRegionsKernel(const uint16_t* __restrict__ data, const uint64_t* __restrict__ off,
-                  uint32_t n_piles, uint32_t coverage, uint32_t* __restrict__ out_begin,
-                  uint32_t* __restrict__ out_end, uint16_t* __restrict__ out_median,
-                  uint8_t* __restrict__ out_invalid) {
+                  uint64_t off_base, uint32_t n_piles, uint32_t coverage,
+                  uint32_t* __restrict__ out_begin, uint32_t* __restrict__ out_end,
+                  uint16_t* __restrict__ out_median, uint8_t* __restrict__ out_invalid) {
   const uint32_t p = (blockIdx.x * 128 + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (p >= n_piles) return;
-  const uint16_t* d = data + off[p];
+  const uint16_t* d = data + (off[p] - off_base);
   const uint32_t nb = static_cast<uint32_t>(off[p + 1] - off[p]);
   uint32_t begin = 0, end = 0;
   long long run = -1;  // start of the run the scan is in
@@ -262,10 +264,12 @@ void KmerComplexity(Ctx& c, const uint32_t* h_read_idx, const uint32_t* h_pos,
   RVN_CUDA(cudaStreamSynchronize(c.stream));
 }
 
-// valid regions and medians of the piles the last stage-1 call left on the device
+// valid regions and medians of the piles of the last stage-1 call: on the device
+// after a resident run; after a windowed run they are on the host and pass
+// through the device in chunks of reads
 void StagePileRegions(Ctx& c, uint32_t coverage, uint32_t* h_begin, uint32_t* h_end,
                       uint16_t* h_median, uint8_t* h_invalid) {
-  if (!c.st_valid || !c.st_piles_on_device) {
+  if (!c.st_valid || !(c.st_piles_on_device || c.st_windowed)) {
     throw StateError("no stage-1 piles on the device (run rvn_find_overlaps_and_create_piles first)");
   }
   const uint32_t n = c.n_reads;
@@ -275,10 +279,31 @@ void StagePileRegions(Ctx& c, uint32_t coverage, uint32_t* h_begin, uint32_t* h_
   uint16_t* d_m = reinterpret_cast<uint16_t*>(c.m_first.reserve(n / 2 + 2));
   uint8_t* d_i = c.m_filt.reserve(n + 1ULL);
   TimerBegin(c, "pile_regions");
-  PileRegionsKernel<<<CeilDiv(n, 4), 128, 0, c.stream>>>(c.p_data.get(), c.p_off.get(), n, coverage,
-                                                       d_b, d_e, d_m, d_i);
-  RVN_LAUNCH_CHECK();
-  ++c.launches;
+  if (c.st_piles_on_device) {
+    PileRegionsKernel<<<CeilDiv(n, 4), 128, 0, c.stream>>>(c.p_data.get(), c.p_off.get(), 0, n,
+                                                         coverage, d_b, d_e, d_m, d_i);
+    RVN_LAUNCH_CHECK();
+    ++c.launches;
+  } else {
+    const std::vector<uint64_t>& off = c.st_pile_off;
+    uint64_t* d_off = c.p_off.reserve(n + 1ULL);
+    RVN_CUDA(cudaMemcpyAsync(d_off, off.data(), (n + 1ULL) * 8, cudaMemcpyHostToDevice,
+                             c.stream));
+    // chunks as large as the window pile buffer of the run (one read at least)
+    const uint64_t cap = std::max<uint64_t>(c.p_data.cap, 1) - 1;
+    for (uint32_t r0 = 0, r1; r0 < n; r0 = r1) {
+      r1 = r0 + 1;
+      while (r1 < n && off[r1 + 1] - off[r0] <= cap) ++r1;
+      const uint64_t bins = off[r1] - off[r0];
+      uint16_t* d = c.p_data.reserve(bins + 1);
+      RVN_CUDA(cudaMemcpyAsync(d, c.st_pile.get() + off[r0], bins * 2, cudaMemcpyHostToDevice,
+                               c.stream));
+      PileRegionsKernel<<<CeilDiv(r1 - r0, 4), 128, 0, c.stream>>>(
+          d, d_off + r0, off[r0], r1 - r0, coverage, d_b + r0, d_e + r0, d_m + r0, d_i + r0);
+      RVN_LAUNCH_CHECK();
+      ++c.launches;
+    }
+  }
   TimerEnd(c);
   RVN_CUDA(cudaMemcpyAsync(h_begin, d_b, n * 4ULL, cudaMemcpyDeviceToHost, c.stream));
   RVN_CUDA(cudaMemcpyAsync(h_end, d_e, n * 4ULL, cudaMemcpyDeviceToHost, c.stream));

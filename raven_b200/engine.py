@@ -280,6 +280,27 @@ class Engine:
     def set_option(self, name, value):
         self._check(self.lib.rvn_set_option(self.h, name.encode(), int(value)))
 
+    def set_stage1_window(self, mode=-1, budget=0):
+        """Where find_overlaps_and_create_piles keeps the piles and overlap lists of all
+        reads: 0 on the device, 1 windowed (on the host; each flush brings the reads it
+        touches to the device), -1 auto (windowed only when the resident estimate exceeds
+        the free device memory, or ``budget`` bytes when that is not 0). Same results."""
+        self.set_option("stage1_window", mode)
+        self.set_option("stage1_window_budget", budget)
+
+    def stage1_footprint(self, max_overlaps=32, index_batch_bases=0, query_batch_bases=0):
+        """The auto mode's estimates for a stage-1 call over the uploaded reads, in bytes:
+        resident (device), windowed_device and windowed_host (pinned)."""
+        r, d, h = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        self._check(self.lib.rvn_stage1_footprint(
+            self.h, max_overlaps, index_batch_bases, query_batch_bases, C.byref(r),
+            C.byref(d), C.byref(h)))
+        return dict(resident=r.value, windowed_device=d.value, windowed_host=h.value)
+
+    def stage1_windowed(self):
+        """Whether the last stage-1 call ran windowed (phase "stage1_window" in its timings)."""
+        return "stage1_window" in self.timings()
+
     def stats(self):
         s = Stats()
         self._check(self.lib.rvn_get_stats(self.h, C.byref(s)))
