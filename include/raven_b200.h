@@ -221,6 +221,14 @@ int rvn_stage1_footprint(rvn_ctx* ctx, uint64_t max_overlaps, uint64_t index_bat
                          uint64_t query_batch_bases, uint64_t* resident,
                          uint64_t* windowed_device, uint64_t* windowed_host);
 
+/* The device working set of the largest index batch of a stage-1 call over the uploaded
+ * reads with index batches of index_batch_bases (0 = 2^32), in bytes: built in one piece,
+ * and built in chunks (option "index_chunk_bases": its chunk size when it is > 0, else
+ * 2^30 bases). The estimates of rvn_stage1_footprint use the chunked one when the call
+ * would chunk. */
+int rvn_index_footprint(rvn_ctx* ctx, uint64_t index_batch_bases, uint64_t* one_shot,
+                        uint64_t* chunked);
+
 /* raven::FindOverlapsAndCreatePiles over the uploaded read set: index batches
  * of >= index_batch_bases (reference: 1<<32), query flushes of >=
  * query_batch_bases (reference: 1<<30); pass 0 for the reference values.
@@ -303,7 +311,17 @@ int rvn_get_stats(rvn_ctx* ctx, rvn_stats* out);
  * (rvn_stage1_footprint), else resident. Results are identical in every
  * mode; a windowed pass takes max_overlaps <= 65536 and leaves phase
  * "stage1_window" in rvn_get_timings); "stage1_window_budget" (bytes: replaces the
- * free device memory in the auto decision, 0 = the free memory); "reset_stats".
+ * free device memory in the auto decision, 0 = the free memory); "index_chunk_bases"
+ * (how rvn_find_overlaps_and_create_piles builds each index batch: 0 = in one piece,
+ * with a sketch of the whole batch; N > 0 = in chunks of reads of >= N bases, cut like
+ * the index batches: each chunk is sketched twice, once for its micromizer thresholds and
+ * once for its records, which go straight into the index's tiers, and the build's buffers
+ * are freed before the first flush; -1 = auto, the default: chunks of 2^30 bases only
+ * when the one-shot pass fits neither resident nor windowed, else one piece. Results
+ * are identical in every mode; a chunked call leaves phase "sketch_tiers" in
+ * rvn_get_timings; with "async_upload" a chunked build first waits for the whole
+ * upload); "index_chunk_budget" (bytes: replaces the free device memory in that auto
+ * decision, 0 = the free memory); "reset_stats".
  * Unknown name or value out of range -> RVN_ERR_INVALID. */
 int rvn_set_option(rvn_ctx* ctx, const char* name, int64_t value);
 

@@ -13,8 +13,9 @@ memory in use after the call.
    genome sized to match; 0 skips it) with index batches of --large-ib bases, one pass
    without warm-up (it includes the first allocation of the pinned host state). The
    resident mode is not run there; the script prints the auto mode's estimates
-   (rvn_stage1_footprint) of what each mode would need. (One C2 pass holds about 44 GB for its 1.98 Gbp index batch, so the
-   default 2^32-base batch does not fit on an 80 GB card in either mode.)
+   (rvn_stage1_footprint) of what each mode would need. (One C2 pass holds about 44 GB for
+   its 1.98 Gbp index batch built in one piece, so the default 2^32-base batch fits an 80 GB
+   card only built in chunks - option "index_chunk_bases", profiles/index_chunks.py.)
 
 Needs an H100; prints the card's name and power limit with the numbers. --out DIR also
 writes them as DIR/stage1_window.json.

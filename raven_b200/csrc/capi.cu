@@ -107,6 +107,45 @@ constexpr uint64_t kWindowMaxOverlaps = 1ULL << 16;
 // self-join slots, one flush's hits, with the buffers' headroom) per base of the
 // batch: a C2 pass (one 1.98 Gbp batch) holds 43.6 GB in all (DESIGN.md §3, §5).
 constexpr double kBatchBytesPerBase = 21.0;
+// The same for a chunked build (BuildIndexChunked), from the per-buffer breakdown of a C2
+// pass (DESIGN.md §3), as three parts that grow with different sizes:
+// - per base of the batch: the index the flushes probe (i_val, i_org, i_bucket, j_packed:
+//   1.8 B) and the build's sort buffers and bare keys, freed before the flushes but held
+//   next to the flush buffers of an earlier batch or pass (i_*_alt, t_b0, t_b1: 3.3 B);
+// - per base of one chunk: its sketch in sweep 1 (s_val, s_org: 4.7 B);
+// - per query base of the largest flush: the flush's hits, chain scratch and overlaps,
+//   and on the probe path its queries' sketch and sorted micromizers. 27 B is the
+//   remainder of the 59.9 GB peak of a 2^32-base batch with 2^30-base query flushes
+//   (DESIGN.md §5); C2's join-only flushes hold 18.4 B.
+constexpr double kIndexBytesPerBase = 1.8 + 3.3;
+constexpr double kChunkSketchBytesPerBase = 4.7;
+constexpr double kFlushBytesPerBase = 27.0;
+// chunk size of option "index_chunk_bases" -1 (auto)
+constexpr uint64_t kAutoIndexChunk = 1ULL << 30;
+
+// Device working set of the largest index batch, one-shot (chunk 0) or in chunks of
+// `chunk` bases.
+double IndexFootprint(const Ctx& c, const std::vector<Batch>& batches, uint64_t chunk) {
+  uint64_t batch_bases = 0, flush_bases = 0;
+  for (const Batch& b : batches) {
+    uint64_t bases = 0;
+    for (uint32_t r = b.j; r < b.end; ++r) bases += c.h_len[r];
+    batch_bases = std::max(batch_bases, bases);
+    for (const auto& f : b.flushes) {
+      uint64_t q = 0;
+      for (uint32_t r = f.first; r < f.second; ++r) q += c.h_len[r];
+      flush_bases = std::max(flush_bases, q);
+    }
+  }
+  const double bb = static_cast<double>(batch_bases);
+  const double one_shot = kBatchBytesPerBase * bb;
+  if (chunk == 0) return one_shot;
+  // (a chunked build holds a subset of the one-shot build's buffers: below a few Gbp
+  // the flush's working set dominates and chunks save little)
+  return std::min(one_shot, kIndexBytesPerBase * bb +
+                                kChunkSketchBytesPerBase * std::min(bb, static_cast<double>(chunk)) +
+                                kFlushBytesPerBase * static_cast<double>(flush_bases));
+}
 
 // Estimated memory of a stage-1 pass over the uploaded reads, in bytes.
 struct Footprint {
@@ -126,18 +165,15 @@ struct Footprint {
 //   (at least 1) records per list row; on the host: the rows, counts and piles of
 //   all reads.
 // off: pile offsets of the reads (len >> 4 bins each, n + 1 entries)
+// chunk: the index build's chunk size (0: one-shot), see IndexFootprint
 Footprint Stage1Footprint(const Ctx& c, const std::vector<uint64_t>& off,
-                          const std::vector<Batch>& batches, uint64_t kmax) {
+                          const std::vector<Batch>& batches, uint64_t kmax, uint64_t chunk) {
   const uint32_t n = c.n_reads;
   const double bins = static_cast<double>(off[n]);
   const double stride = static_cast<double>(std::max<uint64_t>(kmax, 1));
   const double list_bytes = 3.0 * sizeof(rvn_overlap) + 8.0;  // per record
-  uint64_t batch_bases = 0;
   double window = 0;  // device bytes of the largest window
   for (const Batch& b : batches) {
-    uint64_t bases = 0;
-    for (uint32_t r = b.j; r < b.end; ++r) bases += c.h_len[r];
-    batch_bases = std::max(batch_bases, bases);
     for (const auto& f : b.flushes) {
       const uint32_t a0 = std::min(f.first, b.j), a1 = std::min(f.second, b.j);
       const double slots = (b.end - b.j) + (a1 - a0);
@@ -145,7 +181,7 @@ Footprint Stage1Footprint(const Ctx& c, const std::vector<uint64_t>& off,
       window = std::max(window, 6.0 * wbins + 4.0 * slots + slots * stride * list_bytes);
     }
   }
-  const double reads = 8.0 * c.n_words + 32.0 * n + kBatchBytesPerBase * batch_bases;
+  const double reads = 8.0 * c.n_words + 32.0 * n + IndexFootprint(c, batches, chunk);
   const double kept = std::min(static_cast<double>(kmax), n > 0 ? n - 1.0 : 0.0);
   Footprint f;
   f.resident = reads + 6.0 * bins + 4.0 * n + n * kept * list_bytes;
@@ -154,23 +190,38 @@ Footprint Stage1Footprint(const Ctx& c, const std::vector<uint64_t>& off,
   return f;
 }
 
+// device memory a pass can use: `budget`, or when that is 0 the free memory plus the
+// buffers this context already holds (a pass re-uses them)
+double UsableMemory(const Ctx& c, uint64_t budget) {
+  if (budget) return static_cast<double>(budget);
+  size_t free_b = 0, total_b = 0;
+  RVN_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  return static_cast<double>(free_b) + static_cast<double>(c.held_bytes);
+}
+
+// Option "index_chunk_bases": the chunk size of the pass's index builds, 0 = one-shot.
+// -1 (auto): chunks of kAutoIndexChunk bases only when the one-shot pass fits neither
+// resident nor windowed (max_overlaps permitting) in the usable memory
+// ("index_chunk_budget" replaces it when it is not 0).
+uint64_t IndexChunk(const Ctx& c, const std::vector<uint64_t>& off,
+                    const std::vector<Batch>& batches, uint64_t kmax) {
+  if (c.index_chunk_bases >= 0) return static_cast<uint64_t>(c.index_chunk_bases);
+  const Footprint f = Stage1Footprint(c, off, batches, kmax, 0);
+  double one_shot = f.resident;
+  if (kmax <= kWindowMaxOverlaps) one_shot = std::min(one_shot, f.windowed_device);
+  return one_shot > UsableMemory(c, c.index_chunk_budget) ? kAutoIndexChunk : 0;
+}
+
 // Option "stage1_window" -1 (auto): windowed only when the resident estimate exceeds
-// the device memory a pass can use and the windowed pass itself fits: it takes
-// kmax, its own device estimate fits the same memory and its host rows fit the
-// host's free physical memory. Otherwise resident, as before the option existed.
-// Usable device memory: the free memory plus the buffers this context already
-// holds, since a pass re-uses them ("stage1_window_budget" replaces both when it is
-// not 0).
-bool UseWindow(Ctx& c, const std::vector<Batch>& batches, uint64_t kmax) {
+// the usable device memory ("stage1_window_budget" replaces it when it is not 0) and the
+// windowed pass itself fits: it takes kmax, its own device estimate fits the same memory
+// and its host rows fit the host's free physical memory. Otherwise resident, as before
+// the option existed.
+bool UseWindow(Ctx& c, const std::vector<Batch>& batches, uint64_t kmax, uint64_t chunk) {
   if (c.stage1_window >= 0) return c.stage1_window != 0;
   if (kmax > kWindowMaxOverlaps) return false;
-  const Footprint f = Stage1Footprint(c, c.st_pile_off, batches, kmax);
-  double budget = static_cast<double>(c.stage1_window_budget);
-  if (budget == 0) {
-    size_t free_b = 0, total_b = 0;
-    RVN_CUDA(cudaMemGetInfo(&free_b, &total_b));
-    budget = static_cast<double>(free_b) + static_cast<double>(c.held_bytes);
-  }
+  const Footprint f = Stage1Footprint(c, c.st_pile_off, batches, kmax, chunk);
+  const double budget = UsableMemory(c, c.stage1_window_budget);
   if (f.resident <= budget) return false;
   const double host_free = static_cast<double>(sysconf(_SC_AVPHYS_PAGES)) *
                            static_cast<double>(sysconf(_SC_PAGESIZE));
@@ -329,7 +380,8 @@ void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
   }
   const uint64_t total_bins = c.st_pile_off[n];
   const std::vector<Batch> batches = Schedule(c, ib, qb);
-  const bool windowed = UseWindow(c, batches, kmax);
+  const uint64_t chunk = IndexChunk(c, c.st_pile_off, batches, kmax);
+  const bool windowed = UseWindow(c, batches, kmax, chunk);
   c.st_windowed = false;
   uint16_t* d_pile = nullptr;
   if (!windowed) {
@@ -352,13 +404,19 @@ void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
     // Queries are micromizers only (construct.cc:62): no record above the largest
     // micromizer value of any read so far can be hit - those are counted for the
     // occurrence threshold but stay out of the index (index.cu, tiers)
-    uint64_t limit = ~0ULL;
-    if (!minhash) {
-      tmax = std::max(tmax, MaxMicromizerValue(c, b.j, b.end));
-      limit = tmax;
+    if (chunk) {
+      tmax = BuildIndexChunked(c, b.j, b.end, minhash, chunk, tmax);
+      FilterIndex(c, freq);
+      ReleaseIndexBuild(c);
+    } else {
+      uint64_t limit = ~0ULL;
+      if (!minhash) {
+        tmax = std::max(tmax, MaxMicromizerValue(c, b.j, b.end));
+        limit = tmax;
+      }
+      BuildIndex(c, b.j, b.end, minhash, limit);
+      FilterIndex(c, freq);
     }
-    BuildIndex(c, b.j, b.end, minhash, limit);
-    FilterIndex(c, freq);
     if (win) win->BeginBatch(b);
 
     for (const auto& f : b.flushes) {
@@ -797,13 +855,26 @@ RVN_API int rvn_stage1_footprint(rvn_ctx* ctx, uint64_t max_overlaps,
     const uint32_t n = c.n_reads;
     std::vector<uint64_t> off(n + 1ULL, 0);
     for (uint32_t i = 0; i < n; ++i) off[i + 1] = off[i] + (c.h_len[i] >> 4);
-    const Footprint f = Stage1Footprint(
-        c, off, Schedule(c, index_batch_bases ? index_batch_bases : 1ULL << 32,
-                         query_batch_bases ? query_batch_bases : 1ULL << 30),
-        max_overlaps);
+    const std::vector<Batch> batches =
+        Schedule(c, index_batch_bases ? index_batch_bases : 1ULL << 32,
+                 query_batch_bases ? query_batch_bases : 1ULL << 30);
+    const Footprint f = Stage1Footprint(c, off, batches, max_overlaps,
+                                        IndexChunk(c, off, batches, max_overlaps));
     if (resident) *resident = static_cast<uint64_t>(f.resident);
     if (windowed_device) *windowed_device = static_cast<uint64_t>(f.windowed_device);
     if (windowed_host) *windowed_host = static_cast<uint64_t>(f.windowed_host);
+  }, /*sketches_first=*/true);
+}
+
+RVN_API int rvn_index_footprint(rvn_ctx* ctx, uint64_t index_batch_bases, uint64_t* one_shot,
+                                uint64_t* chunked) {
+  return Guard(ctx, [&](Ctx& c) {
+    const std::vector<Batch> batches =
+        Schedule(c, index_batch_bases ? index_batch_bases : 1ULL << 32, 1ULL << 30);
+    const uint64_t chunk =
+        c.index_chunk_bases > 0 ? static_cast<uint64_t>(c.index_chunk_bases) : kAutoIndexChunk;
+    if (one_shot) *one_shot = static_cast<uint64_t>(IndexFootprint(c, batches, 0));
+    if (chunked) *chunked = static_cast<uint64_t>(IndexFootprint(c, batches, chunk));
   }, /*sketches_first=*/true);
 }
 
@@ -1024,6 +1095,12 @@ RVN_API int rvn_set_option(rvn_ctx* ctx, const char* name, int64_t value) {
       c.stage1_window = value;
     } else if (name && std::strcmp(name, "stage1_window_budget") == 0) {
       c.stage1_window_budget = value < 0 ? 0 : static_cast<uint64_t>(value);
+    } else if (name && std::strcmp(name, "index_chunk_bases") == 0) {
+      if (value < -1) throw InvalidArgument("index_chunk_bases: -1 (auto), 0 or a chunk size");
+      c.index_chunk_bases = value;
+    } else if (name && std::strcmp(name, "index_chunk_budget") == 0) {
+      if (value < 0) throw InvalidArgument("index_chunk_budget: bytes, 0 = the free memory");
+      c.index_chunk_budget = static_cast<uint64_t>(value);
     } else if (name && std::strcmp(name, "reset_stats") == 0) {
       std::memset(&c.stats, 0, sizeof(c.stats));
       c.launches = 0;

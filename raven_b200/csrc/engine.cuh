@@ -136,6 +136,14 @@ struct Ctx {
   int bare_cluster = 0;         // cluster size of BareCountKernel on this device (0: not chosen)
   int bare_clusters = 0;        // clusters of that size resident at once
   uint64_t tier_min_records = 1ULL << 18;  // smaller index batches are not worth a partition
+  DevBuf<uint64_t> t_hist;  // chunked build: coarse value histogram (capacity of the tiers)
+  // Chunked build (BuildIndexChunked): the micromizer thresholds and counts of the index
+  // batch [i_first, i_last), kept apart from c.qt_* / c.h_q_off, which the probe-path
+  // flushes of reads before the batch overwrite; valid while jt_gen == i_gen
+  uint64_t jt_gen = 0;
+  DevBuf<uint64_t> jt_val;
+  DevBuf<uint32_t> jt_pos;
+  std::vector<uint64_t> h_jt_off;
   DevBuf<uint32_t> i_bucket;
   int i_bucket_bits = 0;
   DevBuf<uint64_t> i_gaps;  // long empty stretches of the bucket table (index.cu)
@@ -213,6 +221,11 @@ struct Ctx {
   int64_t stage1_window = -1;
   uint64_t stage1_window_budget = 0;
   bool st_windowed = false;  // the last stage-1 call ran windowed
+  // option "index_chunk_bases": -1 (default) chunks of 2^30 bases only when the one-shot
+  // pass does not fit the device ("index_chunk_budget" replaces the free memory when it
+  // is not 0), 0 one-shot index build, N > 0 always chunks of >= N bases
+  int64_t index_chunk_bases = -1;
+  uint64_t index_chunk_budget = 0;
   PinBuf<rvn_overlap> w_rows;  // kmax records per read
   PinBuf<uint32_t> w_cnt;      // kept records per read
   DevBuf<uint64_t> w_pile_off, w_row_off;  // per slot (+1) of the current window
@@ -286,6 +299,16 @@ void EnsureSketch(Ctx& c, uint32_t first, uint32_t last);
 void WaitUpload(Ctx& c);  // the context's stream waits for an asynchronous upload
 void EnsureMicromizers(Ctx& c, uint32_t first, uint32_t last);
 void EnsureThresholds(Ctx& c, uint32_t first, uint32_t last);
+// The sketch records of reads [first, last) straight into the two tiers of an index build
+// (SketchFastKernel's tier-output mode; raven's stage-1 parameters k <= 15, w = 5 only,
+// SketchTiersFused): value <= limit as (value, origin) to a_val / a_org, the others as bare
+// keys to b_val, each in (read, position) order. *n_a / *n_b: the records of each stream;
+// a stream beyond its capacity (cap_a, cap_b) is only counted, and the caller repeats the
+// call with room for all of them.
+bool SketchTiersFused(const Ctx& c);
+void SketchTiers(Ctx& c, uint32_t first, uint32_t last, uint32_t limit, uint32_t* a_val,
+                 uint64_t* a_org, uint64_t cap_a, uint32_t* b_val, uint64_t cap_b,
+                 uint64_t* n_a, uint64_t* n_b);
 
 // ---- index.cu ----
 // value_limit: records whose value exceeds it are counted (occurrence threshold)
@@ -293,6 +316,19 @@ void EnsureThresholds(Ctx& c, uint32_t first, uint32_t last);
 void BuildIndex(Ctx& c, uint32_t first, uint32_t last, bool minhash,
                 uint64_t value_limit = ~0ULL);
 uint64_t MaxMicromizerValue(Ctx& c, uint32_t first, uint32_t last);
+// The same index as BuildIndex(c, first, last, minhash, limit) with limit = the largest of
+// `tmax` and the batch's micromizer values (returned; tmax itself with minhash), built
+// from chunks of reads of >= chunk bases: no sketch of the whole batch is ever held.
+// minhash: one sweep appends each chunk's micromizers to the sort's input. Otherwise
+// sweep 1 sketches each chunk and keeps its thresholds (c.jt_*); sweep 2 sketches it
+// again and appends its records to the sort's input - tiered: split into tier A
+// (c.i_val_alt / c.i_org_alt) and bare keys (c.t_b0), at k <= 15, w = 5 straight from
+// the sketch kernel (SketchTiers).
+uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash,
+                           uint64_t chunk, uint64_t tmax);
+// after the frequency filter of a chunked build: frees what only the build used (the
+// chunk sketch, the sort's second buffers, the tiers' staging and bare keys)
+void ReleaseIndexBuild(Ctx& c);
 // index from device records already in (read, position) order (values as u32
 // or u64, see ValView)
 // count_bare: the bare keys of a tiered build are counted by partition + BareCountKernel

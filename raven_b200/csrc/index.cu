@@ -264,6 +264,28 @@ TierScatterKernel(const uint32_t* __restrict__ val, const uint64_t* __restrict__
   }
 }
 
+// Chunked build: a coarse histogram of the sketch values (top kCapBits key bits) bounds
+// the sizes of both tiers before the limit is known to the chunks
+constexpr int kCapBits = 10;
+constexpr uint32_t kCapBins = 1u << kCapBits;
+
+__global__ void __launch_bounds__(kThreads)
+ValueHistKernel(const uint32_t* __restrict__ val, uint64_t n, int shift,
+                unsigned long long* __restrict__ hist) {
+  __shared__ uint32_t sh[kCapBins];
+  for (uint32_t i = threadIdx.x; i < kCapBins; i += kThreads) sh[i] = 0;
+  __syncthreads();
+  const uint64_t stride = static_cast<uint64_t>(gridDim.x) * kThreads;
+  for (uint64_t i = static_cast<uint64_t>(blockIdx.x) * kThreads + threadIdx.x; i < n;
+       i += stride) {
+    atomicAdd(&sh[(val[i] >> shift) & (kCapBins - 1)], 1u);
+  }
+  __syncthreads();
+  for (uint32_t i = threadIdx.x; i < kCapBins; i += kThreads) {
+    if (sh[i]) atomicAdd(&hist[i], static_cast<unsigned long long>(sh[i]));
+  }
+}
+
 __global__ void MaxU64Kernel(const uint64_t* __restrict__ v, uint64_t n,
                              unsigned long long* __restrict__ out) {
   unsigned long long m = 0;
@@ -598,8 +620,36 @@ void BuildIndex(Ctx& c, uint32_t first, uint32_t last, bool minhash, uint64_t va
   c.i_from_sketch = !minhash;
 }
 
+namespace {
+
+// the build splits a batch into tiers (index.cu, tiers): u32 values, a real limit and
+// an input worth a partition pass
+bool Tiered(const Ctx& c, bool is32, uint64_t value_limit, uint64_t n) {
+  const int key_bits = static_cast<int>(2 * c.prm.k);
+  const uint64_t value_mask = key_bits >= 64 ? ~0ULL : ((1ULL << key_bits) - 1);
+  return is32 && value_limit < value_mask && n >= c.tier_min_records;
+}
+
+// The index of n records. pre_split < 0: the records are src_val / src_org. Otherwise
+// the chunked build has laid them out already: tiered, tier A (pre_split records) in
+// c.i_val_alt / c.i_org_alt and the n - pre_split bare keys in c.t_b0; untiered, all n
+// in c.i_val_alt / c.i_org_alt (= src_val / src_org), the sort's second buffers.
+void BuildIndexImpl(Ctx& c, ValView src_val, const uint64_t* src_org, uint64_t n,
+                    uint64_t index_bases, uint64_t value_limit, bool count_bare,
+                    int64_t pre_split);
+
+}  // namespace
+
 void BuildIndexFrom(Ctx& c, ValView src_val, const uint64_t* src_org, uint64_t n,
                     uint64_t index_bases, uint64_t value_limit, bool count_bare) {
+  BuildIndexImpl(c, src_val, src_org, n, index_bases, value_limit, count_bare, -1);
+}
+
+namespace {
+
+void BuildIndexImpl(Ctx& c, ValView src_val, const uint64_t* src_org, uint64_t n,
+                    uint64_t index_bases, uint64_t value_limit, bool count_bare,
+                    int64_t pre_split) {
   c.i_valid = false;
   c.i_sorted_ids = false;
   c.i_from_sketch = false;
@@ -625,8 +675,7 @@ void BuildIndexFrom(Ctx& c, ValView src_val, const uint64_t* src_org, uint64_t n
 
   const int key_bits = static_cast<int>(2 * c.prm.k);
   const uint64_t value_mask = key_bits >= 64 ? ~0ULL : ((1ULL << key_bits) - 1);
-  // tiers: only for u32 values, a real limit and inputs worth a partition pass
-  const bool tiered = is32 && value_limit < value_mask && n >= c.tier_min_records;
+  const bool tiered = Tiered(c, is32, value_limit, n);
   const uint32_t limit32 = static_cast<uint32_t>(value_limit);
   c.i_limit = tiered ? value_limit : ~0ULL;
   uint64_t n_a = n, n_b = 0;
@@ -640,22 +689,35 @@ void BuildIndexFrom(Ctx& c, ValView src_val, const uint64_t* src_org, uint64_t n
   // bits (k <= 15) are u32 keys straight from the sketch kernel: 12 instead of
   // 16 bytes per record and pass, three 10-bit passes at k = 15.
   if (tiered) {
-    const uint32_t* src32 = static_cast<const uint32_t*>(src_val.p);
-    const uint64_t tiles = (n + kTierTile - 1) / kTierTile;
-    uint32_t* tcnt = c.t_cnt.reserve(tiles + 1);
-    uint64_t* toff = c.t_off.reserve(tiles + 2);
-    TierCountKernel<<<static_cast<unsigned>(tiles), kThreads, 0, c.stream>>>(src32, n, limit32,
-                                                                          tcnt);
-    ExclusiveScanU32(c, tcnt, toff, tiles);
-    n_a = ReadU64(c, toff + tiles);
-    n_b = n - n_a;
-    uint32_t* a_val = reinterpret_cast<uint32_t*>(c.t_aval.reserve(n_a / 2 + 2));
-    uint64_t* a_org = c.t_aorg.reserve(n_a + 1);
-    uint32_t* b_src = reinterpret_cast<uint32_t*>(c.t_b0.reserve(n_b / 2 + 2));
-    TierScatterKernel<<<static_cast<unsigned>(tiles), kThreads, 0, c.stream>>>(
-        src32, src_org, n, limit32, toff, a_val, a_org, b_src);
-    RVN_LAUNCH_CHECK();
-    c.launches += 2;
+    const uint32_t* a_val;
+    const uint64_t* a_org;
+    uint32_t* b_src;
+    if (pre_split >= 0) {
+      n_a = static_cast<uint64_t>(pre_split);
+      n_b = n - n_a;
+      a_val = reinterpret_cast<const uint32_t*>(c.i_val_alt.get());
+      a_org = c.i_org_alt.get();
+      b_src = reinterpret_cast<uint32_t*>(c.t_b0.get());
+    } else {
+      const uint32_t* src32 = static_cast<const uint32_t*>(src_val.p);
+      const uint64_t tiles = (n + kTierTile - 1) / kTierTile;
+      uint32_t* tcnt = c.t_cnt.reserve(tiles + 1);
+      uint64_t* toff = c.t_off.reserve(tiles + 2);
+      TierCountKernel<<<static_cast<unsigned>(tiles), kThreads, 0, c.stream>>>(src32, n, limit32,
+                                                                            tcnt);
+      ExclusiveScanU32(c, tcnt, toff, tiles);
+      n_a = ReadU64(c, toff + tiles);
+      n_b = n - n_a;
+      uint32_t* av = reinterpret_cast<uint32_t*>(c.t_aval.reserve(n_a / 2 + 2));
+      uint64_t* ao = c.t_aorg.reserve(n_a + 1);
+      b_src = reinterpret_cast<uint32_t*>(c.t_b0.reserve(n_b / 2 + 2));
+      TierScatterKernel<<<static_cast<unsigned>(tiles), kThreads, 0, c.stream>>>(
+          src32, src_org, n, limit32, toff, av, ao, b_src);
+      RVN_LAUNCH_CHECK();
+      c.launches += 2;
+      a_val = av;
+      a_org = ao;
+    }
     // the probe-able tier: values <= limit need fewer key bits
     int bits_a = 1;
     while (bits_a < key_bits && (value_limit >> bits_a) != 0) ++bits_a;
@@ -804,6 +866,221 @@ void BuildIndexFrom(Ctx& c, ValView src_val, const uint64_t* src_org, uint64_t n
   c.i_valid = true;
 }
 
+// reads [first, last) cut into ranges of >= chunk bases at read boundaries, by the rule
+// that cuts index batches (construct.cc:36-44): boundaries first, ..., last
+std::vector<uint32_t> ChunkCuts(const Ctx& c, uint32_t first, uint32_t last, uint64_t chunk) {
+  std::vector<uint32_t> cuts{first};
+  uint64_t bases = 0;
+  for (uint32_t r = first; r < last; ++r) {
+    bases += c.h_len[r];
+    if (r + 1 != last && bases < chunk) continue;
+    bases = 0;
+    cuts.push_back(r + 1);
+  }
+  if (cuts.back() != last) cuts.push_back(last);
+  return cuts;
+}
+
+}  // namespace
+
+uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, uint64_t chunk,
+                           uint64_t tmax) {
+  c.i_valid = false;
+  c.occurrence = 0xFFFFFFFFu;
+  if (last > first && (first < c.res_first || last > c.res_last)) {
+    throw StateError("the bases of these reads were not uploaded (rvn_reads_upload_range)");
+  }
+  // (an asynchronous upload: every chunk's bases are there before the first sketch)
+  WaitUpload(c);
+  const std::vector<uint32_t> cuts = ChunkCuts(c, first, last, chunk);
+  const uint32_t nr = last - first;
+  const bool k32 = 2 * c.prm.k <= 30;
+  const int key_bits = static_cast<int>(2 * c.prm.k);
+  const int hist_shift = std::max(0, key_bits - kCapBits);
+  unsigned long long* vhist = reinterpret_cast<unsigned long long*>(c.t_hist.reserve(kCapBins));
+  RVN_CUDA(cudaMemsetAsync(vhist, 0, kCapBins * sizeof(uint64_t), c.stream));
+
+  uint64_t bases = 0;
+  for (uint32_t r = first; r < last; ++r) bases += c.h_len[r];
+  if (minhash) {
+    // one sweep: each chunk's micromizers are appended to the sort's second buffers,
+    // sized by the len / k micromizers a read has at most
+    uint64_t cap = 0;
+    for (uint32_t r = first; r < last; ++r) cap += c.h_len[r] / c.prm.k;
+    const size_t vb = k32 ? 4 : 8;
+    uint64_t* q_val = c.i_val_alt.reserve(k32 ? cap / 2 + 2 : cap + 1);
+    uint64_t* q_org = c.i_org_alt.reserve(cap + 1);
+    uint64_t n = 0;
+    for (size_t i = 0; i + 1 < cuts.size(); ++i) {
+      EnsureMicromizers(c, cuts[i], cuts[i + 1]);  // (sketches the chunk)
+      TimerBegin(c, "sketch_tiers");
+      if (c.q_n) {
+        RVN_CUDA(cudaMemcpyAsync(reinterpret_cast<uint8_t*>(q_val) + n * vb, c.q_val.get(),
+                                 c.q_n * vb, cudaMemcpyDeviceToDevice, c.stream));
+        RVN_CUDA(cudaMemcpyAsync(q_org + n, c.q_org.get(), c.q_n * sizeof(uint64_t),
+                                 cudaMemcpyDeviceToDevice, c.stream));
+      }
+      TimerEnd(c);
+      n += c.q_n;
+    }
+    if (n >= 0xFFFFFFFFULL) throw LimitError("index batch holds 2^32 or more minimizers");
+    c.i_first = first;
+    c.i_last = last;
+    BuildIndexImpl(c, ValView{q_val, k32 ? 1 : 0}, q_org, n, bases, ~0ULL, /*count_bare=*/true, 0);
+    c.i_sorted_ids = c.ids_ascending;
+    c.i_from_sketch = false;
+    return tmax;
+  }
+
+  // ---- sweep 1: per chunk its sketch, its thresholds and micromizer counts (the
+  // self-join's, for the whole batch), the record count and the coarse value histogram
+  // that bounds the tiers ----
+  uint64_t n = 0;
+  c.jt_val.reserve(nr + 1ULL);
+  c.jt_pos.reserve(nr + 1ULL);
+  c.h_jt_off.assign(1, 0);
+  for (size_t i = 0; i + 1 < cuts.size(); ++i) {
+    const uint32_t r0 = cuts[i], r1 = cuts[i + 1];
+    EnsureSketch(c, r0, r1);  // (exactly the chunk: c.s_n and c.s_val are its records)
+    EnsureThresholds(c, r0, r1);
+    n += c.s_n;
+    RVN_CUDA(cudaMemcpyAsync(c.jt_val.get() + (r0 - first), c.qt_val.get(),
+                             (r1 - r0) * sizeof(uint64_t), cudaMemcpyDeviceToDevice, c.stream));
+    RVN_CUDA(cudaMemcpyAsync(c.jt_pos.get() + (r0 - first), c.qt_pos.get(),
+                             (r1 - r0) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, c.stream));
+    const uint64_t base = c.h_jt_off.back();
+    for (uint32_t r = 1; r <= r1 - r0; ++r) c.h_jt_off.push_back(base + c.h_q_off[r]);
+    if (k32 && c.s_n > 0) {
+      ValueHistKernel<<<std::min<unsigned>(CeilDiv(c.s_n, kThreads), c.sms * 4), kThreads, 0,
+                        c.stream>>>(reinterpret_cast<const uint32_t*>(c.s_val.get()), c.s_n,
+                                    hist_shift, vhist);
+      RVN_LAUNCH_CHECK();
+      ++c.launches;
+    }
+  }
+  if (n >= 0xFFFFFFFFULL) throw LimitError("index batch holds 2^32 or more minimizers");
+  // the tier bound: the largest micromizer value of every read sketched so far
+  if (nr > 0) {
+    if (!k32) {
+      tmax = ~0ULL;
+    } else {
+      uint64_t* w = c.m_counter.reserve(8);
+      RVN_CUDA(cudaMemsetAsync(w, 0, sizeof(uint64_t), c.stream));
+      MaxU64Kernel<<<std::min<unsigned>(CeilDiv(nr, 256), c.sms * 8), 256, 0, c.stream>>>(
+          c.jt_val.get(), nr, reinterpret_cast<unsigned long long*>(w));
+      RVN_LAUNCH_CHECK();
+      ++c.launches;
+      tmax = std::max(tmax, ReadU64(c, w));
+    }
+  }
+  const uint64_t limit = tmax;
+  const bool is32 = k32;
+  const bool tiered = Tiered(c, is32, limit, n);
+  // raven's stage-1 parameters: sweep 2 sketches straight into the tiers, and the last
+  // chunk's sketch is not needed any more
+  const bool fused = tiered && SketchTiersFused(c);
+  if (fused) {
+    c.s_valid = c.q_valid = false;
+    c.s_val.release();
+    c.s_org.release();
+  }
+
+  // ---- sweep 2: the chunks' records, appended in (read, position) order ----
+  uint64_t n_a_cap = n, n_b_cap = 0;
+  if (tiered) {  // tier capacities from the histogram (the bin of the limit counts in both)
+    std::vector<uint64_t> h(kCapBins);
+    RVN_CUDA(cudaMemcpyAsync(h.data(), vhist, kCapBins * sizeof(uint64_t),
+                             cudaMemcpyDeviceToHost, c.stream));
+    RVN_CUDA(cudaStreamSynchronize(c.stream));
+    const uint64_t lb = limit >> hist_shift;
+    n_a_cap = 0;
+    for (uint64_t b = 0; b < kCapBins; ++b) {
+      if (b <= lb) n_a_cap += h[b];
+      if (b >= lb) n_b_cap += h[b];
+    }
+  }
+  const uint64_t val_elems = is32 ? n_a_cap / 2 + 2 : n_a_cap + 1;
+  uint64_t* a_val = c.i_val_alt.reserve(val_elems);
+  uint64_t* a_org = c.i_org_alt.reserve(n_a_cap + 1);
+  uint32_t* b_val = tiered ? reinterpret_cast<uint32_t*>(c.t_b0.reserve(n_b_cap / 2 + 2)) : nullptr;
+  const uint32_t limit32 = static_cast<uint32_t>(limit);
+  uint64_t n_a = 0, n_b = 0;
+  for (size_t i = 0; i + 1 < cuts.size(); ++i) {
+    const uint32_t r0 = cuts[i], r1 = cuts[i + 1];
+    if (fused) {
+      TimerBegin(c, "sketch_tiers");
+      uint64_t m_a = 0, m_b = 0;
+      SketchTiers(c, r0, r1, limit32, reinterpret_cast<uint32_t*>(a_val) + n_a, a_org + n_a,
+                  n_a_cap - n_a, b_val + n_b, n_b_cap - n_b, &m_a, &m_b);
+      // (the capacities are the histogram's bound: never exceeded)
+      if (n_a + m_a > n_a_cap || n_b + m_b > n_b_cap) {
+        throw CudaError("chunked index build: tier capacity below the histogram's bound");
+      }
+      n_a += m_a;
+      n_b += m_b;
+      TimerEnd(c);
+      continue;
+    }
+    EnsureSketch(c, r0, r1);  // (no-op for a batch of one chunk)
+    const uint64_t* sv = c.s_val.get();
+    const uint64_t* so = c.s_org.get();
+    const uint64_t m = c.s_n;
+    TimerBegin(c, "sketch_tiers");
+    if (m == 0) {
+    } else if (tiered) {
+      const uint32_t* sv32 = reinterpret_cast<const uint32_t*>(sv);
+      const uint64_t tiles = (m + kTierTile - 1) / kTierTile;
+      uint32_t* tcnt = c.t_cnt.reserve(tiles + 1);
+      uint64_t* toff = c.t_off.reserve(tiles + 2);
+      TierCountKernel<<<static_cast<unsigned>(tiles), kThreads, 0, c.stream>>>(sv32, m, limit32,
+                                                                            tcnt);
+      ExclusiveScanU32(c, tcnt, toff, tiles);
+      const uint64_t m_a = ReadU64(c, toff + tiles);
+      if (n_a + m_a > n_a_cap || n_b + (m - m_a) > n_b_cap) {
+        throw CudaError("chunked index build: tier capacity below the histogram's bound");
+      }
+      TierScatterKernel<<<static_cast<unsigned>(tiles), kThreads, 0, c.stream>>>(
+          sv32, so, m, limit32, toff, reinterpret_cast<uint32_t*>(a_val) + n_a, a_org + n_a,
+          b_val + n_b);
+      RVN_LAUNCH_CHECK();
+      c.launches += 2;
+      n_a += m_a;
+      n_b += m - m_a;
+    } else {
+      const size_t vb = is32 ? 4 : 8;
+      RVN_CUDA(cudaMemcpyAsync(reinterpret_cast<uint8_t*>(a_val) + n_a * vb, sv, m * vb,
+                               cudaMemcpyDeviceToDevice, c.stream));
+      RVN_CUDA(cudaMemcpyAsync(a_org + n_a, so, m * sizeof(uint64_t), cudaMemcpyDeviceToDevice,
+                               c.stream));
+      n_a += m;
+    }
+    TimerEnd(c);
+  }
+  c.i_first = first;
+  c.i_last = last;
+  BuildIndexImpl(c, ValView{a_val, is32 ? 1 : 0}, a_org, n, bases, limit, /*count_bare=*/true,
+                 tiered ? static_cast<int64_t>(n_a) : 0);
+  c.i_sorted_ids = c.ids_ascending;
+  c.i_from_sketch = true;
+  c.jt_gen = c.i_gen;
+  return tmax;
+}
+
+void ReleaseIndexBuild(Ctx& c) {
+  c.s_valid = false;
+  c.s_val.release();
+  c.s_org.release();
+  c.i_val_alt.release();
+  c.i_org_alt.release();
+  c.t_aval.release();
+  c.t_aorg.release();
+  c.t_b0.release();
+  c.t_b1.release();
+  c.t_b2.release();
+  c.t_bstart.release();
+  c.t_sorted_b = nullptr;  // (t_nb stays: FilterIndex refuses what would need the keys)
+}
+
 uint64_t* IndexHistogram(Ctx& c) {  // filled by the build
   return c.i_hist.get();
 }
@@ -848,6 +1125,11 @@ uint32_t FilterIndex(Ctx& c, double frequency) {
     for (uint32_t len = 0; len + 1 < kHistBins; ++len) cum += h[len];
     std::size_t rank = static_cast<std::size_t>((1 - frequency) * static_cast<double>(c.i_keys));
     if (rank >= c.i_keys) rank = c.i_keys - 1;
+    if (c.i_is32 && c.t_nb && !c.t_sorted_b) {
+      throw StateError(
+          "the bare keys of this chunked index build were freed: runs of 65535 or more "
+          "postings need them, build the index again to filter at this frequency");
+    }
     const uint64_t n_long = h[kHistBins - 1];
     uint32_t* out = c.m_cnt.reserve(n_long + 1);
     uint64_t* counter = c.m_counter.reserve(8);

@@ -996,12 +996,17 @@ __global__ void ReorderOverlaps(const rvn_overlap* __restrict__ raw,
 // Reads before `first` are left out: their flushes took the probe path, and their
 // thresholds would cost a sketch of reads that are no longer sketched. The slot
 // offsets are kept with the slots, as a flush over reads outside the batch replaces
-// the micromizer counts (c.h_q_off). Needs the thresholds of reads [first, i_last).
+// the micromizer counts (c.h_q_off). Needs the thresholds of reads [first, i_last): the
+// batch's own (c.jt_*) after a chunked build, else c.qt_*.
 void JoinSweep(Ctx& c, uint32_t first) {
+  const bool batch = c.jt_gen == c.i_gen;
+  const std::vector<uint64_t>& cnt_off = batch ? c.h_jt_off : c.h_q_off;
+  const uint64_t* thr_val = batch ? c.jt_val.get() : c.qt_val.get();
+  const uint32_t* thr_pos = batch ? c.jt_pos.get() : c.qt_pos.get();
   const uint32_t nr = c.i_last - first;
-  const uint64_t t0 = first - c.qt_first, base = c.h_q_off[t0];
+  const uint64_t t0 = first - (batch ? c.i_first : c.qt_first), base = cnt_off[t0];
   c.h_j_off.resize(nr + 1ULL);
-  for (uint32_t i = 0; i <= nr; ++i) c.h_j_off[i] = c.h_q_off[t0 + i] - base;
+  for (uint32_t i = 0; i <= nr; ++i) c.h_j_off[i] = cnt_off[t0 + i] - base;
   const uint64_t n_q = c.h_j_off[nr];
   uint64_t* off = c.j_off.reserve(nr + 1ULL);
   RVN_CUDA(cudaMemcpyAsync(off, c.h_j_off.data(), (nr + 1ULL) * sizeof(uint64_t),
@@ -1012,7 +1017,7 @@ void JoinSweep(Ctx& c, uint32_t first) {
   RVN_CUDA(cudaMemsetAsync(packed, 0, (n_q + 1) * sizeof(uint64_t), c.stream));
   if (c.i_n > 0 && n_q > 0) {
     JoinView jv{ValView{c.i_val.get(), c.i_is32 ? 1 : 0}, c.i_org.get(), c.i_n, c.occurrence,
-                c.qt_val.get() + t0, c.qt_pos.get() + t0, first, c.i_last};
+                thr_val + t0, thr_pos + t0, first, c.i_last};
     JoinSweepKernel<<<CeilDiv(c.i_n, kThreads), kThreads, 0, c.stream>>>(jv, off, cursor,
                                                                           packed);
     RVN_LAUNCH_CHECK();
@@ -1049,7 +1054,8 @@ HitCounts JoinHits(Ctx& c, uint32_t first, uint32_t last, uint64_t* read_hit_off
   const uint32_t nr = last - first;
   HitCounts h;
   const bool sweep = c.j_gen != c.i_gen || c.j_occurrence != c.occurrence || first < c.j_first;
-  if (sweep && !(c.qt_valid && c.qt_first <= first && c.i_last <= c.qt_last)) {
+  if (sweep && c.jt_gen != c.i_gen &&
+      !(c.qt_valid && c.qt_first <= first && c.i_last <= c.qt_last)) {
     EnsureThresholds(c, first, c.i_last);  // (its sketch and micromize time are not probe's)
   }
   TimerBegin(c, "probe");

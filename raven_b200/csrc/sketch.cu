@@ -329,25 +329,30 @@ SketchKernel(const uint64_t* __restrict__ words,
 // ---------------------------------------------------------------------------
 constexpr int kFastGroup = 4;  // consecutive tiles per CTA: one look-back for all
 
+// the n values of one tile, compacted in shared memory in output order, by the CTA: 4 a
+// store; a head up to the first 16-byte boundary and a tail
+__device__ __forceinline__ void StoreTileValues(const uint32_t* __restrict__ sh_val, uint32_t n,
+                                                uint32_t* __restrict__ out_val) {
+  const uint32_t head =
+      min(n, static_cast<uint32_t>((16 - (reinterpret_cast<uintptr_t>(out_val) & 15)) & 15) / 4);
+  const uint32_t nvec = (n - head) / 4;
+  uint4* vp = reinterpret_cast<uint4*>(out_val + head);
+  for (uint32_t i = threadIdx.x; i < nvec; i += kSketchThreads) {
+    const uint32_t* s = sh_val + head + 4 * i;
+    vp[i] = make_uint4(s[0], s[1], s[2], s[3]);
+  }
+  const uint32_t tail = head + 4 * nvec;
+  if (threadIdx.x < head) out_val[threadIdx.x] = sh_val[threadIdx.x];
+  if (threadIdx.x < n - tail) out_val[tail + threadIdx.x] = sh_val[tail + threadIdx.x];
+}
+
 // the n records of one tile, compacted in shared memory in output order, by the CTA
 __device__ __forceinline__ void StoreTileRecords(const uint32_t* __restrict__ sh_val,
                                                  const uint16_t* __restrict__ sh_org,
                                                  uint32_t n, uint64_t org_base,
                                                  uint32_t* __restrict__ out_val,
                                                  uint64_t* __restrict__ out_org) {
-  {  // values: 4 a store; a head up to the first 16-byte boundary and a tail
-    const uint32_t head =
-        min(n, static_cast<uint32_t>((16 - (reinterpret_cast<uintptr_t>(out_val) & 15)) & 15) / 4);
-    const uint32_t nvec = (n - head) / 4;
-    uint4* vp = reinterpret_cast<uint4*>(out_val + head);
-    for (uint32_t i = threadIdx.x; i < nvec; i += kSketchThreads) {
-      const uint32_t* s = sh_val + head + 4 * i;
-      vp[i] = make_uint4(s[0], s[1], s[2], s[3]);
-    }
-    const uint32_t tail = head + 4 * nvec;
-    if (threadIdx.x < head) out_val[threadIdx.x] = sh_val[threadIdx.x];
-    if (threadIdx.x < n - tail) out_val[tail + threadIdx.x] = sh_val[tail + threadIdx.x];
-  }
+  StoreTileValues(sh_val, n, out_val);
   {  // origins: 2 a store
     const uint32_t head = min(n, (reinterpret_cast<uintptr_t>(out_org) & 15) ? 1u : 0u);
     const uint32_t nvec = (n - head) / 2;
@@ -362,7 +367,49 @@ __device__ __forceinline__ void StoreTileRecords(const uint32_t* __restrict__ sh
   }
 }
 
-template <int W>
+// Decoupled look-back of `group` by the first warp, 32 predecessors per step: returns the
+// sum of the totals of the groups before it and publishes its own inclusive prefix.
+__device__ __forceinline__ uint64_t LookBack(uint64_t* __restrict__ status, uint32_t group,
+                                             uint64_t total) {
+  const uint32_t lane = threadIdx.x;
+  uint64_t excl = 0;
+  volatile uint64_t* st = status;
+  if (group > 0) {
+    if (lane == 0) {
+      st[group] = kStAggregate | total;
+      __threadfence();
+    }
+    __syncwarp();
+    int64_t idx = static_cast<int64_t>(group) - 1;
+    while (true) {
+      const int64_t mine = idx - lane;
+      uint64_t v = kStPrefix;  // before group 0: an empty prefix
+      if (mine >= 0) {
+        do {
+          v = st[mine];
+        } while ((v & kStMask) == 0);
+      }
+      const uint32_t pm = __ballot_sync(0xFFFFFFFFu, (v & kStMask) == kStPrefix);
+      const int firstp = __ffs(pm) - 1;
+      uint64_t part = (firstp < 0 || static_cast<int>(lane) <= firstp) ? (v & ~kStMask) : 0;
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) part += __shfl_xor_sync(0xFFFFFFFFu, part, d);
+      excl += part;
+      if (firstp >= 0) break;
+      idx -= 32;
+    }
+  }
+  if (lane == 0) st[group] = kStPrefix | (excl + total);
+  return excl;
+}
+
+// kTiers: the tier-output mode of the chunked index build (index.cu). The records go to
+// two streams in (read, position) order: value <= limit as (value, origin) to out_val /
+// out_org (tier A, capacity out_cap), value > limit as bare keys to out_b (capacity
+// out_cap_b). Each stream has its own status array and look-back (status, status_b), so
+// both counts are exact to 2^62; past its capacity a stream is only counted. tile_out
+// receives the two totals (2 entries) instead of per-tile offsets.
+template <int W, bool kTiers>
 __global__ void __launch_bounds__(kSketchThreads, 4)
 SketchFastKernel(const uint64_t* __restrict__ words, const uint64_t* __restrict__ woff,
                  const uint32_t* __restrict__ lens, const uint32_t* __restrict__ ids,
@@ -371,7 +418,8 @@ SketchFastKernel(const uint64_t* __restrict__ words, const uint64_t* __restrict_
                  uint32_t last_read, uint32_t k, unsigned int* __restrict__ ticket,
                  uint64_t* __restrict__ status, uint64_t* __restrict__ tile_out,
                  uint64_t n_tiles, uint64_t out_cap, uint32_t* __restrict__ out_val,
-                 uint64_t* __restrict__ out_org) {
+                 uint64_t* __restrict__ out_org, uint32_t limit, uint64_t* __restrict__ status_b,
+                 uint64_t out_cap_b, uint32_t* __restrict__ out_b) {
   constexpr uint32_t kBad = 0xFFFFFFFFu;
   constexpr int H = W - 1;
   constexpr int ITEMS = 8;
@@ -395,7 +443,7 @@ SketchFastKernel(const uint64_t* __restrict__ words, const uint64_t* __restrict_
   __shared__ uint32_t sh_id[G], sh_wlo[G], sh_wn[G], sh_wvalid[G];
   __shared__ const uint64_t* sh_wsrc[G];
   __shared__ uint32_t sh_group;
-  __shared__ uint64_t sh_excl;
+  __shared__ uint64_t sh_excl, sh_excl_b;
 
   // ticket: the group of G consecutive tiles this CTA sketches (tiles of one launch
   // are ordered by (read, position), so a group may span reads). One lane per tile
@@ -515,7 +563,7 @@ SketchFastKernel(const uint64_t* __restrict__ words, const uint64_t* __restrict_
 
   // ---- select; one scan counts the records of all tiles (16 bits a tile) ----
   static_assert(kSketchTile < (1u << 16) && G <= 4, "tile counts packed in a u64");
-  uint64_t packed = 0;
+  uint64_t packed = 0, packed_b = 0;  // (kTiers: tier A, bare keys)
 #pragma unroll
   for (int g = 0; g < G; ++g) {
     flags[g] = 0;
@@ -551,66 +599,64 @@ SketchFastKernel(const uint64_t* __restrict__ words, const uint64_t* __restrict_
           const uint32_t hq = h[H + i];
           if (best == hq && hq != kBad) fl |= 1u << i;
         }
+        if (kTiers) {
+          uint32_t fb = 0;
+#pragma unroll
+          for (int i = 0; i < ITEMS; ++i) fb |= (h[H + i] > limit ? 1u : 0u) << i;
+          fb &= fl;
+          packed_b |= static_cast<uint64_t>(__popc(fb)) << (16 * g);
+          packed |= static_cast<uint64_t>(__popc(fl & ~fb)) << (16 * g);
+        } else {
+          packed |= static_cast<uint64_t>(__popc(fl)) << (16 * g);
+        }
       }
       flags[g] = fl;
-      packed |= static_cast<uint64_t>(__popc(fl)) << (16 * g);
     }
   }
-  uint64_t totals;
+  uint64_t totals, totals_b = 0, ex_packed_b = 0;
   const uint64_t ex_packed = BlockExclusiveSum<uint64_t, kSketchThreads>(packed, sh_scan, &totals);
-  uint32_t group_total = 0;
+  if (kTiers) {
+    ex_packed_b = BlockExclusiveSum<uint64_t, kSketchThreads>(packed_b, sh_scan, &totals_b);
+  }
+  uint32_t group_total = 0, group_total_b = 0;
 #pragma unroll
-  for (int g = 0; g < G; ++g) group_total += static_cast<uint32_t>(totals >> (16 * g)) & 0xFFFFu;
+  for (int g = 0; g < G; ++g) {
+    group_total += static_cast<uint32_t>(totals >> (16 * g)) & 0xFFFFu;
+    group_total_b += static_cast<uint32_t>(totals_b >> (16 * g)) & 0xFFFFu;
+  }
 
   // ---- output offset of the group: decoupled look-back by the first warp ----
   if (threadIdx.x < 32) {
-    const uint32_t lane = threadIdx.x;
-    uint64_t excl = 0;
-    volatile uint64_t* st = status;
-    if (group > 0) {
-      if (lane == 0) {
-        st[group] = kStAggregate | group_total;
-        __threadfence();
-      }
-      __syncwarp();
-      int64_t idx = static_cast<int64_t>(group) - 1;
-      while (true) {
-        const int64_t mine = idx - lane;
-        uint64_t v = kStPrefix;  // before group 0: an empty prefix
-        if (mine >= 0) {
-          do {
-            v = st[mine];
-          } while ((v & kStMask) == 0);
+    const uint64_t excl = LookBack(status, group, group_total);
+    const uint64_t excl_b = kTiers ? LookBack(status_b, group, group_total_b) : 0;
+    if (threadIdx.x == 0) {
+      if (kTiers) {
+        if (t_first + g_count == n_tiles) {
+          tile_out[0] = excl + group_total;
+          tile_out[1] = excl_b + group_total_b;
         }
-        const uint32_t pm = __ballot_sync(0xFFFFFFFFu, (v & kStMask) == kStPrefix);
-        const int firstp = __ffs(pm) - 1;
-        uint64_t part = (firstp < 0 || static_cast<int>(lane) <= firstp) ? (v & ~kStMask) : 0;
-#pragma unroll
-        for (int d = 16; d > 0; d >>= 1) part += __shfl_xor_sync(0xFFFFFFFFu, part, d);
-        excl += part;
-        if (firstp >= 0) break;
-        idx -= 32;
+      } else {
+        uint64_t run = excl;
+        for (int g = 0; g < g_count; ++g) {
+          tile_out[t_first + g] = run;
+          run += static_cast<uint32_t>(totals >> (16 * g)) & 0xFFFFu;
+        }
+        if (t_first + g_count == n_tiles) tile_out[n_tiles] = run;
       }
-    }
-    if (lane == 0) {
-      st[group] = kStPrefix | (excl + group_total);
-      uint64_t run = excl;
-      for (int g = 0; g < g_count; ++g) {
-        tile_out[t_first + g] = run;
-        run += static_cast<uint32_t>(totals >> (16 * g)) & 0xFFFFu;
-      }
-      if (t_first + g_count == n_tiles) tile_out[n_tiles] = run;
       sh_excl = excl;
+      sh_excl_b = excl_b;
     }
   }
   __syncthreads();
 
   // ---- write-out, tile by tile: compact in shared memory, then store coalesced ----
-  uint64_t base = sh_excl;
+  // (kTiers: the tile's tier-A records first, its bare keys behind them)
+  uint64_t base = sh_excl, base_b = sh_excl_b;
 #pragma unroll
   for (int g = 0; g < G; ++g) {
     if (g < g_count) {
       const uint32_t n = static_cast<uint32_t>(totals >> (16 * g)) & 0xFFFFu;
+      const uint32_t nb = static_cast<uint32_t>(totals_b >> (16 * g)) & 0xFFFFu;
       uint32_t* sh_val = sh_hash_all[g];
       // the value of record e moves to slot e <= its own slot: every thread reads its
       // values before any is overwritten (the barrier also ends the previous tile's
@@ -621,16 +667,27 @@ SketchFastKernel(const uint64_t* __restrict__ words, const uint64_t* __restrict_
       for (int i = 0; i < ITEMS; ++i) v[i] = own[i];
       __syncthreads();
       uint32_t e = static_cast<uint32_t>(ex_packed >> (16 * g)) & 0xFFFFu;
+      uint32_t eb = n + (static_cast<uint32_t>(ex_packed_b >> (16 * g)) & 0xFFFFu);
 #pragma unroll
       for (int i = 0; i < ITEMS; ++i) {
         if ((flags[g] >> i) & 1u) {
-          sh_val[e] = v[i];
-          sh_org[e] =
-              static_cast<uint16_t>((threadIdx.x * ITEMS + i) << 1 | ((strands[g] >> i) & 1u));
-          ++e;
+          if (kTiers && v[i] > limit) {
+            sh_val[eb++] = v[i];
+          } else {
+            sh_val[e] = v[i];
+            sh_org[e] =
+                static_cast<uint16_t>((threadIdx.x * ITEMS + i) << 1 | ((strands[g] >> i) & 1u));
+            ++e;
+          }
         }
       }
       __syncthreads();
+      if (kTiers) {
+        const uint64_t room_b = base_b < out_cap_b ? out_cap_b - base_b : 0;
+        const uint32_t nb_out = static_cast<uint32_t>(min(static_cast<uint64_t>(nb), room_b));
+        if (nb_out > 0) StoreTileValues(sh_val + n, nb_out, out_b + base_b);
+        base_b += nb;
+      }
       // past out_cap the pass only counts (the host repeats it with the exact size)
       const uint64_t room = base < out_cap ? out_cap - base : 0;
       const uint32_t n_out = static_cast<uint32_t>(min(static_cast<uint64_t>(n), room));
@@ -936,11 +993,11 @@ void EnsureSketch(Ctx& c, uint32_t first, uint32_t last) {
             }
           }
           if (upto <= launched) continue;
-          SketchFastKernel<5><<<static_cast<unsigned>(upto - launched), kSketchThreads, 0,
-                                c.stream>>>(
+          SketchFastKernel<5, false><<<static_cast<unsigned>(upto - launched), kSketchThreads, 0,
+                                       c.stream>>>(
               c.d_words.get(), c.d_woff.get(), c.d_len.get(), c.d_ids.get(),
               c.d_tile_off.get(), c.d_tile_read.get(), first, last, c.prm.k, ticket, status, tout,
-              n_tiles, cap, reinterpret_cast<uint32_t*>(val), org);
+              n_tiles, cap, reinterpret_cast<uint32_t*>(val), org, 0u, nullptr, 0, nullptr);
           launched = upto;
           ++c.launches;
         }
@@ -984,6 +1041,40 @@ void EnsureSketch(Ctx& c, uint32_t first, uint32_t last) {
   c.s_n = total;
   c.s_is32 = 2 * c.prm.k <= 30;
   c.s_valid = true;
+}
+
+bool SketchTiersFused(const Ctx& c) { return 2 * c.prm.k <= 30 && c.prm.w == 5; }
+
+void SketchTiers(Ctx& c, uint32_t first, uint32_t last, uint32_t limit, uint32_t* a_val,
+                 uint64_t* a_org, uint64_t cap_a, uint32_t* b_val, uint64_t cap_b,
+                 uint64_t* n_a, uint64_t* n_b) {
+  if (first < last && (first < c.res_first || last > c.res_last)) {
+    throw StateError("the bases of these reads were not uploaded (rvn_reads_upload_range)");
+  }
+  EnsureTiles(c);
+  WaitUpload(c);
+  *n_a = *n_b = 0;
+  const uint64_t n_tiles = c.h_tile_off[last] - c.h_tile_off[first];
+  if (n_tiles == 0) return;
+  if (n_tiles >= (1ULL << 31)) throw LimitError("too many sketch tiles");
+  const uint64_t n_groups = (n_tiles + kFastGroup - 1) / kFastGroup;
+  uint64_t* tout = c.tile_out.reserve(4);
+  // status words of both streams + ticket
+  uint64_t* status = c.tile_status.reserve(2 * (n_groups + 1) + 2);
+  uint64_t* status_b = status + n_groups + 1;
+  unsigned int* ticket = reinterpret_cast<unsigned int*>(status_b + n_groups + 1);
+  RVN_CUDA(cudaMemsetAsync(status, 0, (2 * (n_groups + 1) + 2) * sizeof(uint64_t), c.stream));
+  SketchFastKernel<5, true><<<static_cast<unsigned>(n_groups), kSketchThreads, 0, c.stream>>>(
+      c.d_words.get(), c.d_woff.get(), c.d_len.get(), c.d_ids.get(), c.d_tile_off.get(),
+      c.d_tile_read.get(), first, last, c.prm.k, ticket, status, tout, n_tiles, cap_a, a_val,
+      a_org, limit, status_b, cap_b, b_val);
+  RVN_LAUNCH_CHECK();
+  ++c.launches;
+  uint64_t* h = c.pin64.reserve(8);
+  RVN_CUDA(cudaMemcpyAsync(h, tout, 2 * sizeof(uint64_t), cudaMemcpyDeviceToHost, c.stream));
+  RVN_CUDA(cudaStreamSynchronize(c.stream));
+  *n_a = h[0];
+  *n_b = h[1];
 }
 
 namespace {

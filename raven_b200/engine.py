@@ -301,6 +301,26 @@ class Engine:
         """Whether the last stage-1 call ran windowed (phase "stage1_window" in its timings)."""
         return "stage1_window" in self.timings()
 
+    def set_index_chunks(self, bases=-1, budget=0):
+        """How find_overlaps_and_create_piles builds each index batch: 0 in one piece, N > 0
+        in chunks of reads of at least N bases (no sketch of the whole batch is held), -1
+        auto (chunks of 2^30 bases only when the one-shot pass does not fit the free device
+        memory, or ``budget`` bytes when that is not 0). Same results."""
+        self.set_option("index_chunk_bases", bases)
+        self.set_option("index_chunk_budget", budget)
+
+    def index_footprint(self, index_batch_bases=0):
+        """Device working set of the largest index batch over the uploaded reads, in bytes:
+        one_shot and chunked builds."""
+        o, ch = C.c_uint64(0), C.c_uint64(0)
+        self._check(self.lib.rvn_index_footprint(self.h, index_batch_bases, C.byref(o),
+                                                 C.byref(ch)))
+        return dict(one_shot=o.value, chunked=ch.value)
+
+    def stage1_index_chunked(self):
+        """Whether the last stage-1 call built its index in chunks (phase "sketch_tiers")."""
+        return "sketch_tiers" in self.timings()
+
     def stats(self):
         s = Stats()
         self._check(self.lib.rvn_get_stats(self.h, C.byref(s)))
