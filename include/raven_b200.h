@@ -249,9 +249,20 @@ int rvn_stage1_results(rvn_ctx* ctx, const rvn_overlap** overlaps,
  * sequences [win_first[w], win_first[w+1]); the first is the backbone (draft),
  * the others are layers aligned to backbone positions [seq_begin, seq_end]
  * (inclusive, < backbone length); sequence s = bases[seq_off[s]..seq_off[s+1])
- * as ACGT letters, quals (Phred+33) at the same offsets or NULL (layers weigh 1,
- * the backbone 0 like racon's dummy '!' quality).
+ * as upper-case ACGT letters (any other byte -> RVN_ERR_INVALID), quals
+ * (Phred+33) at the same offsets, the backbone's included, or NULL (layers weigh
+ * 1, the backbone 0 like racon's dummy '!' quality).
+ * A layer without bases or with seq_begin == seq_end is dropped like
+ * racon::Window::AddLayer drops it: it is no sequence of its window (not for
+ * "fewer than 3 sequences", not for the trimming threshold) and its coordinates
+ * are not looked at. Any other layer needs seq_begin < seq_end < backbone length
+ * (racon itself lets seq_end reach the backbone length) -> RVN_ERR_INVALID.
  * g must be negative (racon throws otherwise -> RVN_ERR_INVALID).
+ * Limits, each RVN_ERR_LIMIT for the whole call: 65000 bases in one window
+ * (backbone + layers; about 130 layers of a 500-base window), 32000 bases in one
+ * layer, 4095 kept layers in one window, a graph beyond 65000 nodes or edges,
+ * and int16 scores: max(|m|,|n|,|g|) * (graph nodes + layer bases + 2) <= 32000
+ * for every layer. After a failed call rvn_poa_results is RVN_ERR_STATE.
  * Results: consensus letters per window (cons_off has n_windows+1 entries),
  * status bit 0 = polished (>= 3 sequences), bit 1 = trimming skipped
  * ("might be chimeric"), coverage per consensus base if requested. */

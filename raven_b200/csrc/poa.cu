@@ -38,6 +38,7 @@ constexpr int kPoaStatusOk = 1;        // polished
 constexpr int kPoaStatusChimeric = 2;  // trimming skipped (racon's warning)
 constexpr int kPoaStatusCapacity = 64; // scratch too small: host retries bigger
 constexpr int kPoaStatusInvalid = 128; // bad layer coordinates / letters
+constexpr uint32_t kPoaMaxLayers = 4095;  // kept layers of one window (16-bit order slots)
 
 struct PoaShape {
   uint32_t ncap;   // node capacity
@@ -77,7 +78,7 @@ __host__ __device__ inline PoaLayout MakePoaLayout(const PoaShape& s) {
   L.r2n = take(2ULL * s.ncap);
   L.n2r = take(2ULL * s.ncap);
   L.stack = take(2ULL * 4 * s.ncap);
-  L.order = take(2ULL * 4096);
+  L.order = take(2ULL * (kPoaMaxLayers + 1));
   L.e_tail = take(2ULL * s.ecap);
   L.e_head = take(2ULL * s.ecap);
   L.e_next_in = take(2ULL * s.ecap);
@@ -105,14 +106,61 @@ struct PoaGraph {
   bool overflow;
 };
 
+// Upper-case ACGT only, which is all racon passes. spoa codes letters as they
+// come (a lower-case letter is a fifth letter there and is printed as given), so
+// anything else has no code here and fails the window.
 __device__ __forceinline__ int CodeOf(uint8_t c) {
   switch (c) {
-    case 'A': case 'a': return 0;
-    case 'C': case 'c': return 1;
-    case 'G': case 'g': return 2;
-    case 'T': case 't': case 'U': case 'u': return 3;
+    case 'A': return 0;
+    case 'C': return 1;
+    case 'G': return 2;
+    case 'T': return 3;
     default: return -1;
   }
+}
+
+// racon::Window::AddLayer drops a layer without bases or with begin == end
+// before it looks at anything else: such an entry is not a sequence of its
+// window. It does not count for "fewer than 3 sequences" or for the trimming
+// threshold, and its coordinates are never checked.
+__host__ __device__ inline bool LayerKept(const uint64_t* seq_off, const uint32_t* seq_begin,
+                                          const uint32_t* seq_end, uint32_t s) {
+  return seq_off[s + 1] != seq_off[s] && seq_begin[s] != seq_end[s];
+}
+
+// (all lanes) the sequences of window [s0, s1) under that rule, backbone included
+__device__ uint32_t KeptSequences(const uint64_t* seq_off, const uint32_t* seq_begin,
+                                  const uint32_t* seq_end, uint32_t s0, uint32_t s1,
+                                  uint32_t lane) {
+  uint32_t kept = 0;
+  for (uint32_t s = s0 + 1 + lane; s < s1; s += 32) {
+    kept += LayerKept(seq_off, seq_begin, seq_end, s);
+  }
+  return 1 + __reduce_add_sync(0xffffffffu, kept);
+}
+
+// (lane 0) order[] = the kept layers of the window as offsets from s0, by begin
+// position, stable (equal begins keep their arrival order). Returns 0, or the
+// status that ends the window: racon's coordinate check (with end < L0, as a
+// layer's end is a node of the backbone chain), a layer beyond `lmax` bases, or
+// more layers than order[] holds (PoaBatch refuses those before any launch).
+__device__ uint32_t OrderLayers(uint16_t* order, const uint64_t* seq_off,
+                                const uint32_t* seq_begin, const uint32_t* seq_end,
+                                uint32_t s0, uint32_t s1, uint32_t L0, uint32_t lmax) {
+  uint32_t n = 0;
+  for (uint32_t s = s0 + 1; s < s1; ++s) {
+    if (!LayerKept(seq_off, seq_begin, seq_end, s)) continue;
+    if (n >= kPoaMaxLayers) return kPoaStatusCapacity;
+    if (seq_begin[s] > seq_end[s] || seq_end[s] >= L0) return kPoaStatusInvalid;
+    if (seq_off[s + 1] - seq_off[s] > lmax) return kPoaStatusInvalid;
+    uint32_t b = n++;
+    while (b > 0 && seq_begin[s0 + order[b - 1]] > seq_begin[s]) {
+      order[b] = order[b - 1];
+      --b;
+    }
+    order[b] = static_cast<uint16_t>(s - s0);
+  }
+  return 0;
 }
 
 __device__ uint16_t AddNode(PoaGraph& g, uint32_t code) {
@@ -354,7 +402,7 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
   const uint32_t lane = threadIdx.x;
   const uint32_t w = win_list ? win_list[blockIdx.x] : blockIdx.x;
   const uint32_t s0 = win_first[w], s1 = win_first[w + 1];
-  const uint32_t nseq = s1 - s0;
+  const uint32_t nseq = KeptSequences(seq_off, seq_begin, seq_end, s0, s1, lane);
   const uint32_t L0 = static_cast<uint32_t>(seq_off[s0 + 1] - seq_off[s0]);
   uint8_t* out = cons + cons_off[w];
   uint32_t* cov_dst = cov_out ? cov_out + cons_off[w] : nullptr;
@@ -371,7 +419,7 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
     return;
   }
 
-  // only ACGT(U) letters are valid (racon feeds 2-bit reads)
+  // only ACGT letters are valid (racon feeds 2-bit reads)
   {
     bool bad_letter = false;
     for (uint64_t i = seq_off[s0] + lane; i < seq_off[s1]; i += 32) {
@@ -421,35 +469,15 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
     g.ecap = shape.ecap;
     g.stack_cap = 4 * shape.ncap;
     g.overflow = false;
-    sh_fail = 0;
-
-    // letters + layer coordinates are validated up front
-    bool bad = nseq - 1 > 4095;
-    for (uint32_t s = s0; s < s1 && !bad; ++s) {
-      const uint32_t len = static_cast<uint32_t>(seq_off[s + 1] - seq_off[s]);
-      if (s > s0 && (seq_begin[s] >= seq_end[s] || seq_end[s] >= L0)) bad = true;
-      if (s > s0 && len > shape.lmax) bad = true;
-    }
-    if (bad) sh_fail = kPoaStatusInvalid;
-
-    if (!bad) {
-      // backbone chain (spoa AddAlignment with an empty alignment)
-      // racon gives the backbone a dummy quality of '!' (weight 0) in any case
+    // layer coordinates are validated up front
+    sh_fail = OrderLayers(g.order, seq_off, seq_begin, seq_end, s0, s1, L0, shape.lmax);
+    if (!sh_fail) {
+      // backbone chain (spoa AddAlignment with an empty alignment): its edges weigh
+      // by its own qualities when the batch has qualities, and 0 when it has none
       SeqView bb{bases + seq_off[s0], quals ? quals + seq_off[s0] : nullptr, L0, 0};
       AddChain(g, bb, 0, L0);
       if (L0 >= 2) {
         for (uint32_t v = 0; v < g.n_nodes; ++v) g.cov[v] += 1;
-      }
-      // layers by begin position, stable
-      for (uint32_t i = 0; i + 1 < nseq; ++i) g.order[i] = static_cast<uint16_t>(i + 1);
-      for (uint32_t a = 1; a + 1 < nseq; ++a) {
-        const uint16_t v = g.order[a];
-        uint32_t b = a;
-        while (b > 0 && seq_begin[s0 + g.order[b - 1]] > seq_begin[s0 + v]) {
-          g.order[b] = g.order[b - 1];
-          --b;
-        }
-        g.order[b] = v;
       }
     }
   }
@@ -465,7 +493,6 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
     const SeqView sv{bases + seq_off[s], quals ? quals + seq_off[s] : nullptr,
                      static_cast<uint32_t>(seq_off[s + 1] - seq_off[s]), 1};
     const uint32_t len = sv.len;
-    if (len == 0) continue;
 
     // ---- (lane 0) the graph this layer aligns to, in topological order ----
     if (lane == 0) {
@@ -759,9 +786,10 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
     }
     cons_len[w] = clen;
     status[w] = static_cast<uint8_t>(st);
+    // DP cells of this window (lanes hold the same count); an attempt that ran out
+    // of capacity is run again and counted then
+    if (cells && st != kPoaStatusCapacity) atomicAdd(cells, my_cells);
   }
-  // DP cells of this window (lanes hold the same count)
-  if (lane == 0 && cells) atomicAdd(cells, my_cells);
 }
 
 }  // namespace
@@ -806,17 +834,24 @@ void PoaBatch(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first,
   std::vector<uint64_t> w_tot(n_windows, 1);
   for (uint32_t w = 0; w < n_windows; ++w) {
     const uint32_t s0 = h_win_first[w], s1 = h_win_first[w + 1];
-    uint64_t tot = 0;
+    uint64_t tot = 0, lmax = 0;
+    uint32_t kept = 0;
     for (uint32_t s = s0; s < s1; ++s) {
       const uint64_t len = h_seq_off[s + 1] - h_seq_off[s];
       tot += len;
-      if (s > s0) w_lmax[w] = std::max<uint32_t>(w_lmax[w], static_cast<uint32_t>(len));
-      else w_bb[w] = std::max<uint32_t>(w_bb[w], static_cast<uint32_t>(len));
+      if (s > s0) {
+        lmax = std::max(lmax, len);
+        kept += LayerKept(h_seq_off, h_seq_begin, h_seq_end, s);
+      } else {
+        w_bb[w] = std::max<uint32_t>(w_bb[w], static_cast<uint32_t>(len));
+      }
     }
+    // 16-bit node ids, int16 layer positions, 16-bit layer order slots
+    if (tot > 65000) throw LimitError("a POA window holds more than 65000 bases");
+    if (lmax > 32000) throw LimitError("a layer of a POA window holds more than 32000 bases");
+    if (kept > kPoaMaxLayers) throw LimitError("a POA window holds more than 4095 layers");
+    w_lmax[w] = std::max<uint32_t>(w_lmax[w], static_cast<uint32_t>(lmax));
     w_tot[w] = std::max<uint64_t>(tot, 1);
-    if (tot > 65000 || w_lmax[w] > 32000) {
-      throw LimitError("a POA window holds more than 65000 bases");
-    }
     c.po_cons_off[w + 1] = c.po_cons_off[w] + tot;
   }
   const uint64_t out_total = c.po_cons_off[n_windows];

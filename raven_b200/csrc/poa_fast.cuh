@@ -43,7 +43,7 @@ __host__ __device__ inline FastLayout MakeFastLayout(const PoaShape& s) {
   L.edgeA = take(8ULL * s.ecap);
   L.edgeW = take(4ULL * s.ecap);
   L.stack = take(2ULL * 4 * s.ncap);
-  L.order = take(2ULL * 4096);
+  L.order = take(2ULL * (kPoaMaxLayers + 1));
   L.aln_node = take(2ULL * (s.ncap + s.lmax + 2));
   L.aln_pos = take(2ULL * (s.ncap + s.lmax + 2));
   L.pred = take(4ULL * s.ncap);
@@ -374,7 +374,7 @@ PoaKernelFast(uint32_t n_windows, const uint32_t* __restrict__ win_list,
   const uint32_t lane = threadIdx.x;
   const uint32_t w = win_list ? win_list[blockIdx.x] : blockIdx.x;
   const uint32_t s0 = win_first[w], s1 = win_first[w + 1];
-  const uint32_t nseq = s1 - s0;
+  const uint32_t nseq = KeptSequences(seq_off, seq_begin, seq_end, s0, s1, lane);
   const uint32_t L0 = static_cast<uint32_t>(seq_off[s0 + 1] - seq_off[s0]);
   uint8_t* out = cons + cons_off[w];
   uint32_t* cov_dst = cov_out ? cov_out + cons_off[w] : nullptr;
@@ -429,29 +429,12 @@ PoaKernelFast(uint32_t n_windows, const uint32_t* __restrict__ win_list,
     g.ecap = shape.ecap;
     g.stack_cap = 4 * shape.ncap;
     g.overflow = false;
-    sh_fail = 0;
-    bool bad = nseq - 1 > 4095;
-    for (uint32_t s = s0; s < s1 && !bad; ++s) {
-      const uint32_t len = static_cast<uint32_t>(seq_off[s + 1] - seq_off[s]);
-      if (s > s0 && (seq_begin[s] >= seq_end[s] || seq_end[s] >= L0)) bad = true;
-      if (s > s0 && len + 1 > kFastCols) bad = true;
-    }
-    if (bad) sh_fail = kPoaStatusInvalid;
-    if (!bad) {
+    sh_fail = OrderLayers(g.order, seq_off, seq_begin, seq_end, s0, s1, L0, kFastCols - 1);
+    if (!sh_fail) {
       SeqView bb{bases + seq_off[s0], quals ? quals + seq_off[s0] : nullptr, L0, 0};
       FAddChain(g, bb, 0, L0);
       if (L0 >= 2) {
         for (uint32_t v = 0; v < g.n_nodes; ++v) FAddCov(g, v);
-      }
-      for (uint32_t i = 0; i + 1 < nseq; ++i) g.order[i] = static_cast<uint16_t>(i + 1);
-      for (uint32_t a = 1; a + 1 < nseq; ++a) {
-        const uint16_t v = g.order[a];
-        uint32_t b = a;
-        while (b > 0 && seq_begin[s0 + g.order[b - 1]] > seq_begin[s0 + v]) {
-          g.order[b] = g.order[b - 1];
-          --b;
-        }
-        g.order[b] = v;
       }
     }
   }
@@ -466,7 +449,6 @@ PoaKernelFast(uint32_t n_windows, const uint32_t* __restrict__ win_list,
     const SeqView sv{bases + seq_off[s], quals ? quals + seq_off[s] : nullptr,
                      static_cast<uint32_t>(seq_off[s + 1] - seq_off[s]), 1};
     const uint32_t len = sv.len;
-    if (len == 0) continue;
     const uint32_t lb = seq_begin[s], le = seq_end[s];
     const bool full = lb < offset && le > L0 - offset;
 
@@ -868,7 +850,7 @@ PoaKernelFast(uint32_t n_windows, const uint32_t* __restrict__ win_list,
     }
     cons_len[w] = clen;
     status[w] = static_cast<uint8_t>(st);
-    if (cells) atomicAdd(cells, my_cells);
+    if (cells && st != kPoaStatusCapacity) atomicAdd(cells, my_cells);
   }
 }
 
