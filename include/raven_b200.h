@@ -88,7 +88,10 @@ typedef struct rvn_stats {
 int rvn_version(void);
 
 /* device: CUDA ordinal. stream: a cudaStream_t to run on (e.g. torch's
- * current stream) or NULL for a stream owned by the context. */
+ * current stream) or NULL for a stream owned by the context. The environment variable
+ * RVN_SET_OPTIONS="name=value,..." sets rvn_set_option options on every context created
+ * (for programs that reach the library only through a facade); a bad entry fails the
+ * call with RVN_ERR_INVALID. */
 int rvn_ctx_create(int device, void* stream, rvn_ctx** out);
 void rvn_ctx_destroy(rvn_ctx* ctx);
 const char* rvn_last_error(const rvn_ctx* ctx);
@@ -121,7 +124,10 @@ int rvn_reads_upload_ids(rvn_ctx* ctx, const uint64_t* words,
                          const uint64_t* word_off, const uint32_t* lens,
                          const uint32_t* ids, uint32_t n_reads);
 
-/* Minimize(reads[first..last), minhash): sketch and index. */
+/* Minimize(reads[first..last), minhash): sketch and index. The index holds every record
+ * (full sketches may probe it). Option "index_chunk_bases" applies: built in chunks, no
+ * sketch of the whole range is held, and the rvn_filter that follows frees the build's
+ * buffers; the index, the threshold and every map result are the one-shot build's. */
 int rvn_minimize(rvn_ctx* ctx, uint32_t first, uint32_t last, int minhash);
 
 /* Filter(frequency): occurrence threshold of the current index.
@@ -133,6 +139,11 @@ int rvn_filter(rvn_ctx* ctx, double frequency, uint32_t* occurrence);
  * grouped by query in ascending id, each group in the reference engine's
  * emission order; ovl_off has (last-first)+1 entries. `filtered` are the
  * positions of over-frequent query minimizers (only if want_filtered). */
+/* The range is worked in flushes of query bases, as the reference cuts its queries
+ * (construct.cc:67): 2^30 bases, fewer when the device has less room; the hits, chain
+ * scratch and overlaps of one flush are on the device at a time and the results are those
+ * of one piece. A multi-flush call leaves one phase "map_flush" per flush in
+ * rvn_get_timings. */
 int rvn_map(rvn_ctx* ctx, uint32_t first, uint32_t last, int avoid_equal,
             int avoid_symmetric, int minhash, int want_filtered);
 /* Map one read that is NOT in the uploaded set (e.g. a query of an earlier
@@ -229,6 +240,14 @@ int rvn_stage1_footprint(rvn_ctx* ctx, uint64_t max_overlaps, uint64_t index_bat
 int rvn_index_footprint(rvn_ctx* ctx, uint64_t index_batch_bases, uint64_t* one_shot,
                         uint64_t* chunked);
 
+/* Estimated device memory of rvn_minimize(first, last), in bytes: the reads, the index of
+ * every record with the sort's second buffers, and the sketch of the whole range
+ * (one_shot) or of one chunk (chunked: option "index_chunk_bases" when it is > 0, else
+ * 2^30 bases). chunk: what the call would do under the options in force, 0 = one piece,
+ * else its chunk size. */
+int rvn_minimize_footprint(rvn_ctx* ctx, uint32_t first, uint32_t last, uint64_t* one_shot,
+                           uint64_t* chunked, uint64_t* chunk);
+
 /* raven::FindOverlapsAndCreatePiles over the uploaded read set: index batches
  * of >= index_batch_bases (reference: 1<<32), query flushes of >=
  * query_batch_bases (reference: 1<<30); pass 0 for the reference values.
@@ -323,16 +342,19 @@ int rvn_get_stats(rvn_ctx* ctx, rvn_stats* out);
  * mode; a windowed pass takes max_overlaps <= 65536 and leaves phase
  * "stage1_window" in rvn_get_timings); "stage1_window_budget" (bytes: replaces the
  * free device memory in the auto decision, 0 = the free memory); "index_chunk_bases"
- * (how rvn_find_overlaps_and_create_piles builds each index batch: 0 = in one piece,
+ * (how rvn_find_overlaps_and_create_piles and rvn_minimize build an index batch: 0 = in one piece,
  * with a sketch of the whole batch; N > 0 = in chunks of reads of >= N bases, cut like
  * the index batches: each chunk is sketched twice, once for its micromizer thresholds and
  * once for its records, which go straight into the index's tiers, and the build's buffers
  * are freed before the first flush; -1 = auto, the default: chunks of 2^30 bases only
- * when the one-shot pass fits neither resident nor windowed, else one piece. Results
+ * when the one-shot pass fits neither resident nor windowed (rvn_minimize: when its
+ * one-shot estimate, rvn_minimize_footprint, exceeds the memory), else one piece. Results
  * are identical in every mode; a chunked call leaves phase "sketch_tiers" in
  * rvn_get_timings; with "async_upload" a chunked build first waits for the whole
  * upload); "index_chunk_budget" (bytes: replaces the free device memory in that auto
- * decision, 0 = the free memory); "reset_stats".
+ * decision, 0 = the free memory); "map_flush_bases" (rvn_map cuts its range into flushes of
+ * >= N query bases; 0 = the default, from the device memory; for tests of the flush
+ * path, results do not depend on it); "reset_stats".
  * Unknown name or value out of range -> RVN_ERR_INVALID. */
 int rvn_set_option(rvn_ctx* ctx, const char* name, int64_t value);
 

@@ -64,6 +64,7 @@ SIGNATURES = {
     "rvn_stage1_footprint": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64,
                                        U64P, U64P, U64P]),
     "rvn_index_footprint": (C.c_int, [C.c_void_p, C.c_uint64, U64P, U64P]),
+    "rvn_minimize_footprint": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, U64P, U64P, U64P]),
     "rvn_stage1_results": (C.c_int, [C.c_void_p, C.POINTER(OVLP), C.POINTER(U64P),
                                      C.POINTER(U16P), C.POINTER(U64P), U64P]),
     "rvn_sketch": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_int,

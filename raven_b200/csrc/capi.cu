@@ -2,6 +2,7 @@
 // the stage-1 driver that replaces raven::FindOverlapsAndCreatePiles
 // (RavenLib/src/construct.cc:14-121).
 #include <algorithm>
+#include <cstdlib>
 #include <cstring>
 #include <memory>
 
@@ -199,17 +200,112 @@ double UsableMemory(const Ctx& c, uint64_t budget) {
   return static_cast<double>(free_b) + static_cast<double>(c.held_bytes);
 }
 
-// Option "index_chunk_bases": the chunk size of the pass's index builds, 0 = one-shot.
-// -1 (auto): chunks of kAutoIndexChunk bases only when the one-shot pass fits neither
-// resident nor windowed (max_overlaps permitting) in the usable memory
+// Option "index_chunk_bases": the chunk size of an index build, 0 = one-shot.
+// -1 (auto): chunks of kAutoIndexChunk bases only when `one_shot`, the caller's estimate
+// of its device memory with one-shot builds, exceeds the usable memory
 // ("index_chunk_budget" replaces it when it is not 0).
-uint64_t IndexChunk(const Ctx& c, const std::vector<uint64_t>& off,
-                    const std::vector<Batch>& batches, uint64_t kmax) {
+uint64_t IndexChunk(const Ctx& c, double one_shot) {
   if (c.index_chunk_bases >= 0) return static_cast<uint64_t>(c.index_chunk_bases);
-  const Footprint f = Stage1Footprint(c, off, batches, kmax, 0);
-  double one_shot = f.resident;
-  if (kmax <= kWindowMaxOverlaps) one_shot = std::min(one_shot, f.windowed_device);
   return one_shot > UsableMemory(c, c.index_chunk_budget) ? kAutoIndexChunk : 0;
+}
+
+// a stage-1 pass with one-shot builds: resident, or windowed (max_overlaps permitting)
+double Stage1OneShot(const Ctx& c, const std::vector<uint64_t>& off,
+                     const std::vector<Batch>& batches, uint64_t kmax) {
+  const Footprint f = Stage1Footprint(c, off, batches, kmax, 0);
+  return kmax <= kWindowMaxOverlaps ? std::min(f.resident, f.windowed_device) : f.resident;
+}
+
+// The untiered index rvn_minimize builds holds every record of the batch: values, origins
+// and the sort's second buffers (two copies of 12 B for an estimated 0.34 records per base,
+// with the buffers' headroom) and the bucket table. Estimate, not measured.
+constexpr double kUntieredIndexBytesPerBase = 8.9;
+
+// Device memory of rvn_minimize over reads [first, last): the reads, the untiered index and
+// the sketch of the batch (one-shot, chunk 0) or of one chunk of `chunk` bases.
+double MinimizeFootprint(const Ctx& c, uint32_t first, uint32_t last, uint64_t chunk) {
+  uint64_t bases = 0;
+  for (uint32_t r = first; r < last; ++r) bases += c.h_len[r];
+  const double bb = static_cast<double>(bases);
+  const double sketched = chunk ? std::min(bb, static_cast<double>(chunk)) : bb;
+  return 8.0 * c.n_words + 32.0 * c.n_reads + kUntieredIndexBytesPerBase * bb +
+         kChunkSketchBytesPerBase * sketched;
+}
+
+// rvn_map works its query range in flushes, as the reference cuts its queries
+// (construct.cc:67): at most kMapFlushCeiling bases, fewer when the device has no room for
+// the per-query-base working set of a flush (kFlushBytesPerBase on the probe path,
+// kJoinFlushBytesPerBase for the self-join, DESIGN.md §3). A range of up to kMapFlushFloor
+// bases is never cut.
+constexpr uint64_t kMapFlushCeiling = 1ULL << 30;
+constexpr uint64_t kMapFlushFloor = 1ULL << 24;
+constexpr double kJoinFlushBytesPerBase = 18.4;
+
+uint64_t MapFlushBases(const Ctx& c, uint64_t range_bases, bool join) {
+  if (c.map_flush_bases) return c.map_flush_bases;
+  if (range_bases <= kMapFlushFloor) return kMapFlushCeiling;
+  // a flush can grow into the free memory and into every buffer of the context but the
+  // reads and the index
+  auto bytes = [](const auto& b) { return static_cast<double>(b.cap * sizeof(*b.p)); };
+  const double fixed = bytes(c.d_words) + bytes(c.i_val) + bytes(c.i_org) + bytes(c.i_val_alt) +
+                       bytes(c.i_org_alt) + bytes(c.i_bucket) + bytes(c.j_packed);
+  const double room = UsableMemory(c, 0) - fixed;
+  const double flush = room / (join ? kJoinFlushBytesPerBase : kFlushBytesPerBase);
+  if (flush >= static_cast<double>(kMapFlushCeiling)) return kMapFlushCeiling;
+  return std::max(kMapFlushFloor, static_cast<uint64_t>(std::max(flush, 0.0)));
+}
+
+// rvn_map: MapRange flush by flush, each flush's overlaps, offsets and filtered positions
+// appended to the pinned host results, so that they read as one MapRange over the range.
+// One flush (and keep_hits, whose hits are those of one piece) is exactly that MapRange.
+void MapFlushes(Ctx& c, uint32_t first, uint32_t last, bool avoid_equal, bool avoid_symmetric,
+                bool minhash, bool want_filtered) {
+  uint64_t bases = 0;
+  for (uint32_t r = first; r < last; ++r) bases += c.h_len[r];
+  const bool join = c.self_join && minhash && avoid_equal && avoid_symmetric && !want_filtered &&
+                    first >= c.i_first && last <= c.i_last;
+  const std::vector<uint32_t> cuts = ChunkCuts(c, first, last, MapFlushBases(c, bases, join));
+  if (c.keep_hits || cuts.size() <= 2) {
+    MapRange(c, first, last, avoid_equal, avoid_symmetric, minhash, want_filtered);
+    return;
+  }
+  const uint32_t nr = last - first;
+  uint64_t* off = c.a_ovl_off.reserve(nr + 2ULL);
+  uint64_t* foff = c.a_filt_off.reserve(nr + 2ULL);
+  off[0] = foff[0] = 0;
+  uint64_t total = 0, f_total = 0;
+  for (size_t i = 0; i + 1 < cuts.size(); ++i) {
+    const uint32_t r0 = cuts[i], m = cuts[i + 1] - cuts[i];
+    MapRange(c, r0, r0 + m, avoid_equal, avoid_symmetric, minhash, want_filtered,
+             /*fetch=*/false);
+    TimerBegin(c, "map_flush");
+    const uint64_t n = c.r_n_ovl;
+    rvn_overlap* o = c.a_ovl.reserve_keep(total + n + 1, total);
+    uint64_t* o_off = off + (r0 - first);
+    RVN_CUDA(cudaMemcpyAsync(o + total, c.m_ovl.get(), n * sizeof(rvn_overlap),
+                             cudaMemcpyDeviceToHost, c.stream));
+    RVN_CUDA(cudaMemcpyAsync(o_off + 1, c.m_ovl_off.get() + 1, m * sizeof(uint64_t),
+                             cudaMemcpyDeviceToHost, c.stream));
+    TimerEnd(c);
+    RVN_CUDA(cudaStreamSynchronize(c.stream));
+    for (uint32_t r = 1; r <= m; ++r) o_off[r] += total;
+    // (MapRange leaves the flush's filtered positions on the host)
+    const uint64_t* ff = c.r_filt_off.get();
+    const uint64_t nf = ff[m];
+    uint32_t* f = c.a_filtered.reserve_keep(f_total + nf + 1, f_total);
+    if (nf) std::memcpy(f + f_total, c.r_filtered.get(), nf * sizeof(uint32_t));
+    for (uint32_t r = 1; r <= m; ++r) foff[r0 - first + r] = f_total + ff[r];
+    total += n;
+    f_total += nf;
+  }
+  c.r_ovl.swap(c.a_ovl);
+  c.r_ovl_off.swap(c.a_ovl_off);
+  c.r_filtered.swap(c.a_filtered);
+  c.r_filt_off.swap(c.a_filt_off);
+  c.r_n_ovl = total;
+  c.m_first_read = first;
+  c.m_last_read = last;
+  c.r_valid = true;
 }
 
 // Option "stage1_window" -1 (auto): windowed only when the resident estimate exceeds
@@ -380,7 +476,7 @@ void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
   }
   const uint64_t total_bins = c.st_pile_off[n];
   const std::vector<Batch> batches = Schedule(c, ib, qb);
-  const uint64_t chunk = IndexChunk(c, c.st_pile_off, batches, kmax);
+  const uint64_t chunk = IndexChunk(c, Stage1OneShot(c, c.st_pile_off, batches, kmax));
   const bool windowed = UseWindow(c, batches, kmax, chunk);
   c.st_windowed = false;
   uint16_t* d_pile = nullptr;
@@ -450,6 +546,60 @@ void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
   c.st_piles_on_device = !windowed;
 }
 
+void SetOption(Ctx& c, const char* name, int64_t value) {
+  if (name && std::strcmp(name, "keep_hits") == 0) {
+    c.keep_hits = value != 0;
+  } else if (name && std::strcmp(name, "async_upload") == 0) {
+    c.async_upload = value != 0;
+  } else if (name && std::strcmp(name, "self_join") == 0) {
+    c.self_join = value != 0;
+  } else if (name && std::strcmp(name, "bare_count") == 0) {
+    if (value != 0 && value != 1 && value != 8 && value != 16) {
+      throw InvalidArgument("bare_count: 0, 1, 8 or 16");
+    }
+    c.bare_count = value;
+    c.bare_cluster = 0;  // (chosen again at the next build)
+  } else if (name && std::strcmp(name, "tier_min_records") == 0) {
+    c.tier_min_records = value < 0 ? 0 : static_cast<uint64_t>(value);
+  } else if (name && std::strcmp(name, "stage1_window") == 0) {
+    if (value < -1 || value > 1) throw InvalidArgument("stage1_window: -1 (auto), 0 or 1");
+    c.stage1_window = value;
+  } else if (name && std::strcmp(name, "stage1_window_budget") == 0) {
+    c.stage1_window_budget = value < 0 ? 0 : static_cast<uint64_t>(value);
+  } else if (name && std::strcmp(name, "index_chunk_bases") == 0) {
+    if (value < -1) throw InvalidArgument("index_chunk_bases: -1 (auto), 0 or a chunk size");
+    c.index_chunk_bases = value;
+  } else if (name && std::strcmp(name, "index_chunk_budget") == 0) {
+    if (value < 0) throw InvalidArgument("index_chunk_budget: bytes, 0 = the free memory");
+    c.index_chunk_budget = static_cast<uint64_t>(value);
+  } else if (name && std::strcmp(name, "map_flush_bases") == 0) {
+    if (value < 0) throw InvalidArgument("map_flush_bases: bases, 0 = from the device memory");
+    c.map_flush_bases = static_cast<uint64_t>(value);
+  } else if (name && std::strcmp(name, "reset_stats") == 0) {
+    std::memset(&c.stats, 0, sizeof(c.stats));
+    c.launches = 0;
+    TimerReset(c);
+  } else {
+    throw InvalidArgument("unknown option");
+  }
+}
+
+// RVN_SET_OPTIONS="name=value,...": options of every context the process creates, for
+// programs that reach the library only through a facade (the reference's own executable)
+void EnvOptions(Ctx& c) {
+  const char* env = std::getenv("RVN_SET_OPTIONS");
+  if (!env) return;
+  std::string all(env);
+  for (size_t b = 0; b < all.size();) {
+    const size_t e = std::min(all.find(',', b), all.size());
+    const std::string item = all.substr(b, e - b);
+    const size_t eq = item.find('=');
+    if (eq == std::string::npos) throw InvalidArgument("RVN_SET_OPTIONS: name=value,...");
+    SetOption(c, item.substr(0, eq).c_str(), std::stoll(item.substr(eq + 1)));
+    b = e + 1;
+  }
+}
+
 }  // namespace
 
 extern "C" {
@@ -481,6 +631,7 @@ RVN_API int rvn_ctx_create(int device, void* stream, rvn_ctx** out) {
       RVN_CUDA(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
       c.own_stream = true;
     }
+    EnvOptions(c);
   });
   if (rc != RVN_OK) {
     delete ctx;
@@ -732,13 +883,24 @@ RVN_API int rvn_minimize(rvn_ctx* ctx, uint32_t first, uint32_t last,
                          int minhash) {
   return Guard(ctx, [&](Ctx& c) {
     CheckRange(c, first, last);
-    BuildIndex(c, first, last, minhash != 0);
+    const uint64_t chunk = IndexChunk(c, MinimizeFootprint(c, first, last, 0));
+    if (chunk) {
+      // untiered: a later rvn_map may probe with full sketches
+      BuildIndexChunked(c, first, last, minhash != 0, chunk, 0, /*tiers=*/false);
+      c.i_build_held = true;
+    } else {
+      BuildIndex(c, first, last, minhash != 0);
+    }
   }, /*sketches_first=*/true);
 }
 
 RVN_API int rvn_filter(rvn_ctx* ctx, double frequency, uint32_t* occurrence) {
   return Guard(ctx, [&](Ctx& c) {
     uint32_t occ = FilterIndex(c, frequency);
+    if (c.i_build_held) {
+      ReleaseIndexBuild(c);
+      c.i_build_held = false;
+    }
     if (occurrence) *occurrence = occ;
   });
 }
@@ -748,8 +910,8 @@ RVN_API int rvn_map(rvn_ctx* ctx, uint32_t first, uint32_t last,
                     int want_filtered) {
   return Guard(ctx, [&](Ctx& c) {
     CheckRange(c, first, last);
-    MapRange(c, first, last, avoid_equal != 0, avoid_symmetric != 0,
-             minhash != 0, want_filtered != 0);
+    MapFlushes(c, first, last, avoid_equal != 0, avoid_symmetric != 0, minhash != 0,
+               want_filtered != 0);
     TimerCollect(c);
   });
 }
@@ -859,7 +1021,7 @@ RVN_API int rvn_stage1_footprint(rvn_ctx* ctx, uint64_t max_overlaps,
         Schedule(c, index_batch_bases ? index_batch_bases : 1ULL << 32,
                  query_batch_bases ? query_batch_bases : 1ULL << 30);
     const Footprint f = Stage1Footprint(c, off, batches, max_overlaps,
-                                        IndexChunk(c, off, batches, max_overlaps));
+                                        IndexChunk(c, Stage1OneShot(c, off, batches, max_overlaps)));
     if (resident) *resident = static_cast<uint64_t>(f.resident);
     if (windowed_device) *windowed_device = static_cast<uint64_t>(f.windowed_device);
     if (windowed_host) *windowed_host = static_cast<uint64_t>(f.windowed_host);
@@ -875,6 +1037,19 @@ RVN_API int rvn_index_footprint(rvn_ctx* ctx, uint64_t index_batch_bases, uint64
         c.index_chunk_bases > 0 ? static_cast<uint64_t>(c.index_chunk_bases) : kAutoIndexChunk;
     if (one_shot) *one_shot = static_cast<uint64_t>(IndexFootprint(c, batches, 0));
     if (chunked) *chunked = static_cast<uint64_t>(IndexFootprint(c, batches, chunk));
+  }, /*sketches_first=*/true);
+}
+
+RVN_API int rvn_minimize_footprint(rvn_ctx* ctx, uint32_t first, uint32_t last,
+                                   uint64_t* one_shot, uint64_t* chunked, uint64_t* chunk) {
+  return Guard(ctx, [&](Ctx& c) {
+    CheckRange(c, first, last);
+    const uint64_t size =
+        c.index_chunk_bases > 0 ? static_cast<uint64_t>(c.index_chunk_bases) : kAutoIndexChunk;
+    const double fit = MinimizeFootprint(c, first, last, 0);
+    if (one_shot) *one_shot = static_cast<uint64_t>(fit);
+    if (chunked) *chunked = static_cast<uint64_t>(MinimizeFootprint(c, first, last, size));
+    if (chunk) *chunk = IndexChunk(c, fit);
   }, /*sketches_first=*/true);
 }
 
@@ -1075,40 +1250,7 @@ RVN_API int rvn_get_stats(rvn_ctx* ctx, rvn_stats* out) {
 }
 
 RVN_API int rvn_set_option(rvn_ctx* ctx, const char* name, int64_t value) {
-  return Guard(ctx, [&](Ctx& c) {
-    if (name && std::strcmp(name, "keep_hits") == 0) {
-      c.keep_hits = value != 0;
-    } else if (name && std::strcmp(name, "async_upload") == 0) {
-      c.async_upload = value != 0;
-    } else if (name && std::strcmp(name, "self_join") == 0) {
-      c.self_join = value != 0;
-    } else if (name && std::strcmp(name, "bare_count") == 0) {
-      if (value != 0 && value != 1 && value != 8 && value != 16) {
-        throw InvalidArgument("bare_count: 0, 1, 8 or 16");
-      }
-      c.bare_count = value;
-      c.bare_cluster = 0;  // (chosen again at the next build)
-    } else if (name && std::strcmp(name, "tier_min_records") == 0) {
-      c.tier_min_records = value < 0 ? 0 : static_cast<uint64_t>(value);
-    } else if (name && std::strcmp(name, "stage1_window") == 0) {
-      if (value < -1 || value > 1) throw InvalidArgument("stage1_window: -1 (auto), 0 or 1");
-      c.stage1_window = value;
-    } else if (name && std::strcmp(name, "stage1_window_budget") == 0) {
-      c.stage1_window_budget = value < 0 ? 0 : static_cast<uint64_t>(value);
-    } else if (name && std::strcmp(name, "index_chunk_bases") == 0) {
-      if (value < -1) throw InvalidArgument("index_chunk_bases: -1 (auto), 0 or a chunk size");
-      c.index_chunk_bases = value;
-    } else if (name && std::strcmp(name, "index_chunk_budget") == 0) {
-      if (value < 0) throw InvalidArgument("index_chunk_budget: bytes, 0 = the free memory");
-      c.index_chunk_budget = static_cast<uint64_t>(value);
-    } else if (name && std::strcmp(name, "reset_stats") == 0) {
-      std::memset(&c.stats, 0, sizeof(c.stats));
-      c.launches = 0;
-      TimerReset(c);
-    } else {
-      throw InvalidArgument("unknown option");
-    }
-  }, /*sketches_first=*/true);
+  return Guard(ctx, [&](Ctx& c) { SetOption(c, name, value); }, /*sketches_first=*/true);
 }
 
 RVN_API int rvn_get_timings(rvn_ctx* ctx, const char* const** names,

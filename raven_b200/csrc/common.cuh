@@ -140,7 +140,24 @@ struct PinBuf {
     }
     return p;
   }
+  // growth keeps the first `keep` elements
+  T* reserve_keep(std::size_t n, std::size_t keep) {
+    if (n > cap) {
+      T* np = nullptr;
+      std::size_t want = n + n / 16 + 64;
+      RVN_CUDA(cudaMallocHost(&np, want * sizeof(T)));
+      for (std::size_t i = 0; p && i < keep; ++i) np[i] = p[i];
+      if (p) cudaFreeHost(p);
+      p = np;
+      cap = want;
+    }
+    return p;
+  }
   T* get() const { return p; }
+  void swap(PinBuf& o) {
+    std::swap(p, o.p);
+    std::swap(cap, o.cap);
+  }
 };
 
 inline unsigned CeilDiv(std::uint64_t a, std::uint64_t b) {

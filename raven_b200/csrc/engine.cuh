@@ -194,6 +194,10 @@ struct Ctx {
   uint64_t r_n_ovl = 0;
   bool r_valid = false;
   PinBuf<uint64_t> r_hit_grp, r_hit_pos, r_hit_off;
+  // rvn_map in several flushes: the results gathered so far (they become r_* at the end)
+  PinBuf<rvn_overlap> a_ovl;
+  PinBuf<uint64_t> a_ovl_off, a_filt_off;
+  PinBuf<uint32_t> a_filtered;
   uint64_t r_n_hits = 0;
 
   // introspection staging
@@ -226,6 +230,12 @@ struct Ctx {
   // is not 0), 0 one-shot index build, N > 0 always chunks of >= N bases
   int64_t index_chunk_bases = -1;
   uint64_t index_chunk_budget = 0;
+  // rvn_minimize built the index in chunks and rvn_filter has not yet freed what only the
+  // build used (ReleaseIndexBuild)
+  bool i_build_held = false;
+  // option "map_flush_bases": rvn_map works its query range in flushes of >= N bases;
+  // 0 (default) = from the usable device memory, at most the reference's 2^30
+  uint64_t map_flush_bases = 0;
   PinBuf<rvn_overlap> w_rows;  // kmax records per read
   PinBuf<uint32_t> w_cnt;      // kept records per read
   DevBuf<uint64_t> w_pile_off, w_row_off;  // per slot (+1) of the current window
@@ -310,6 +320,16 @@ void SketchTiers(Ctx& c, uint32_t first, uint32_t last, uint32_t limit, uint32_t
                  uint64_t* a_org, uint64_t cap_a, uint32_t* b_val, uint64_t cap_b,
                  uint64_t* n_a, uint64_t* n_b);
 
+// The sketch records of reads [first, last) behind the `base` records that out_val / out_org
+// (room for cap records in all) already hold, in (read, position) order (SketchFastKernel's
+// append mode, SketchTiersFused parameters only): sweep 2 of the untiered chunked build
+// calls it chunk after chunk, `base` being the records of the chunks before, without a
+// copy of the chunk's sketch. Records past cap are only counted. SketchAppendTotal: the
+// records of the stream after the last call, base included (synchronises).
+void SketchAppend(Ctx& c, uint32_t first, uint32_t last, uint32_t* out_val, uint64_t* out_org,
+                  uint64_t base, uint64_t cap);
+uint64_t SketchAppendTotal(Ctx& c);
+
 // ---- index.cu ----
 // value_limit: records whose value exceeds it are counted (occurrence threshold)
 // but not indexed - the caller guarantees that no query value is larger
@@ -324,8 +344,14 @@ uint64_t MaxMicromizerValue(Ctx& c, uint32_t first, uint32_t last);
 // again and appends its records to the sort's input - tiered: split into tier A
 // (c.i_val_alt / c.i_org_alt) and bare keys (c.t_b0), at k <= 15, w = 5 straight from
 // the sketch kernel (SketchTiers).
+// tiers = false: the untiered index BuildIndex(c, first, last, minhash) builds, which full
+// sketches may probe (tmax is returned as it came); its records go to c.i_val_alt /
+// c.i_org_alt, at k <= 15, w = 5 straight from the sketch kernel (SketchAppend).
 uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash,
-                           uint64_t chunk, uint64_t tmax);
+                           uint64_t chunk, uint64_t tmax, bool tiers = true);
+// reads [first, last) cut into ranges of >= chunk bases at read boundaries, by the rule
+// that cuts index batches (construct.cc:36-44): boundaries first, ..., last
+std::vector<uint32_t> ChunkCuts(const Ctx& c, uint32_t first, uint32_t last, uint64_t chunk);
 // after the frequency filter of a chunked build: frees what only the build used (the
 // chunk sketch, the sort's second buffers, the tiers' staging and bare keys)
 void ReleaseIndexBuild(Ctx& c);

@@ -653,6 +653,7 @@ void BuildIndexImpl(Ctx& c, ValView src_val, const uint64_t* src_org, uint64_t n
   c.i_valid = false;
   c.i_sorted_ids = false;
   c.i_from_sketch = false;
+  c.i_build_held = false;
   c.occurrence = 0xFFFFFFFFu;
   ++c.i_gen;  // (results derived from an earlier index are stale)
   if (n >= 0xFFFFFFFFULL) {
@@ -866,8 +867,8 @@ void BuildIndexImpl(Ctx& c, ValView src_val, const uint64_t* src_org, uint64_t n
   c.i_valid = true;
 }
 
-// reads [first, last) cut into ranges of >= chunk bases at read boundaries, by the rule
-// that cuts index batches (construct.cc:36-44): boundaries first, ..., last
+}  // namespace
+
 std::vector<uint32_t> ChunkCuts(const Ctx& c, uint32_t first, uint32_t last, uint64_t chunk) {
   std::vector<uint32_t> cuts{first};
   uint64_t bases = 0;
@@ -881,10 +882,8 @@ std::vector<uint32_t> ChunkCuts(const Ctx& c, uint32_t first, uint32_t last, uin
   return cuts;
 }
 
-}  // namespace
-
 uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, uint64_t chunk,
-                           uint64_t tmax) {
+                           uint64_t tmax, bool tiers) {
   c.i_valid = false;
   c.occurrence = 0xFFFFFFFFu;
   if (last > first && (first < c.res_first || last > c.res_last)) {
@@ -936,6 +935,7 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
   // self-join's, for the whole batch), the record count and the coarse value histogram
   // that bounds the tiers ----
   uint64_t n = 0;
+  std::vector<uint64_t> chunk_first{0};  // records before every chunk
   c.jt_val.reserve(nr + 1ULL);
   c.jt_pos.reserve(nr + 1ULL);
   c.h_jt_off.assign(1, 0);
@@ -944,13 +944,14 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
     EnsureSketch(c, r0, r1);  // (exactly the chunk: c.s_n and c.s_val are its records)
     EnsureThresholds(c, r0, r1);
     n += c.s_n;
+    chunk_first.push_back(n);
     RVN_CUDA(cudaMemcpyAsync(c.jt_val.get() + (r0 - first), c.qt_val.get(),
                              (r1 - r0) * sizeof(uint64_t), cudaMemcpyDeviceToDevice, c.stream));
     RVN_CUDA(cudaMemcpyAsync(c.jt_pos.get() + (r0 - first), c.qt_pos.get(),
                              (r1 - r0) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, c.stream));
     const uint64_t base = c.h_jt_off.back();
     for (uint32_t r = 1; r <= r1 - r0; ++r) c.h_jt_off.push_back(base + c.h_q_off[r]);
-    if (k32 && c.s_n > 0) {
+    if (tiers && k32 && c.s_n > 0) {
       ValueHistKernel<<<std::min<unsigned>(CeilDiv(c.s_n, kThreads), c.sms * 4), kThreads, 0,
                         c.stream>>>(reinterpret_cast<const uint32_t*>(c.s_val.get()), c.s_n,
                                     hist_shift, vhist);
@@ -960,7 +961,7 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
   }
   if (n >= 0xFFFFFFFFULL) throw LimitError("index batch holds 2^32 or more minimizers");
   // the tier bound: the largest micromizer value of every read sketched so far
-  if (nr > 0) {
+  if (tiers && nr > 0) {
     if (!k32) {
       tmax = ~0ULL;
     } else {
@@ -973,13 +974,14 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
       tmax = std::max(tmax, ReadU64(c, w));
     }
   }
-  const uint64_t limit = tmax;
+  const uint64_t limit = tiers ? tmax : ~0ULL;
   const bool is32 = k32;
   const bool tiered = Tiered(c, is32, limit, n);
-  // raven's stage-1 parameters: sweep 2 sketches straight into the tiers, and the last
-  // chunk's sketch is not needed any more
+  // raven's stage-1 parameters: sweep 2 sketches straight into the tiers, or untiered into
+  // the sort's second buffers, and the last chunk's sketch is not needed any more
   const bool fused = tiered && SketchTiersFused(c);
-  if (fused) {
+  const bool append = !tiered && SketchTiersFused(c);
+  if (fused || append) {
     c.s_valid = c.q_valid = false;
     c.s_val.release();
     c.s_org.release();
@@ -1021,6 +1023,12 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
       TimerEnd(c);
       continue;
     }
+    if (append) {
+      TimerBegin(c, "sketch_tiers");
+      SketchAppend(c, r0, r1, reinterpret_cast<uint32_t*>(a_val), a_org, chunk_first[i], n);
+      TimerEnd(c);
+      continue;
+    }
     EnsureSketch(c, r0, r1);  // (no-op for a batch of one chunk)
     const uint64_t* sv = c.s_val.get();
     const uint64_t* so = c.s_org.get();
@@ -1055,6 +1063,10 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
       n_a += m;
     }
     TimerEnd(c);
+  }
+  // (sweep 1 counted the same records: the stream ends where its capacity does)
+  if (append && nr > 0 && SketchAppendTotal(c) != n) {
+    throw CudaError("chunked index build: the sweeps disagree on the batch's records");
   }
   c.i_first = first;
   c.i_last = last;

@@ -403,13 +403,19 @@ __device__ __forceinline__ uint64_t LookBack(uint64_t* __restrict__ status, uint
   return excl;
 }
 
-// kTiers: the tier-output mode of the chunked index build (index.cu). The records go to
+// kSketchTiers: the tier-output mode of the chunked index build (index.cu). The records go to
 // two streams in (read, position) order: value <= limit as (value, origin) to out_val /
 // out_org (tier A, capacity out_cap), value > limit as bare keys to out_b (capacity
 // out_cap_b). Each stream has its own status array and look-back (status, status_b), so
 // both counts are exact to 2^62; past its capacity a stream is only counted. tile_out
 // receives the two totals (2 entries) instead of per-tile offsets.
-template <int W, bool kTiers>
+// kSketchAppend: the append mode of the untiered chunked build. One stream, written at
+// out_val / out_org from record out_base on: the look-back chain of the chunk before goes
+// on in this launch. Past out_cap (records of the whole stream) the pass only counts;
+// tile_out[0] receives the stream's running total, out_base included.
+enum SketchOut { kSketchPerTile = 0, kSketchTiers = 1, kSketchAppend = 2 };
+
+template <int W, int kOut>
 __global__ void __launch_bounds__(kSketchThreads, 4)
 SketchFastKernel(const uint64_t* __restrict__ words, const uint64_t* __restrict__ woff,
                  const uint32_t* __restrict__ lens, const uint32_t* __restrict__ ids,
@@ -419,7 +425,9 @@ SketchFastKernel(const uint64_t* __restrict__ words, const uint64_t* __restrict_
                  uint64_t* __restrict__ status, uint64_t* __restrict__ tile_out,
                  uint64_t n_tiles, uint64_t out_cap, uint32_t* __restrict__ out_val,
                  uint64_t* __restrict__ out_org, uint32_t limit, uint64_t* __restrict__ status_b,
-                 uint64_t out_cap_b, uint32_t* __restrict__ out_b) {
+                 uint64_t out_cap_b, uint32_t* __restrict__ out_b, uint64_t out_base) {
+  constexpr bool kTiers = kOut == kSketchTiers;
+  constexpr bool kAppend = kOut == kSketchAppend;
   constexpr uint32_t kBad = 0xFFFFFFFFu;
   constexpr int H = W - 1;
   constexpr int ITEMS = 8;
@@ -627,13 +635,13 @@ SketchFastKernel(const uint64_t* __restrict__ words, const uint64_t* __restrict_
 
   // ---- output offset of the group: decoupled look-back by the first warp ----
   if (threadIdx.x < 32) {
-    const uint64_t excl = LookBack(status, group, group_total);
+    const uint64_t excl = LookBack(status, group, group_total) + (kAppend ? out_base : 0);
     const uint64_t excl_b = kTiers ? LookBack(status_b, group, group_total_b) : 0;
     if (threadIdx.x == 0) {
-      if (kTiers) {
+      if (kTiers || kAppend) {
         if (t_first + g_count == n_tiles) {
           tile_out[0] = excl + group_total;
-          tile_out[1] = excl_b + group_total_b;
+          if (kTiers) tile_out[1] = excl_b + group_total_b;
         }
       } else {
         uint64_t run = excl;
@@ -993,11 +1001,11 @@ void EnsureSketch(Ctx& c, uint32_t first, uint32_t last) {
             }
           }
           if (upto <= launched) continue;
-          SketchFastKernel<5, false><<<static_cast<unsigned>(upto - launched), kSketchThreads, 0,
+          SketchFastKernel<5, kSketchPerTile><<<static_cast<unsigned>(upto - launched), kSketchThreads, 0,
                                        c.stream>>>(
               c.d_words.get(), c.d_woff.get(), c.d_len.get(), c.d_ids.get(),
               c.d_tile_off.get(), c.d_tile_read.get(), first, last, c.prm.k, ticket, status, tout,
-              n_tiles, cap, reinterpret_cast<uint32_t*>(val), org, 0u, nullptr, 0, nullptr);
+              n_tiles, cap, reinterpret_cast<uint32_t*>(val), org, 0u, nullptr, 0, nullptr, 0);
           launched = upto;
           ++c.launches;
         }
@@ -1064,10 +1072,10 @@ void SketchTiers(Ctx& c, uint32_t first, uint32_t last, uint32_t limit, uint32_t
   uint64_t* status_b = status + n_groups + 1;
   unsigned int* ticket = reinterpret_cast<unsigned int*>(status_b + n_groups + 1);
   RVN_CUDA(cudaMemsetAsync(status, 0, (2 * (n_groups + 1) + 2) * sizeof(uint64_t), c.stream));
-  SketchFastKernel<5, true><<<static_cast<unsigned>(n_groups), kSketchThreads, 0, c.stream>>>(
+  SketchFastKernel<5, kSketchTiers><<<static_cast<unsigned>(n_groups), kSketchThreads, 0, c.stream>>>(
       c.d_words.get(), c.d_woff.get(), c.d_len.get(), c.d_ids.get(), c.d_tile_off.get(),
       c.d_tile_read.get(), first, last, c.prm.k, ticket, status, tout, n_tiles, cap_a, a_val,
-      a_org, limit, status_b, cap_b, b_val);
+      a_org, limit, status_b, cap_b, b_val, 0);
   RVN_LAUNCH_CHECK();
   ++c.launches;
   uint64_t* h = c.pin64.reserve(8);
@@ -1076,6 +1084,36 @@ void SketchTiers(Ctx& c, uint32_t first, uint32_t last, uint32_t limit, uint32_t
   *n_a = h[0];
   *n_b = h[1];
 }
+
+void SketchAppend(Ctx& c, uint32_t first, uint32_t last, uint32_t* out_val, uint64_t* out_org,
+                  uint64_t base, uint64_t cap) {
+  if (first < last && (first < c.res_first || last > c.res_last)) {
+    throw StateError("the bases of these reads were not uploaded (rvn_reads_upload_range)");
+  }
+  EnsureTiles(c);
+  WaitUpload(c);
+  const uint64_t n_tiles = c.h_tile_off[last] - c.h_tile_off[first];
+  uint64_t* tout = c.tile_out.reserve(4);
+  if (n_tiles == 0) {  // (nothing to add: the running total stays the chunk's offset)
+    RVN_CUDA(cudaMemcpyAsync(tout, &base, sizeof(uint64_t), cudaMemcpyHostToDevice, c.stream));
+    RVN_CUDA(cudaStreamSynchronize(c.stream));
+    return;
+  }
+  if (n_tiles >= (1ULL << 31)) throw LimitError("too many sketch tiles");
+  const uint64_t n_groups = (n_tiles + kFastGroup - 1) / kFastGroup;
+  uint64_t* status = c.tile_status.reserve(n_groups + 2);
+  unsigned int* ticket = reinterpret_cast<unsigned int*>(status + n_groups + 1);
+  RVN_CUDA(cudaMemsetAsync(status, 0, (n_groups + 2) * sizeof(uint64_t), c.stream));
+  SketchFastKernel<5, kSketchAppend><<<static_cast<unsigned>(n_groups), kSketchThreads, 0,
+                                       c.stream>>>(
+      c.d_words.get(), c.d_woff.get(), c.d_len.get(), c.d_ids.get(), c.d_tile_off.get(),
+      c.d_tile_read.get(), first, last, c.prm.k, ticket, status, tout, n_tiles, cap, out_val,
+      out_org, 0u, nullptr, 0, nullptr, base);
+  RVN_LAUNCH_CHECK();
+  ++c.launches;
+}
+
+uint64_t SketchAppendTotal(Ctx& c) { return ReadU64(c, c.tile_out.get()); }
 
 namespace {
 

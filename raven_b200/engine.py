@@ -302,7 +302,7 @@ class Engine:
         return "stage1_window" in self.timings()
 
     def set_index_chunks(self, bases=-1, budget=0):
-        """How find_overlaps_and_create_piles builds each index batch: 0 in one piece, N > 0
+        """How find_overlaps_and_create_piles and minimize build an index batch: 0 in one piece, N > 0
         in chunks of reads of at least N bases (no sketch of the whole batch is held), -1
         auto (chunks of 2^30 bases only when the one-shot pass does not fit the free device
         memory, or ``budget`` bytes when that is not 0). Same results."""
@@ -320,6 +320,27 @@ class Engine:
     def stage1_index_chunked(self):
         """Whether the last stage-1 call built its index in chunks (phase "sketch_tiers")."""
         return "sketch_tiers" in self.timings()
+
+    def minimize_footprint(self, first, last):
+        """Estimated device memory of minimize(first, last), in bytes: one_shot and chunked
+        builds, and chunk, what the call would do now (0 = one piece, else its chunk size)."""
+        o, ch, k = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        self._check(self.lib.rvn_minimize_footprint(self.h, first, last, C.byref(o),
+                                                    C.byref(ch), C.byref(k)))
+        return dict(one_shot=o.value, chunked=ch.value, chunk=k.value)
+
+    def minimize_chunked(self):
+        """Whether a minimize call since the last "reset_stats" built its index in chunks
+        (phase "sketch_tiers")."""
+        return "sketch_tiers" in self.timings()
+
+    def map_flushes(self):
+        """Flushes of the map calls since the last "reset_stats" that took more than one
+        (one phase "map_flush" each); 0 when every call mapped its range in one piece."""
+        names = C.POINTER(C.c_char_p)()
+        n = C.c_uint32(0)
+        self._check(self.lib.rvn_get_timings(self.h, C.byref(names), None, C.byref(n)))
+        return sum(names[i] == b"map_flush" for i in range(n.value))
 
     def stats(self):
         s = Stats()
