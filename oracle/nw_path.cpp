@@ -64,17 +64,20 @@ std::vector<std::int32_t> DistanceColumn(const char* q, std::int64_t n, const ch
 // then the diagonal. `pref` = experiment knob (ORC_NW_PREF).
 void Traceback(const char* q, std::int64_t n, const char* t, std::int64_t m,
                std::int64_t k, const int* pref, std::string* out) {
-  // band of diagonals j - i in [lo, hi]
-  const std::int64_t lo = -k + std::min<std::int64_t>(0, m - n) - 1;
-  const std::int64_t hi = k + std::max<std::int64_t>(0, m - n) + 1;
-  const std::int64_t width = hi - lo + 1;
+  // band of diagonals j - i in [lo, hi], clipped to the matrix; row i keeps
+  // columns [max(0, i + lo), min(m, i + hi)] (at most m + 1 of them, so a long
+  // query against a short target does not pay for the whole diagonal range)
+  const std::int64_t lo = std::max(-n, -k + std::min<std::int64_t>(0, m - n) - 1);
+  const std::int64_t hi = std::min(m, k + std::max<std::int64_t>(0, m - n) + 1);
+  const std::int64_t width = std::min(hi - lo + 1, m + 1);
   std::vector<std::int32_t> H(static_cast<std::size_t>(n + 1) * width, kInf);
-  auto at = [&](std::int64_t i, std::int64_t j) -> std::int32_t& {
-    return H[static_cast<std::size_t>(i) * width + (j - i - lo)];
+  auto slot = [&](std::int64_t i, std::int64_t j) -> std::size_t {
+    return static_cast<std::size_t>(i) * width + (j - std::max<std::int64_t>(0, i + lo));
   };
+  auto at = [&](std::int64_t i, std::int64_t j) -> std::int32_t& { return H[slot(i, j)]; };
   auto get = [&](std::int64_t i, std::int64_t j) -> std::int32_t {
-    if (i < 0 || j < 0 || j - i < lo || j - i > hi) return kInf;
-    return H[static_cast<std::size_t>(i) * width + (j - i - lo)];
+    if (i < 0 || j < 0 || j > m || j - i < lo || j - i > hi) return kInf;
+    return H[slot(i, j)];
   };
   for (std::int64_t i = 0; i <= n; ++i) {
     const std::int64_t jb = std::max<std::int64_t>(0, i + lo), je = std::min(m, i + hi);

@@ -849,6 +849,10 @@ void AlignBreakingPoints(Ctx& c, uint64_t n, const uint32_t* q_read, const uint3
       ++x1;
     }
     const uint32_t nl = static_cast<uint32_t>(x1 - x0);
+    if (trace) {
+      std::fprintf(stderr, "[rvn::AlignBreakingPoints]   leaves: chunk of %u leaves, %.3f G words of scratch\n",
+                   nl, used * 1e-9);
+    }
     uint64_t* store = c.m_scratch64.reserve(used + 16);
     d_leaves.reserve(nl);
     RVN_CUDA(cudaMemcpyAsync(d_leaves.get(), leaves.data() + x0, nl * sizeof(LeafTask),

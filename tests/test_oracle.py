@@ -331,24 +331,37 @@ def test_product_edlib_equals_oracle(oracle):
              (700, 0.3), (1500, 0.15), (3000, 0.1), (4100, 0.02), (6000, 0.12),
              (10000, 0.1), (12000, 0.01), (11000, 0.15)]
     cases += [(int(rng.integers(1, 900)), float(rng.uniform(0, 0.4))) for _ in range(30)]
+    pairs = []
     for n, err in cases:
         a = rng.integers(0, 4, n, dtype=np.uint8)
         b = synth.mutate(a, rng, err / 3, err / 3, err / 3) if n else a
         if n and rng.random() < 0.3:   # unequal ends
             b = np.concatenate([rng.integers(0, 4, int(rng.integers(0, 40)), dtype=np.uint8), b])
-        sa, sb = letters[a].tobytes(), letters[np.asarray(b, dtype=np.uint8)].tobytes()
+        pairs.append(((n, err), a, np.asarray(b, dtype=np.uint8)))
+    # repeats with many equally good paths, and the leaf / split boundaries and the
+    # split-row fallbacks that the GPU alignment path is tested on
+    import test_gpu_alnpath_edges as edges
+    pairs += [(c, c.q, c.t) for c in edges.build_cases()
+              if c.group in ("ties", "leaf_split", "fallbacks")]
+    t = rng.integers(0, 4, 10_000, dtype=np.uint8)
+    pairs += [("64 at the start of 10 kb", t[:64], t), ("64 at the end of 10 kb", t[-64:], t),
+              ("10 kb against 60", t, t[5000:5060]),
+              ("unrelated 8 kb", rng.integers(0, 4, 8000, dtype=np.uint8), t[:8000])]
+    pairs += [(f"{m} x {n}", t[:m], t[1000:1000 + n]) for m in (320, 321, 384) for n in (8191, 8192)]
+    for case, a, b in pairs:
+        sa, sb = letters[a].tobytes(), letters[b].tobytes()
         d, path = align(sa, sb, 2)
         d0, _ = align(sa, sb, 0)
         assert d == d0
         if max(len(sa), len(sb)) <= 3000:
-            assert d == oracle.edit_distance(sa, sb), (n, err)
+            assert d == oracle.edit_distance(sa, sb), case
         buf = C.create_string_buffer(len(sa) + len(sb) + 1)
         ln = oracle.lib.orc_nw_path(sa, len(sa), sb, len(sb), buf)
         want = buf.raw[:ln]
         got = path.translate(bytes.maketrans(bytes([0, 1, 2, 3]), b"MIDM"))
-        assert got == want, (n, err)
+        assert got == want, case
         assert d == want.count(b"I") + want.count(b"D") + sum(
-            1 for op in path if op == 3), (n, err)
+            1 for op in path if op == 3), case
         # bounded calls: k below the distance -> -1, k at the distance -> found
         if d > 0:
             assert align(sa, sb, 0, d - 1)[0] == -1
