@@ -341,7 +341,14 @@ int rvn_get_stats(rvn_ctx* ctx, rvn_stats* out);
  * (rvn_stage1_footprint), else resident. Results are identical in every
  * mode; a windowed pass takes max_overlaps <= 65536 and leaves phase
  * "stage1_window" in rvn_get_timings); "stage1_window_budget" (bytes: replaces the
- * free device memory in the auto decision, 0 = the free memory); "index_chunk_bases"
+ * free device memory in the auto decision, 0 = the free memory); "stage1_stream" (0/1,
+ * default 1: a resident rvn_find_overlaps_and_create_piles copies the piles and lists of
+ * the reads no later flush touches to the host on a stream of its own while the later
+ * flushes run, lists only at max_overlaps <= 256 and up to 8 GiB of them (the pinned
+ * buffer is sized for max_overlaps records per read); with 0 all of them follow the last
+ * flush. Either way the call returns with every result on the host, the same results,
+ * and phase "results" in rvn_get_timings is the copying that no kernel hides);
+ * "index_chunk_bases"
  * (how rvn_find_overlaps_and_create_piles and rvn_minimize build an index batch: 0 = in one piece,
  * with a sketch of the whole batch; N > 0 = in chunks of reads of >= N bases, cut like
  * the index batches: each chunk is sketched twice, once for its micromizer thresholds and

@@ -442,6 +442,128 @@ class WindowedStage1 {
   uint64_t bb_ = 0;
 };
 
+// Reads whose piles and lists no flush after flush i of the schedule touches (flushes in
+// schedule order): every stage-1 overlap has rhs_id > lhs_id and a flush over the queries
+// [k0, k1) only names reads >= k0, so after flush i that is every read below the first
+// query of every flush still to run - n after the last flush, 0 before the last index
+// batch (each batch's flushes start at read 0 again). Such a read's pile gets no marks
+// (the coverage pass skips it), ListTotals gives its list the old count, at most kmax, which
+// Truncate leaves alone, and its compact offset is a prefix of the same scan.
+std::vector<uint32_t> FinalReads(const std::vector<Batch>& batches, uint32_t n) {
+  std::vector<uint32_t> first;
+  for (const Batch& b : batches) {
+    for (const auto& f : b.flushes) first.push_back(f.first);
+  }
+  std::vector<uint32_t> out(first.size());
+  uint32_t fin = n;
+  for (size_t i = first.size(); i-- > 0;) {
+    out[i] = fin;
+    fin = std::min(fin, first[i]);
+  }
+  return out;
+}
+
+// The pinned list buffer is sized up front for min(kmax, n - 1) records per read: lists of
+// more records per read than this, or more bytes in all, are not streamed.
+constexpr uint64_t kStreamMaxOverlaps = 256;
+constexpr uint64_t kStreamMaxListBytes = 8ULL << 30;
+
+// Resident stage 1, option "stage1_stream": the piles and lists of the reads that are
+// final (FinalReads) go to the pinned host results on c.d2h_stream while the later
+// flushes run, the piles right after a flush's coverage pass, the lists after its gather.
+// Sources: the final prefix of c.p_data, which no later coverage pass touches, and of
+// the current list buffer and offsets, which the gather two flushes later overwrites;
+// c.stream waits for all copies issued so far before every gather (BeforeGather) and at
+// the end (Finish). The pinned buffers are sized before the first copy.
+class ResultStream {
+ public:
+  ResultStream(Ctx& c, uint64_t kmax, uint64_t total_bins) : c_(c) {
+    const uint32_t n = c.n_reads;
+    if (!c.d2h_stream) {
+      RVN_CUDA(cudaStreamCreateWithFlags(&c.d2h_stream, cudaStreamNonBlocking));
+      RVN_CUDA(cudaEventCreateWithFlags(&c.d2h_ready, cudaEventDisableTiming));
+      RVN_CUDA(cudaEventCreateWithFlags(&c.d2h_done, cudaEventDisableTiming));
+    }
+    c.st_pile.reserve(total_bins + 1);
+    c.st_ovl_off.reserve(n + 1ULL)[0] = 0;
+    per_read_ = std::min<uint64_t>(kmax, n ? n - 1 : 0);
+    // a larger kmax: the lists go to the host after the last flush, as without streaming
+    lists_ = per_read_ <= kStreamMaxOverlaps &&
+             per_read_ * n * sizeof(rvn_overlap) <= kStreamMaxListBytes;
+    if (lists_) c.st_ovl.reserve(per_read_ * n + 1);
+  }
+  // (a pass that throws leaves no copy into the pinned buffers behind)
+  ~ResultStream() { cudaStreamSynchronize(c_.d2h_stream); }
+
+  bool lists() const { return lists_; }
+
+  // the piles of reads below `final` are final: c.p_data after the coverage pass
+  void Piles(uint32_t final) {
+    if (final <= pile_read_) return;
+    const std::vector<uint64_t>& off = c_.st_pile_off;
+    const uint64_t b0 = off[pile_read_], b1 = off[final];
+    pile_read_ = final;
+    if (b1 == b0) return;
+    Begin();
+    RVN_CUDA(cudaMemcpyAsync(c_.st_pile.get() + b0, c_.p_data.get() + b0,
+                             (b1 - b0) * sizeof(uint16_t), cudaMemcpyDeviceToHost,
+                             c_.d2h_stream));
+    End();
+  }
+
+  // the lists of reads below `final` are final; final_off: their records (the gather's
+  // compact offset of `final`)
+  void Lists(uint32_t final, uint64_t final_off) {
+    if (!lists_ || final <= list_read_) return;
+    if (final_off + 1 > c_.st_ovl.cap) {
+      // more than min(kmax, n - 1) records per read: grow once the copies are through
+      RVN_CUDA(cudaStreamSynchronize(c_.d2h_stream));
+      c_.st_ovl.reserve_keep(final_off + per_read_ * (c_.n_reads - final) + 1, list_off_);
+    }
+    Begin();
+    RVN_CUDA(cudaMemcpyAsync(c_.st_ovl_off.get() + list_read_ + 1,
+                             c_.g_off.get() + list_read_ + 1,
+                             (final - list_read_) * sizeof(uint64_t), cudaMemcpyDeviceToHost,
+                             c_.d2h_stream));
+    if (final_off > list_off_) {
+      RVN_CUDA(cudaMemcpyAsync(c_.st_ovl.get() + list_off_,
+                               c_.g_list[c_.g_cur].get() + list_off_,
+                               (final_off - list_off_) * sizeof(rvn_overlap),
+                               cudaMemcpyDeviceToHost, c_.d2h_stream));
+    }
+    End();
+    list_read_ = final;
+    list_off_ = final_off;
+  }
+
+  void BeforeGather() {
+    if (issued_) RVN_CUDA(cudaStreamWaitEvent(c_.stream, c_.d2h_done, 0));
+  }
+
+  // after the last flush: c.stream waits for every copy (the lists follow when they
+  // were not streamed)
+  void Finish() {
+    BeforeGather();
+    if (!lists_) GatherFetch(c_);
+  }
+
+ private:
+  void Begin() {
+    RVN_CUDA(cudaEventRecord(c_.d2h_ready, c_.stream));
+    RVN_CUDA(cudaStreamWaitEvent(c_.d2h_stream, c_.d2h_ready, 0));
+  }
+  void End() {
+    RVN_CUDA(cudaEventRecord(c_.d2h_done, c_.d2h_stream));
+    issued_ = true;
+  }
+
+  Ctx& c_;
+  uint64_t per_read_ = 0;
+  bool lists_ = false, issued_ = false;
+  uint32_t pile_read_ = 0, list_read_ = 0;  // reads whose piles / lists are on their way
+  uint64_t list_off_ = 0;                   // records of list_read_ reads
+};
+
 // raven::FindOverlapsAndCreatePiles, same batch / flush schedule as the
 // reference; every step runs on the GPU (Minimize, Filter, Map, AddLayers,
 // gather, truncation); the host only drives the schedule (and, windowed, keeps
@@ -494,6 +616,10 @@ void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
   c.st_mapped = 0;
   std::unique_ptr<WindowedStage1> win;
   if (windowed) win.reset(new WindowedStage1(c, kmax, total_bins));
+  std::unique_ptr<ResultStream> out;
+  if (!windowed && c.stage1_stream) out.reset(new ResultStream(c, kmax, total_bins));
+  const std::vector<uint32_t> final_reads = FinalReads(batches, n);
+  size_t flush = 0;  // index of the flush in the schedule
 
   uint64_t tmax = 0;  // largest micromizer value of the reads sketched so far
   for (const Batch& b : batches) {
@@ -517,13 +643,22 @@ void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
 
     for (const auto& f : b.flushes) {
       MapRange(c, f.first, f.second, true, true, true, false, /*fetch=*/false);
+      const uint32_t final = final_reads[flush++];
       if (win) {
         win->Flush(f.first, f.second);
       } else {
+        // (the flush names no read below f.first)
         PileAddLayersDevice(c, d_pile, d_poff, total_bins, Window::All(n), c.m_ovl.get(),
-                            c.r_n_ovl);
+                            c.r_n_ovl, f.first);
+        uint64_t final_off = 0;
+        if (out) {
+          out->BeforeGather();
+          out->Piles(final);
+        }
         GatherFlush(c, c.m_ovl.get(), c.m_ovl_off.get(), c.r_n_ovl, f.first, f.second, kmax,
-                    Window::All(n));
+                    Window::All(n), nullptr, 0, final,
+                    out && out->lists() ? &final_off : nullptr);
+        if (out) out->Lists(final, final_off);
       }
       c.st_mapped += c.r_n_ovl;
     }
@@ -533,9 +668,17 @@ void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
   if (win) {
     win->Fetch();
   } else {
-    GatherFetch(c);
-    RVN_CUDA(cudaMemcpyAsync(c.st_pile.reserve(total_bins + 1), d_pile,
-                             total_bins * sizeof(uint16_t), cudaMemcpyDeviceToHost, c.stream));
+    // what of the copy to the host still runs after the last kernel
+    TimerBegin(c, "results");
+    if (out) {
+      out->Finish();
+    } else {
+      GatherFetch(c);
+      RVN_CUDA(cudaMemcpyAsync(c.st_pile.reserve(total_bins + 1), d_pile,
+                               total_bins * sizeof(uint16_t), cudaMemcpyDeviceToHost,
+                               c.stream));
+    }
+    TimerEnd(c);
   }
   RVN_CUDA(cudaStreamSynchronize(c.stream));
   TimerCollect(c);
@@ -564,6 +707,9 @@ void SetOption(Ctx& c, const char* name, int64_t value) {
   } else if (name && std::strcmp(name, "stage1_window") == 0) {
     if (value < -1 || value > 1) throw InvalidArgument("stage1_window: -1 (auto), 0 or 1");
     c.stage1_window = value;
+  } else if (name && std::strcmp(name, "stage1_stream") == 0) {
+    if (value != 0 && value != 1) throw InvalidArgument("stage1_stream: 0 or 1");
+    c.stage1_stream = value;
   } else if (name && std::strcmp(name, "stage1_window_budget") == 0) {
     c.stage1_window_budget = value < 0 ? 0 : static_cast<uint64_t>(value);
   } else if (name && std::strcmp(name, "index_chunk_bases") == 0) {
@@ -654,6 +800,12 @@ RVN_API void rvn_ctx_destroy(rvn_ctx* ctx) {
   if (ctx->c.copy_stream) {
     cudaStreamSynchronize(ctx->c.copy_stream);
     cudaStreamDestroy(ctx->c.copy_stream);
+  }
+  if (ctx->c.d2h_stream) {
+    cudaStreamSynchronize(ctx->c.d2h_stream);
+    cudaStreamDestroy(ctx->c.d2h_stream);
+    cudaEventDestroy(ctx->c.d2h_ready);
+    cudaEventDestroy(ctx->c.d2h_done);
   }
   for (auto e : ctx->c.up_events) cudaEventDestroy(e);
   if (ctx->c.up_fence) cudaEventDestroy(ctx->c.up_fence);

@@ -259,6 +259,13 @@ struct Ctx {
   uint64_t st_mapped = 0;
   bool st_valid = false;
   bool st_piles_on_device = false;  // c.p_data / c.p_off still hold the piles of that call
+  // option "stage1_stream": a resident pass copies the piles and lists of the reads no
+  // later flush touches to the host while the later flushes run (1, default), or all
+  // of them after the last flush (0). d2h_stream carries those copies; d2h_ready is
+  // recorded on `stream` when a source is final, d2h_done after the copies
+  int64_t stage1_stream = 1;
+  cudaStream_t d2h_stream = nullptr;
+  cudaEvent_t d2h_ready = nullptr, d2h_done = nullptr;
 
   // ---- read ownership of the stage-1 tail: read r is owned iff r % own_mod ==
   // own_rem (1 / 0 = every read: the single-GPU path) ----
@@ -293,7 +300,9 @@ struct Ctx {
 // ---- utilities (scan.cu) ----
 // out[i] = sum_{j<i} in[j] for i in [0, n]; out has n + 1 entries.
 void ExclusiveScanU32(Ctx& c, const uint32_t* in, uint64_t* out, uint64_t n);
-uint64_t ReadU64(Ctx& c, const uint64_t* dptr);  // sync D2H of one value
+// sync D2H of one value (and of a second one into *value2 when value2 is not null)
+uint64_t ReadU64(Ctx& c, const uint64_t* dptr, const uint64_t* dptr2 = nullptr,
+                 uint64_t* value2 = nullptr);
 
 void TimerBegin(Ctx& c, const char* name);
 void TimerEnd(Ctx& c);
@@ -410,9 +419,12 @@ void GatherReset(Ctx& c);
 // row_off null: the lists are compact (c.g_off) and are re-compacted; otherwise
 // every slot owns a fixed row of row_stride records at row_off[slot] and the lists
 // stay in their rows
+// mark_off (compact lists only): set to the new compact offset of slot `mark`, read
+// back with the lists' total
 void GatherFlush(Ctx& c, const rvn_overlap* ovl, const uint64_t* q_ovl_off,
                  uint64_t m, uint32_t k0, uint32_t k1, uint64_t kmax, const Window& w,
-                 const uint64_t* row_off = nullptr, uint64_t row_stride = 0);
+                 const uint64_t* row_off = nullptr, uint64_t row_stride = 0,
+                 uint32_t mark = 0, uint64_t* mark_off = nullptr);
 void GatherFetch(Ctx& c);
 // the window tables: row_off[s] = s * stride, pile_off[s] = first bin of slot s
 // in a pile buffer that holds the window's piles in slot order (both nw + 1)
@@ -459,9 +471,12 @@ void EditDistanceBatch(Ctx& c, uint64_t n, const uint32_t* lhs_read, const uint3
 
 // ---- pile.cu ----
 // data: device u16 bins of the piles of window `w` in slot order, off: their device
-// u64 offsets (w.size() + 1), `bins` of them in all
+// u64 offsets (w.size() + 1), `bins` of them in all. No overlap may name a pile of a
+// slot below `first`: the coverage pass skips those piles, and neither reads nor
+// writes their bins.
 void PileAddLayersDevice(Ctx& c, uint16_t* d_data, const uint64_t* d_off, uint64_t bins,
-                         const Window& w, const rvn_overlap* d_ovl, uint64_t n_ovl);
+                         const Window& w, const rvn_overlap* d_ovl, uint64_t n_ovl,
+                         uint32_t first = 0);
 
 // ---- poa.cu ---- racon window consensus over a flat batch of windows
 void PoaBatch(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first,

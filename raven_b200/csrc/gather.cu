@@ -178,9 +178,13 @@ void GatherReset(Ctx& c) {
 // overlap names lies in the window `w`; the lists of its reads are indexed by slot.
 void GatherFlush(Ctx& c, const rvn_overlap* ovl, const uint64_t* q_ovl_off,
                  uint64_t m64, uint32_t k0, uint32_t k1, uint64_t kmax, const Window& w,
-                 const uint64_t* row_off, uint64_t row_stride) {
+                 const uint64_t* row_off, uint64_t row_stride, uint32_t mark,
+                 uint64_t* mark_off) {
   const uint32_t n = w.size();
-  if (m64 == 0) return;
+  if (m64 == 0) {
+    if (mark_off) *mark_off = ReadU64(c, c.g_off.get() + mark);
+    return;
+  }
   if (m64 >= 0xFFFFFFFFULL) throw LimitError("2^32 or more overlaps in one flush");
   const uint32_t m = static_cast<uint32_t>(m64);
   TimerBegin(c, "gather");
@@ -242,7 +246,7 @@ void GatherFlush(Ctx& c, const rvn_overlap* ovl, const uint64_t* q_ovl_off,
   } else {
     uint64_t* new_off = c.g_off_alt.reserve(n + 2ULL);
     ExclusiveScanU32(c, kept, new_off, n);
-    const uint64_t new_total = ReadU64(c, new_off + n);
+    const uint64_t new_total = ReadU64(c, new_off + n, new_off + mark, mark_off);
     rvn_overlap* next = c.g_list[c.g_cur ^ 1].reserve(new_total + 1);
     Compact<<<CeilDiv(n, kThreads / 32), kThreads, 0, c.stream>>>(
         stage, t_off, total, c.g_cnt.get(), kept, pairs, kmax, new_off, n, next);

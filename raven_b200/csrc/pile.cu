@@ -45,11 +45,14 @@ __global__ void ScatterMarks(const rvn_overlap* __restrict__ ovl, uint64_t n,
 
 // one warp per pile: inclusive scan of the differences, saturating add,
 // and the differences are cleared for the next call (piles by slot: a window
-// other than all reads is only used with mod == 1)
+// other than all reads is only used with mod == 1). Piles from the owned ones
+// at or above `first` on (first is a multiple of mod).
 __global__ void __launch_bounds__(256)
 ApplyCoverage(uint16_t* __restrict__ data, const uint64_t* __restrict__ bin_off,
-              uint32_t n_piles, uint32_t mod, uint32_t rem, int32_t* __restrict__ diff) {
-  const uint64_t p64 = static_cast<uint64_t>(blockIdx.x * 8 + (threadIdx.x >> 5)) * mod + rem;
+              uint32_t first, uint32_t n_piles, uint32_t mod, uint32_t rem,
+              int32_t* __restrict__ diff) {
+  const uint64_t p64 =
+      first + static_cast<uint64_t>(blockIdx.x * 8 + (threadIdx.x >> 5)) * mod + rem;
   if (p64 >= n_piles) return;
   const uint32_t p = static_cast<uint32_t>(p64);
   const uint32_t lane = threadIdx.x & 31;
@@ -80,9 +83,11 @@ ApplyCoverage(uint16_t* __restrict__ data, const uint64_t* __restrict__ bin_off,
 }  // namespace
 
 void PileAddLayersDevice(Ctx& c, uint16_t* d_data, const uint64_t* d_off, uint64_t bins,
-                         const Window& w, const rvn_overlap* d_ovl, uint64_t n_ovl) {
+                         const Window& w, const rvn_overlap* d_ovl, uint64_t n_ovl,
+                         uint32_t first) {
   const uint32_t n_piles = w.size();
-  if (n_piles == 0 || n_ovl == 0) return;
+  first -= first % c.own_mod;  // (the piles below `first` have no marks)
+  if (n_piles <= first || n_ovl == 0) return;
   const uint64_t slots = bins + n_piles;
   if (c.p_diff.cap < slots) {
     int32_t* d = c.p_diff.reserve(slots);
@@ -91,9 +96,9 @@ void PileAddLayersDevice(Ctx& c, uint16_t* d_data, const uint64_t* d_off, uint64
   TimerBegin(c, "pile");
   ScatterMarks<<<CeilDiv(n_ovl, 256), 256, 0, c.stream>>>(
       d_ovl, n_ovl, d_off, w, c.own_mod, c.own_rem, c.p_diff.get());
-  const uint32_t owned = CeilDiv(n_piles, c.own_mod);
-  ApplyCoverage<<<CeilDiv(owned, 8), 256, 0, c.stream>>>(d_data, d_off, n_piles, c.own_mod,
-                                                         c.own_rem, c.p_diff.get());
+  const uint32_t owned = CeilDiv(n_piles - first, c.own_mod);
+  ApplyCoverage<<<CeilDiv(owned, 8), 256, 0, c.stream>>>(d_data, d_off, first, n_piles,
+                                                         c.own_mod, c.own_rem, c.p_diff.get());
   RVN_LAUNCH_CHECK();
   c.launches += 2;
   TimerEnd(c);

@@ -87,11 +87,25 @@ void ExclusiveScanU32(Ctx& c, const uint32_t* in, uint64_t* out, uint64_t n) {
   c.launches += 3;
 }
 
-uint64_t ReadU64(Ctx& c, const uint64_t* dptr) {
+namespace {
+
+// h: pinned host memory, which the device addresses directly (unified addressing)
+__global__ void ReadBackKernel(const uint64_t* a, const uint64_t* b, uint64_t* h) {
+  h[0] = *a;
+  if (b) h[1] = *b;
+}
+
+}  // namespace
+
+// The values travel as stores of a one-thread kernel, not as a copy: a copy would queue
+// behind whatever the copy engines carry for other streams (stage 1's result copies,
+// megabytes, run beside its flushes). Not counted in c.launches: it stands for a copy.
+uint64_t ReadU64(Ctx& c, const uint64_t* dptr, const uint64_t* dptr2, uint64_t* value2) {
   uint64_t* h = c.pin64.reserve(8);
-  RVN_CUDA(cudaMemcpyAsync(h, dptr, sizeof(uint64_t), cudaMemcpyDeviceToHost,
-                           c.stream));
+  ReadBackKernel<<<1, 1, 0, c.stream>>>(dptr, value2 ? dptr2 : nullptr, h);
+  RVN_LAUNCH_CHECK();
   RVN_CUDA(cudaStreamSynchronize(c.stream));
+  if (value2) *value2 = h[1];
   return h[0];
 }
 
