@@ -46,6 +46,9 @@ class Polisher {
   // counters of the last Polish() (POA windows/s accounting)
   std::uint64_t num_windows() const { return num_windows_; }
   std::uint64_t num_polished_windows() const { return num_polished_windows_; }
+  // windows that ran on the wide (32-bit) consensus kernel: deeper than the 16-bit
+  // kernels take (option "poa_wide" of include/raven_b200.h)
+  std::uint64_t num_wide_windows() const { return num_wide_windows_; }
   double poa_seconds() const { return poa_seconds_; }
   // map (GPU), alignment paths + window cuts (GPU), window packing, consensus (GPU),
   // stitch, layer rules (host pool)
@@ -61,7 +64,7 @@ class Polisher {
   bool trim_;
   std::int8_t m_, n_, g_;
   rvn_ctx* ctx_;
-  std::uint64_t num_windows_ = 0, num_polished_windows_ = 0;
+  std::uint64_t num_windows_ = 0, num_polished_windows_ = 0, num_wide_windows_ = 0;
   double poa_seconds_ = 0;
   double phase_seconds_[6] = {0, 0, 0, 0, 0, 0};
 };

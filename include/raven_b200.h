@@ -282,6 +282,15 @@ int rvn_stage1_results(rvn_ctx* ctx, const rvn_overlap** overlaps,
  * layer, 4095 kept layers in one window, a graph beyond 65000 nodes or edges,
  * and int16 scores: max(|m|,|n|,|g|) * (graph nodes + layer bases + 2) <= 32000
  * for every layer. After a failed call rvn_poa_results is RVN_ERR_STATE.
+ * Option "poa_wide" (rvn_set_option) lifts those limits: 0 (default) as above; 1 the
+ * windows past them - refused up front, or out of graph capacity or int16 range after
+ * the retry at their exact bound - run on a kernel with 32-bit ids and int32 cells
+ * (same results; the other windows take their usual kernels); 2 every window runs on
+ * that kernel (for tests). A wide window's scratch is sized from an estimate and
+ * doubled while it runs out, up to its exact bound; one that does not fit the scratch
+ * budget of a launch even alone is RVN_ERR_LIMIT, naming the bytes it needs. The budget
+ * is 16 GB or half the free device memory, or option "poa_scratch_budget" (bytes) when
+ * that is not 0. Phase "poa_wide" in rvn_get_timings is the wide kernel's share.
  * Results: consensus letters per window (cons_off has n_windows+1 entries),
  * status bit 0 = polished (>= 3 sequences), bit 1 = trimming skipped
  * ("might be chimeric"), coverage per consensus base if requested. */
@@ -292,6 +301,11 @@ int rvn_poa_batch(rvn_ctx* ctx, uint32_t n_windows, const uint32_t* win_first,
 int rvn_poa_results(rvn_ctx* ctx, const char** consensus, const uint64_t** cons_off,
                     const uint8_t** status, const uint32_t** coverage,
                     uint64_t* cells);
+/* The kernels of the last successful rvn_poa_batch: windows[k] = windows that finished
+ * on kernel k, launches[k] = its launches, for k = 0 the register-row (fast) kernel,
+ * 1 the generic kernel, 2 the wide kernel ("poa_wide"). Either pointer may be NULL
+ * (else 3 entries). RVN_ERR_STATE when there are no POA results. */
+int rvn_poa_routes(rvn_ctx* ctx, uint32_t* windows, uint32_t* launches);
 
 /* ---- introspection (parity tests, profiling) ---- */
 
@@ -361,7 +375,8 @@ int rvn_get_stats(rvn_ctx* ctx, rvn_stats* out);
  * upload); "index_chunk_budget" (bytes: replaces the free device memory in that auto
  * decision, 0 = the free memory); "map_flush_bases" (rvn_map cuts its range into flushes of
  * >= N query bases; 0 = the default, from the device memory; for tests of the flush
- * path, results do not depend on it); "reset_stats".
+ * path, results do not depend on it); "poa_wide" and "poa_scratch_budget" (rvn_poa_batch);
+ * "reset_stats".
  * Unknown name or value out of range -> RVN_ERR_INVALID. */
 int rvn_set_option(rvn_ctx* ctx, const char* name, int64_t value);
 

@@ -721,6 +721,12 @@ void SetOption(Ctx& c, const char* name, int64_t value) {
   } else if (name && std::strcmp(name, "map_flush_bases") == 0) {
     if (value < 0) throw InvalidArgument("map_flush_bases: bases, 0 = from the device memory");
     c.map_flush_bases = static_cast<uint64_t>(value);
+  } else if (name && std::strcmp(name, "poa_wide") == 0) {
+    if (value < 0 || value > 2) throw InvalidArgument("poa_wide: 0, 1 or 2");
+    c.poa_wide = value;
+  } else if (name && std::strcmp(name, "poa_scratch_budget") == 0) {
+    if (value < 0) throw InvalidArgument("poa_scratch_budget: bytes, 0 = from the device memory");
+    c.poa_scratch_budget = static_cast<uint64_t>(value);
   } else if (name && std::strcmp(name, "reset_stats") == 0) {
     std::memset(&c.stats, 0, sizeof(c.stats));
     c.launches = 0;
@@ -1134,6 +1140,16 @@ RVN_API int rvn_poa_results(rvn_ctx* ctx, const char** consensus,
     if (status) *status = c.po_h_status.data();
     if (coverage) *coverage = c.po_has_cov ? c.po_out_cov.data() : nullptr;
     if (cells) *cells = c.po_cells;
+  });
+}
+
+RVN_API int rvn_poa_routes(rvn_ctx* ctx, uint32_t* windows, uint32_t* launches) {
+  return Guard(ctx, [&](Ctx& c) {
+    if (!c.poa_valid) throw StateError("no POA results");
+    for (int k = 0; k < 3; ++k) {
+      if (windows) windows[k] = c.po_route_windows[k];
+      if (launches) launches[k] = c.po_route_launches[k];
+    }
   });
 }
 

@@ -250,6 +250,13 @@ struct Ctx {
   uint64_t po_cells = 0;
   uint32_t po_n_windows = 0;
   bool po_has_cov = false, poa_valid = false;
+  // option "poa_wide": 0 (default) windows past the 16-bit kernels' limits fail the call;
+  // 1 they run on the 32-bit kernel; 2 every window does. "poa_scratch_budget" (bytes)
+  // replaces the scratch budget of a launch when it is not 0
+  int64_t poa_wide = 0;
+  uint64_t poa_scratch_budget = 0;
+  // windows and launches of the last rvn_poa_batch per kernel: fast, generic, wide
+  uint32_t po_route_windows[3] = {0, 0, 0}, po_route_launches[3] = {0, 0, 0};
 
   // ---- stage-1 results ----
   PinBuf<rvn_overlap> st_ovl;  // pinned: the D2H of the results runs at link speed

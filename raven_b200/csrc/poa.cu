@@ -48,6 +48,43 @@ struct PoaShape {
   uint32_t width;  // DP row stride (lmax + 1 rounded up to 32)
 };
 
+// The two widths of the generic kernel: one definition of PoaKernel and its helpers,
+// instantiated for each.
+//   PoaNarrow: 16-bit node, edge and order ids and coverage, int16 layer positions and
+//     DP cells - every window of the default contract (65000 window bases, 32000 layer
+//     bases, 4095 layers, 65000 nodes or edges, the int16 score guard).
+//   PoaWide: 32-bit ids, positions and coverage, int32 cells - the windows past those
+//     limits (option "poa_wide"); its order slots are sized per launch.
+struct PoaNarrow {
+  using Id = uint16_t;   // node, edge, order and stack slots; coverage
+  using Pos = int16_t;   // traceback node / layer position, -1 = gap
+  using Cell = int16_t;  // DP cell
+  using Shape = PoaShape;
+  static constexpr Id kNone = 0xFFFF;
+  // |score| <= max(|m|,|n|,|g|) * (rows + len + 2) must stay below this
+  static constexpr long long kCellLimit = 32000;
+  static constexpr int kNoCell = -1000000;     // M of a column past the layer
+  static constexpr int kNoScan = -1000000000;  // scan value of a lane past the layer
+  __host__ __device__ static uint32_t Layers(const Shape&) { return kPoaMaxLayers; }
+};
+
+struct PoaWideShape : PoaShape {
+  uint32_t layers;  // order slots: the most kept layers of a window of the launch
+};
+
+struct PoaWide {
+  using Id = uint32_t;
+  using Pos = int32_t;
+  using Cell = int32_t;
+  using Shape = PoaWideShape;
+  static constexpr Id kNone = 0xFFFFFFFFu;
+  // far beyond any window (2^28 / 127 > 2 million rows + bases) and far inside int32
+  static constexpr long long kCellLimit = 1LL << 28;
+  static constexpr int kNoCell = -(1 << 29);
+  static constexpr int kNoScan = -(1 << 30);
+  __host__ __device__ static uint32_t Layers(const Shape& s) { return s.layers; }
+};
+
 // byte offsets of the arrays inside one window's scratch slab
 struct PoaLayout {
   size_t code, n_aligned, marks, ignored, in_sub, sink;
@@ -56,7 +93,9 @@ struct PoaLayout {
   size_t aln_node, aln_pos, pred, score, H, bytes;
 };
 
-__host__ __device__ inline PoaLayout MakePoaLayout(const PoaShape& s) {
+template <class W>
+__host__ __device__ inline PoaLayout MakePoaLayout(const typename W::Shape& s) {
+  constexpr size_t id = sizeof(typename W::Id), pos = sizeof(typename W::Pos);
   PoaLayout L;
   size_t o = 0;
   auto take = [&](size_t bytes) {
@@ -70,38 +109,40 @@ __host__ __device__ inline PoaLayout MakePoaLayout(const PoaShape& s) {
   L.ignored = take(s.ncap);
   L.in_sub = take(s.ncap);
   L.sink = take(s.ncap);
-  L.in_head = take(2ULL * s.ncap);
-  L.in_tail = take(2ULL * s.ncap);
-  L.out_head = take(2ULL * s.ncap);
-  L.aligned = take(2ULL * 3 * s.ncap);
-  L.cov = take(2ULL * s.ncap);
-  L.r2n = take(2ULL * s.ncap);
-  L.n2r = take(2ULL * s.ncap);
-  L.stack = take(2ULL * 4 * s.ncap);
-  L.order = take(2ULL * (kPoaMaxLayers + 1));
-  L.e_tail = take(2ULL * s.ecap);
-  L.e_head = take(2ULL * s.ecap);
-  L.e_next_in = take(2ULL * s.ecap);
-  L.e_next_out = take(2ULL * s.ecap);
+  L.in_head = take(id * s.ncap);
+  L.in_tail = take(id * s.ncap);
+  L.out_head = take(id * s.ncap);
+  L.aligned = take(id * 3 * s.ncap);
+  L.cov = take(id * s.ncap);
+  L.r2n = take(id * s.ncap);
+  L.n2r = take(id * s.ncap);
+  L.stack = take(id * 4 * s.ncap);
+  L.order = take(id * (W::Layers(s) + 1));
+  L.e_tail = take(id * s.ecap);
+  L.e_head = take(id * s.ecap);
+  L.e_next_in = take(id * s.ecap);
+  L.e_next_out = take(id * s.ecap);
   L.e_weight = take(4ULL * s.ecap);
-  L.aln_node = take(2ULL * (s.ncap + s.lmax + 2));
-  L.aln_pos = take(2ULL * (s.ncap + s.lmax + 2));
+  L.aln_node = take(pos * (s.ncap + s.lmax + 2));
+  L.aln_pos = take(pos * (s.ncap + s.lmax + 2));
   L.pred = take(4ULL * s.ncap);
   L.score = take(8ULL * s.ncap);
-  L.H = take(2ULL * s.rows * s.width);
+  L.H = take(sizeof(typename W::Cell) * s.rows * s.width);
   L.bytes = o;
   return L;
 }
 
+template <class W>
 struct PoaGraph {
+  using Id = typename W::Id;
   uint8_t *code, *n_aligned, *marks, *ignored, *in_sub, *sink;
-  uint16_t *in_head, *in_tail, *out_head, *aligned, *cov, *r2n, *n2r, *stack, *order;
-  uint16_t *e_tail, *e_head, *e_next_in, *e_next_out;
+  Id *in_head, *in_tail, *out_head, *aligned, *cov, *r2n, *n2r, *stack, *order;
+  Id *e_tail, *e_head, *e_next_in, *e_next_out;
   int32_t* e_weight;
-  int16_t *aln_node, *aln_pos;
+  typename W::Pos *aln_node, *aln_pos;
   int32_t* pred;
   long long* score;
-  int16_t* H;
+  typename W::Cell* H;
   uint32_t n_nodes, n_edges, ncap, ecap, stack_cap;
   bool overflow;
 };
@@ -144,13 +185,15 @@ __device__ uint32_t KeptSequences(const uint64_t* seq_off, const uint32_t* seq_b
 // status that ends the window: racon's coordinate check (with end < L0, as a
 // layer's end is a node of the backbone chain), a layer beyond `lmax` bases, or
 // more layers than order[] holds (PoaBatch refuses those before any launch).
-__device__ uint32_t OrderLayers(uint16_t* order, const uint64_t* seq_off,
+template <class Order>
+__device__ uint32_t OrderLayers(Order* order, const uint64_t* seq_off,
                                 const uint32_t* seq_begin, const uint32_t* seq_end,
-                                uint32_t s0, uint32_t s1, uint32_t L0, uint32_t lmax) {
+                                uint32_t s0, uint32_t s1, uint32_t L0, uint32_t lmax,
+                                uint32_t max_layers = kPoaMaxLayers) {
   uint32_t n = 0;
   for (uint32_t s = s0 + 1; s < s1; ++s) {
     if (!LayerKept(seq_off, seq_begin, seq_end, s)) continue;
-    if (n >= kPoaMaxLayers) return kPoaStatusCapacity;
+    if (n >= max_layers) return kPoaStatusCapacity;
     if (seq_begin[s] > seq_end[s] || seq_end[s] >= L0) return kPoaStatusInvalid;
     if (seq_off[s + 1] - seq_off[s] > lmax) return kPoaStatusInvalid;
     uint32_t b = n++;
@@ -158,12 +201,13 @@ __device__ uint32_t OrderLayers(uint16_t* order, const uint64_t* seq_off,
       order[b] = order[b - 1];
       --b;
     }
-    order[b] = static_cast<uint16_t>(s - s0);
+    order[b] = static_cast<Order>(s - s0);
   }
   return 0;
 }
 
-__device__ uint16_t AddNode(PoaGraph& g, uint32_t code) {
+template <class W>
+__device__ typename W::Id AddNode(PoaGraph<W>& g, uint32_t code) {
   if (g.n_nodes >= g.ncap) {
     g.overflow = true;
     return 0;
@@ -171,16 +215,18 @@ __device__ uint16_t AddNode(PoaGraph& g, uint32_t code) {
   const uint32_t v = g.n_nodes++;
   g.code[v] = static_cast<uint8_t>(code);
   g.n_aligned[v] = 0;
-  g.in_head[v] = g.in_tail[v] = g.out_head[v] = kNone;
+  g.in_head[v] = g.in_tail[v] = g.out_head[v] = W::kNone;
   g.cov[v] = 0;
-  return static_cast<uint16_t>(v);
+  return static_cast<typename W::Id>(v);
 }
 
 // spoa Graph::AddEdge: bump the weight of an existing edge or append a new
 // one at the END of both adjacency lists (insertion order is observable)
-__device__ void AddEdge(PoaGraph& g, uint16_t tail, uint16_t head, int32_t w) {
-  uint16_t last_out = kNone;
-  for (uint16_t e = g.out_head[tail]; e != kNone; e = g.e_next_out[e]) {
+template <class W>
+__device__ void AddEdge(PoaGraph<W>& g, typename W::Id tail, typename W::Id head, int32_t w) {
+  using Id = typename W::Id;
+  Id last_out = W::kNone;
+  for (Id e = g.out_head[tail]; e != W::kNone; e = g.e_next_out[e]) {
     if (g.e_head[e] == head) {
       g.e_weight[e] += w;
       return;
@@ -191,17 +237,17 @@ __device__ void AddEdge(PoaGraph& g, uint16_t tail, uint16_t head, int32_t w) {
     g.overflow = true;
     return;
   }
-  const uint16_t e = static_cast<uint16_t>(g.n_edges++);
+  const Id e = static_cast<Id>(g.n_edges++);
   g.e_tail[e] = tail;
   g.e_head[e] = head;
   g.e_weight[e] = w;
-  g.e_next_in[e] = g.e_next_out[e] = kNone;
-  if (last_out == kNone) {
+  g.e_next_in[e] = g.e_next_out[e] = W::kNone;
+  if (last_out == W::kNone) {
     g.out_head[tail] = e;
   } else {
     g.e_next_out[last_out] = e;
   }
-  if (g.in_head[head] == kNone) {
+  if (g.in_head[head] == W::kNone) {
     g.in_head[head] = e;
   } else {
     g.e_next_in[g.in_tail[head]] = e;
@@ -219,15 +265,17 @@ struct SeqView {
   }
 };
 
-// a chain of fresh nodes for s[begin, end); returns its first node or kNone
-__device__ uint16_t AddChain(PoaGraph& g, const SeqView& s, uint32_t begin,
-                             uint32_t end) {
-  if (begin == end) return kNone;
-  uint16_t first = kNone, prev = kNone;
+// a chain of fresh nodes for s[begin, end); returns its first node or W::kNone
+template <class W>
+__device__ typename W::Id AddChain(PoaGraph<W>& g, const SeqView& s, uint32_t begin,
+                                   uint32_t end) {
+  using Id = typename W::Id;
+  if (begin == end) return W::kNone;
+  Id first = W::kNone, prev = W::kNone;
   for (uint32_t i = begin; i < end && !g.overflow; ++i) {
-    const uint16_t cur = AddNode(g, CodeOf(s.bases[i]));
-    if (prev != kNone) AddEdge(g, prev, cur, s.weight(i - 1) + s.weight(i));
-    if (first == kNone) first = cur;
+    const Id cur = AddNode(g, CodeOf(s.bases[i]));
+    if (prev != W::kNone) AddEdge(g, prev, cur, s.weight(i - 1) + s.weight(i));
+    if (first == W::kNone) first = cur;
     prev = cur;
   }
   return first;
@@ -236,7 +284,9 @@ __device__ uint16_t AddChain(PoaGraph& g, const SeqView& s, uint32_t begin,
 // spoa Graph::TopologicalSort restricted to the nodes with in_sub != 0
 // (Graph::Subgraph keeps relative ids and adjacency order, so the restricted
 // DFS over the full graph yields exactly the sub-graph's order)
-__device__ uint32_t TopoSort(PoaGraph& g) {
+template <class W>
+__device__ uint32_t TopoSort(PoaGraph<W>& g) {
+  using Id = typename W::Id;
   const uint32_t n = g.n_nodes;
   for (uint32_t v = 0; v < n; ++v) {
     g.marks[v] = 0;
@@ -245,13 +295,13 @@ __device__ uint32_t TopoSort(PoaGraph& g) {
   uint32_t rank = 0, sp = 0;
   for (uint32_t root = 0; root < n; ++root) {
     if (!g.in_sub[root] || g.marks[root] != 0) continue;
-    g.stack[sp++] = static_cast<uint16_t>(root);
+    g.stack[sp++] = static_cast<Id>(root);
     while (sp > 0) {
-      const uint16_t cur = g.stack[sp - 1];
+      const Id cur = g.stack[sp - 1];
       bool valid = true;
       if (g.marks[cur] != 2) {
-        for (uint16_t e = g.in_head[cur]; e != kNone; e = g.e_next_in[e]) {
-          const uint16_t t = g.e_tail[e];
+        for (Id e = g.in_head[cur]; e != W::kNone; e = g.e_next_in[e]) {
+          const Id t = g.e_tail[e];
           if (g.in_sub[t] && g.marks[t] != 2) {
             if (sp >= g.stack_cap) {
               g.overflow = true;
@@ -263,7 +313,7 @@ __device__ uint32_t TopoSort(PoaGraph& g) {
         }
         if (!g.ignored[cur]) {
           for (uint32_t a = 0; a < g.n_aligned[cur]; ++a) {
-            const uint16_t t = g.aligned[3 * cur + a];
+            const Id t = g.aligned[3 * cur + a];
             if (g.in_sub[t] && g.marks[t] != 2) {
               if (sp >= g.stack_cap) {
                 g.overflow = true;
@@ -278,12 +328,12 @@ __device__ uint32_t TopoSort(PoaGraph& g) {
         if (valid) {
           g.marks[cur] = 2;
           if (!g.ignored[cur]) {
-            g.n2r[cur] = static_cast<uint16_t>(rank);
+            g.n2r[cur] = static_cast<Id>(rank);
             g.r2n[rank++] = cur;
             for (uint32_t a = 0; a < g.n_aligned[cur]; ++a) {
-              const uint16_t t = g.aligned[3 * cur + a];
+              const Id t = g.aligned[3 * cur + a];
               if (g.in_sub[t]) {
-                g.n2r[t] = static_cast<uint16_t>(rank);
+                g.n2r[t] = static_cast<Id>(rank);
                 g.r2n[rank++] = t;
               }
             }
@@ -300,14 +350,16 @@ __device__ uint32_t TopoSort(PoaGraph& g) {
 
 // spoa Graph::ExtractSubgraph(nodes[end], nodes[begin]): backward reachability
 // from `from` through in-edges and aligned nodes, keeping ids >= min_id
-__device__ void MarkSubgraph(PoaGraph& g, uint32_t from, uint32_t min_id) {
+template <class W>
+__device__ void MarkSubgraph(PoaGraph<W>& g, uint32_t from, uint32_t min_id) {
+  using Id = typename W::Id;
   for (uint32_t v = 0; v < g.n_nodes; ++v) g.in_sub[v] = 0;
   uint32_t sp = 0;
-  g.stack[sp++] = static_cast<uint16_t>(from);
+  g.stack[sp++] = static_cast<Id>(from);
   while (sp > 0) {
-    const uint16_t cur = g.stack[--sp];
+    const Id cur = g.stack[--sp];
     if (g.in_sub[cur] || cur < min_id) continue;
-    for (uint16_t e = g.in_head[cur]; e != kNone; e = g.e_next_in[e]) {
+    for (Id e = g.in_head[cur]; e != W::kNone; e = g.e_next_in[e]) {
       if (sp >= g.stack_cap) {
         g.overflow = true;
         return;
@@ -326,7 +378,9 @@ __device__ void MarkSubgraph(PoaGraph& g, uint32_t from, uint32_t min_id) {
 }
 
 // spoa Graph::AddAlignment (alignment non-empty)
-__device__ void AddAlignment(PoaGraph& g, const SeqView& s, uint32_t aln_len) {
+template <class W>
+__device__ void AddAlignment(PoaGraph<W>& g, const SeqView& s, uint32_t aln_len) {
+  using Id = typename W::Id;
   // valid = sequence positions that appear in the alignment
   int32_t first_pos = -1, last_pos = -1;
   for (uint32_t i = 0; i < aln_len; ++i) {
@@ -336,9 +390,9 @@ __device__ void AddAlignment(PoaGraph& g, const SeqView& s, uint32_t aln_len) {
     }
   }
   const uint32_t before = g.n_nodes;
-  uint16_t begin = AddChain(g, s, 0, first_pos);
-  uint16_t prev = before == g.n_nodes ? kNone : static_cast<uint16_t>(g.n_nodes - 1);
-  const uint16_t last = AddChain(g, s, last_pos + 1, s.len);
+  Id begin = AddChain(g, s, 0, first_pos);
+  Id prev = before == g.n_nodes ? W::kNone : static_cast<Id>(g.n_nodes - 1);
+  const Id last = AddChain(g, s, last_pos + 1, s.len);
   // count this sequence on the chains (coverage = sequences through a node)
   const bool counts = s.len >= 2;
   if (counts) {
@@ -348,27 +402,27 @@ __device__ void AddAlignment(PoaGraph& g, const SeqView& s, uint32_t aln_len) {
     const int32_t pos = g.aln_pos[i];
     if (pos == -1) continue;
     const uint32_t code = CodeOf(s.bases[pos]);
-    uint16_t cur = kNone;
+    Id cur = W::kNone;
     if (g.aln_node[i] == -1) {
       cur = AddNode(g, code);
     } else {
-      const uint16_t jt = static_cast<uint16_t>(g.aln_node[i]);
+      const Id jt = static_cast<Id>(g.aln_node[i]);
       if (g.code[jt] == code) {
         cur = jt;
       } else {
         for (uint32_t a = 0; a < g.n_aligned[jt]; ++a) {
-          const uint16_t kt = g.aligned[3 * jt + a];
+          const Id kt = g.aligned[3 * jt + a];
           if (g.code[kt] == code) {
             cur = kt;
             break;
           }
         }
-        if (cur == kNone) {  // a new letter for this column
+        if (cur == W::kNone) {  // a new letter for this column
           cur = AddNode(g, code);
           if (g.overflow) break;
           const uint32_t na = g.n_aligned[jt];
           for (uint32_t a = 0; a < na; ++a) {
-            const uint16_t kt = g.aligned[3 * jt + a];
+            const Id kt = g.aligned[3 * jt + a];
             g.aligned[3 * kt + g.n_aligned[kt]++] = cur;
             g.aligned[3 * cur + g.n_aligned[cur]++] = kt;
           }
@@ -379,25 +433,29 @@ __device__ void AddAlignment(PoaGraph& g, const SeqView& s, uint32_t aln_len) {
     }
     if (g.overflow) break;
     if (counts) g.cov[cur] += 1;
-    if (begin == kNone) begin = cur;
-    if (prev != kNone) AddEdge(g, prev, cur, s.weight(pos - 1) + s.weight(pos));
+    if (begin == W::kNone) begin = cur;
+    if (prev != W::kNone) AddEdge(g, prev, cur, s.weight(pos - 1) + s.weight(pos));
     prev = cur;
   }
-  if (last != kNone && !g.overflow) {
+  if (last != W::kNone && !g.overflow) {
     AddEdge(g, prev, last, s.weight(last_pos) + s.weight(last_pos + 1));
   }
 }
 
+template <class W>
 __global__ void __launch_bounds__(32)
 PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
           const uint32_t* __restrict__ win_first, const uint64_t* __restrict__ seq_off,
           const uint8_t* __restrict__ bases, const uint8_t* __restrict__ quals,
           const uint32_t* __restrict__ seq_begin, const uint32_t* __restrict__ seq_end,
-          int m, int n, int gap, int trim, int tgs, PoaShape shape,
+          int m, int n, int gap, int trim, int tgs, typename W::Shape shape,
           uint8_t* __restrict__ scratch, size_t scratch_stride,
           uint8_t* __restrict__ cons, const uint64_t* __restrict__ cons_off,
           uint32_t* __restrict__ cons_len, uint32_t* __restrict__ cov_out,
           uint8_t* __restrict__ status, unsigned long long* __restrict__ cells) {
+  using Id = typename W::Id;
+  using Pos = typename W::Pos;
+  using Cell = typename W::Cell;
   if (blockIdx.x >= n_windows) return;
   const uint32_t lane = threadIdx.x;
   const uint32_t w = win_list ? win_list[blockIdx.x] : blockIdx.x;
@@ -435,8 +493,8 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
   }
 
   uint8_t* base = scratch + scratch_stride * blockIdx.x;
-  const PoaLayout L = MakePoaLayout(shape);
-  __shared__ PoaGraph g;
+  const PoaLayout L = MakePoaLayout<W>(shape);
+  __shared__ PoaGraph<W> g;
   __shared__ uint32_t sh_rows, sh_fail;
   if (lane == 0) {
     g.code = base + L.code;
@@ -445,32 +503,33 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
     g.ignored = base + L.ignored;
     g.in_sub = base + L.in_sub;
     g.sink = base + L.sink;
-    g.in_head = reinterpret_cast<uint16_t*>(base + L.in_head);
-    g.in_tail = reinterpret_cast<uint16_t*>(base + L.in_tail);
-    g.out_head = reinterpret_cast<uint16_t*>(base + L.out_head);
-    g.aligned = reinterpret_cast<uint16_t*>(base + L.aligned);
-    g.cov = reinterpret_cast<uint16_t*>(base + L.cov);
-    g.r2n = reinterpret_cast<uint16_t*>(base + L.r2n);
-    g.n2r = reinterpret_cast<uint16_t*>(base + L.n2r);
-    g.stack = reinterpret_cast<uint16_t*>(base + L.stack);
-    g.order = reinterpret_cast<uint16_t*>(base + L.order);
-    g.e_tail = reinterpret_cast<uint16_t*>(base + L.e_tail);
-    g.e_head = reinterpret_cast<uint16_t*>(base + L.e_head);
-    g.e_next_in = reinterpret_cast<uint16_t*>(base + L.e_next_in);
-    g.e_next_out = reinterpret_cast<uint16_t*>(base + L.e_next_out);
+    g.in_head = reinterpret_cast<Id*>(base + L.in_head);
+    g.in_tail = reinterpret_cast<Id*>(base + L.in_tail);
+    g.out_head = reinterpret_cast<Id*>(base + L.out_head);
+    g.aligned = reinterpret_cast<Id*>(base + L.aligned);
+    g.cov = reinterpret_cast<Id*>(base + L.cov);
+    g.r2n = reinterpret_cast<Id*>(base + L.r2n);
+    g.n2r = reinterpret_cast<Id*>(base + L.n2r);
+    g.stack = reinterpret_cast<Id*>(base + L.stack);
+    g.order = reinterpret_cast<Id*>(base + L.order);
+    g.e_tail = reinterpret_cast<Id*>(base + L.e_tail);
+    g.e_head = reinterpret_cast<Id*>(base + L.e_head);
+    g.e_next_in = reinterpret_cast<Id*>(base + L.e_next_in);
+    g.e_next_out = reinterpret_cast<Id*>(base + L.e_next_out);
     g.e_weight = reinterpret_cast<int32_t*>(base + L.e_weight);
-    g.aln_node = reinterpret_cast<int16_t*>(base + L.aln_node);
-    g.aln_pos = reinterpret_cast<int16_t*>(base + L.aln_pos);
+    g.aln_node = reinterpret_cast<Pos*>(base + L.aln_node);
+    g.aln_pos = reinterpret_cast<Pos*>(base + L.aln_pos);
     g.pred = reinterpret_cast<int32_t*>(base + L.pred);
     g.score = reinterpret_cast<long long*>(base + L.score);
-    g.H = reinterpret_cast<int16_t*>(base + L.H);
+    g.H = reinterpret_cast<Cell*>(base + L.H);
     g.n_nodes = g.n_edges = 0;
     g.ncap = shape.ncap;
     g.ecap = shape.ecap;
     g.stack_cap = 4 * shape.ncap;
     g.overflow = false;
     // layer coordinates are validated up front
-    sh_fail = OrderLayers(g.order, seq_off, seq_begin, seq_end, s0, s1, L0, shape.lmax);
+    sh_fail = OrderLayers(g.order, seq_off, seq_begin, seq_end, s0, s1, L0, shape.lmax,
+                          W::Layers(shape));
     if (!sh_fail) {
       // backbone chain (spoa AddAlignment with an empty alignment): its edges weigh
       // by its own qualities when the batch has qualities, and 0 when it has none
@@ -484,7 +543,7 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
   __syncwarp();
 
   const uint32_t offset = static_cast<uint32_t>(0.01 * L0);
-  const uint32_t W = shape.width;
+  const uint32_t width = shape.width;
   unsigned long long my_cells = 0;
 
   for (uint32_t li = 0; li + 1 < nseq; ++li) {
@@ -505,9 +564,9 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
       uint32_t rows = g.overflow ? 0 : TopoSort(g);
       // a node is a sink if it has no out-edge inside the (sub)graph
       for (uint32_t r = 0; r < rows; ++r) {
-        const uint16_t v = g.r2n[r];
+        const Id v = g.r2n[r];
         uint8_t sink = 1;
-        for (uint16_t e = g.out_head[v]; e != kNone; e = g.e_next_out[e]) {
+        for (Id e = g.out_head[v]; e != W::kNone; e = g.e_next_out[e]) {
           if (g.in_sub[g.e_head[e]]) {
             sink = 0;
             break;
@@ -515,9 +574,9 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
         }
         g.sink[v] = sink;
       }
-      // int16 cells: |score| <= max|m,n,g| * (rows + columns)
+      // the cells' range: |score| <= max|m,n,g| * (rows + columns)
       const int amax = max(max(abs(m), abs(n)), abs(gap));
-      if (static_cast<long long>(amax) * (rows + len + 2) > 32000) g.overflow = true;
+      if (static_cast<long long>(amax) * (rows + len + 2) > W::kCellLimit) g.overflow = true;
       sh_rows = rows;
     }
     __syncwarp();
@@ -526,39 +585,39 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
     my_cells += static_cast<unsigned long long>(rows + 1) * (len + 1);
 
     // ---- DP (all lanes) ----
-    int16_t* H = g.H;
-    for (uint32_t j = lane; j <= len; j += 32) H[j] = static_cast<int16_t>(j * gap);
+    Cell* H = g.H;
+    for (uint32_t j = lane; j <= len; j += 32) H[j] = static_cast<Cell>(j * gap);
     __syncwarp();
     int best_score = -2147483647, best_row = -1;
     for (uint32_t r = 0; r < rows; ++r) {
-      const uint16_t v = g.r2n[r];
+      const Id v = g.r2n[r];
       const uint32_t vcode = g.code[v];
-      int16_t* row = H + static_cast<size_t>(r + 1) * W;
+      Cell* row = H + static_cast<size_t>(r + 1) * width;
       // column 0
       int col0 = 0;
       {
         bool any = false;
         int pen = -2147483647;
-        for (uint16_t e = g.in_head[v]; e != kNone; e = g.e_next_in[e]) {
-          const uint16_t t = g.e_tail[e];
+        for (Id e = g.in_head[v]; e != W::kNone; e = g.e_next_in[e]) {
+          const Id t = g.e_tail[e];
           if (!g.in_sub[t]) continue;
           any = true;
-          pen = max(pen, static_cast<int>(H[static_cast<size_t>(g.n2r[t] + 1) * W]));
+          pen = max(pen, static_cast<int>(H[static_cast<size_t>(g.n2r[t] + 1) * width]));
         }
         col0 = (any ? pen : 0) + gap;
       }
       int carry = col0;  // running max of M[k] - k*g over k < chunk start (k = 0 term)
       for (uint32_t c0 = 1; c0 <= len; c0 += 32) {
         const uint32_t j = c0 + lane;
-        int M = -1000000;
+        int M = W::kNoCell;
         if (j <= len) {
           const int match = (static_cast<uint32_t>(CodeOf(sv.bases[j - 1])) == vcode) ? m : n;
           bool any = false;
-          for (uint16_t e = g.in_head[v]; e != kNone; e = g.e_next_in[e]) {
-            const uint16_t t = g.e_tail[e];
+          for (Id e = g.in_head[v]; e != W::kNone; e = g.e_next_in[e]) {
+            const Id t = g.e_tail[e];
             if (!g.in_sub[t]) continue;
             any = true;
-            const int16_t* pr = H + static_cast<size_t>(g.n2r[t] + 1) * W;
+            const Cell* pr = H + static_cast<size_t>(g.n2r[t] + 1) * width;
             M = max(M, max(static_cast<int>(pr[j - 1]) + match,
                            static_cast<int>(pr[j]) + gap));
           }
@@ -567,17 +626,17 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
           }
         }
         // horizontal recurrence as a max-scan of T = M - j*g
-        int T = j <= len ? M - static_cast<int>(j) * gap : -1000000000;
+        int T = j <= len ? M - static_cast<int>(j) * gap : W::kNoScan;
 #pragma unroll
         for (int d = 1; d < 32; d <<= 1) {
           const int o = __shfl_up_sync(0xffffffffu, T, d);
           if (static_cast<int>(lane) >= d) T = max(T, o);
         }
         T = max(T, carry);
-        if (j <= len) row[j] = static_cast<int16_t>(T + static_cast<int>(j) * gap);
+        if (j <= len) row[j] = static_cast<Cell>(T + static_cast<int>(j) * gap);
         carry = __shfl_sync(0xffffffffu, T, 31);
       }
-      if (lane == 0) row[0] = static_cast<int16_t>(col0);
+      if (lane == 0) row[0] = static_cast<Cell>(col0);
       __syncwarp();
       if (g.sink[v]) {
         const int sc = row[len];
@@ -595,20 +654,20 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
       if (best_row < 0) j = 0;
       const uint32_t acap = shape.ncap + shape.lmax + 2;
       while (!(i == 0 && j == 0)) {
-        const int h = H[static_cast<size_t>(i) * W + j];
+        const int h = H[static_cast<size_t>(i) * width + j];
         uint32_t pi = 0, pj = 0;
         bool found = false;
         if (i != 0 && j != 0) {
-          const uint16_t v = g.r2n[i - 1];
+          const Id v = g.r2n[i - 1];
           const int match =
               (static_cast<uint32_t>(CodeOf(sv.bases[j - 1])) == g.code[v]) ? m : n;
           bool any = false;
-          for (uint16_t e = g.in_head[v]; e != kNone && !found; e = g.e_next_in[e]) {
-            const uint16_t t = g.e_tail[e];
+          for (Id e = g.in_head[v]; e != W::kNone && !found; e = g.e_next_in[e]) {
+            const Id t = g.e_tail[e];
             if (!g.in_sub[t]) continue;
             any = true;
             const uint32_t p = g.n2r[t] + 1;
-            if (h == H[static_cast<size_t>(p) * W + (j - 1)] + match) {
+            if (h == H[static_cast<size_t>(p) * width + (j - 1)] + match) {
               pi = p;
               pj = j - 1;
               found = true;
@@ -621,14 +680,14 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
           }
         }
         if (!found && i != 0) {
-          const uint16_t v = g.r2n[i - 1];
+          const Id v = g.r2n[i - 1];
           bool any = false;
-          for (uint16_t e = g.in_head[v]; e != kNone && !found; e = g.e_next_in[e]) {
-            const uint16_t t = g.e_tail[e];
+          for (Id e = g.in_head[v]; e != W::kNone && !found; e = g.e_next_in[e]) {
+            const Id t = g.e_tail[e];
             if (!g.in_sub[t]) continue;
             any = true;
             const uint32_t p = g.n2r[t] + 1;
-            if (h == H[static_cast<size_t>(p) * W + j] + gap) {
+            if (h == H[static_cast<size_t>(p) * width + j] + gap) {
               pi = p;
               pj = j;
               found = true;
@@ -640,7 +699,7 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
             found = true;
           }
         }
-        if (!found && j != 0 && h == H[static_cast<size_t>(i) * W + j - 1] + gap) {
+        if (!found && j != 0 && h == H[static_cast<size_t>(i) * width + j - 1] + gap) {
           pi = i;
           pj = j - 1;
           found = true;
@@ -649,15 +708,15 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
           g.overflow = true;
           break;
         }
-        g.aln_node[alen] = i == pi ? -1 : static_cast<int16_t>(g.r2n[i - 1]);
-        g.aln_pos[alen] = j == pj ? -1 : static_cast<int16_t>(j - 1);
+        g.aln_node[alen] = i == pi ? -1 : static_cast<Pos>(g.r2n[i - 1]);
+        g.aln_pos[alen] = j == pj ? -1 : static_cast<Pos>(j - 1);
         ++alen;
         i = pi;
         j = pj;
       }
       // reverse into emission order
       for (uint32_t a = 0; a < alen / 2; ++a) {
-        const int16_t tn = g.aln_node[a], tp = g.aln_pos[a];
+        const Pos tn = g.aln_node[a], tp = g.aln_pos[a];
         g.aln_node[a] = g.aln_node[alen - 1 - a];
         g.aln_pos[a] = g.aln_pos[alen - 1 - a];
         g.aln_node[alen - 1 - a] = tn;
@@ -697,9 +756,9 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
           g.pred[v] = -1;
           g.score[v] = -1;
         }
-        auto relax = [&](uint16_t v) {
-          for (uint16_t e = g.in_head[v]; e != kNone; e = g.e_next_in[e]) {
-            const uint16_t t = g.e_tail[e];
+        auto relax = [&](Id v) {
+          for (Id e = g.in_head[v]; e != W::kNone; e = g.e_next_in[e]) {
+            const Id t = g.e_tail[e];
             const long long wgt = g.e_weight[e];
             if (g.score[v] < wgt ||
                 (g.score[v] == wgt && g.score[g.pred[v]] <= g.score[t])) {
@@ -711,25 +770,25 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
         };
         int32_t mx = -1;
         for (uint32_t r = 0; r < rows; ++r) {
-          const uint16_t v = g.r2n[r];
+          const Id v = g.r2n[r];
           relax(v);
           if (mx < 0 || g.score[mx] < g.score[v]) mx = v;
         }
-        while (g.out_head[mx] != kNone) {  // branch completion
+        while (g.out_head[mx] != W::kNone) {  // branch completion
           const uint32_t rank = g.n2r[mx];
-          for (uint16_t e = g.out_head[mx]; e != kNone; e = g.e_next_out[e]) {
-            const uint16_t hd = g.e_head[e];
-            for (uint16_t f = g.in_head[hd]; f != kNone; f = g.e_next_in[f]) {
+          for (Id e = g.out_head[mx]; e != W::kNone; e = g.e_next_out[e]) {
+            const Id hd = g.e_head[e];
+            for (Id f = g.in_head[hd]; f != W::kNone; f = g.e_next_in[f]) {
               if (g.e_tail[f] != mx) g.score[g.e_tail[f]] = -1;
             }
           }
           int32_t nmx = -1;
           for (uint32_t r = rank + 1; r < rows; ++r) {
-            const uint16_t v = g.r2n[r];
+            const Id v = g.r2n[r];
             g.score[v] = -1;
             g.pred[v] = -1;
-            for (uint16_t e = g.in_head[v]; e != kNone; e = g.e_next_in[e]) {
-              const uint16_t t = g.e_tail[e];
+            for (Id e = g.in_head[v]; e != W::kNone; e = g.e_next_in[e]) {
+              const Id t = g.e_tail[e];
               if (g.score[t] == -1) continue;
               const long long wgt = g.e_weight[e];
               if (g.score[v] < wgt ||
@@ -747,13 +806,13 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
         uint32_t plen = 0;
         int32_t v = mx;
         while (g.pred[v] != -1) {
-          g.r2n[plen++] = static_cast<uint16_t>(v);
+          g.r2n[plen++] = static_cast<Id>(v);
           v = g.pred[v];
         }
-        g.r2n[plen++] = static_cast<uint16_t>(v);
+        g.r2n[plen++] = static_cast<Id>(v);
         // coverage of a consensus base = its node + the aligned nodes
         auto coverage = [&](uint32_t idx) -> uint32_t {
-          const uint16_t nd = g.r2n[plen - 1 - idx];
+          const Id nd = g.r2n[plen - 1 - idx];
           uint32_t cvg = g.cov[nd];
           for (uint32_t a = 0; a < g.n_aligned[nd]; ++a) cvg += g.cov[g.aligned[3 * nd + a]];
           return cvg;
@@ -778,7 +837,7 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
         }
         clen = ce - cb;
         for (uint32_t i = 0; i < clen; ++i) {
-          const uint16_t nd = g.r2n[plen - 1 - (cb + i)];
+          const Id nd = g.r2n[plen - 1 - (cb + i)];
           out[i] = "ACGT"[g.code[nd]];
           if (cov_dst) cov_dst[i] = coverage(cb + i);
         }
@@ -799,8 +858,128 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
 
 namespace rvn {
 
+namespace {
+
+// scratch of one launch: up to 16 GB, at most half of what the device has left (the
+// stage-1 buffers of the same context stay resident on an 80 GB card), or option
+// "poa_scratch_budget"
+size_t PoaScratchBudget(Ctx& c) {
+  if (c.poa_scratch_budget) return c.poa_scratch_budget;
+  size_t free_b = 0, total_b = 0;
+  RVN_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  return std::min<size_t>(16ULL << 30, (free_b + c.po_scratch.cap) / 2);
+}
+
+// The windows `todo` on PoaKernel<PoaWide>. A window's node capacity starts at an
+// estimate (the first tier's, plus 1/16 of its layer bases for the columns the layers
+// open) and doubles while the window reports kPoaStatusCapacity, up to its bases (every
+// node holds one base of the window). Edges: 3 per node, and never more than the bases.
+// Each round sorts the windows by scratch and launches runs of them that fit the budget
+// at the largest shape of the run.
+struct PoaWindowDims {
+  const std::vector<uint32_t>& lmax;
+  const std::vector<uint32_t>& bb;
+  const std::vector<uint32_t>& kept;
+  const std::vector<uint64_t>& tot;
+};
+
+void PoaWideRun(Ctx& c, std::vector<uint32_t> todo, const PoaWindowDims& d,
+                uint32_t n_windows, const uint32_t* d_wf, const uint64_t* d_so,
+                const uint8_t* d_bases, const uint8_t* d_quals, const uint32_t* d_sb,
+                const uint32_t* d_se, int m, int n, int gap, bool trim, bool tgs,
+                uint8_t* d_cons, const uint64_t* d_coff, uint32_t* d_clen, uint32_t* d_cov,
+                uint8_t* d_status, uint64_t* d_cells) {
+  std::vector<uint64_t> ncap(n_windows, 0);
+  for (uint32_t w : todo) {
+    ncap[w] = std::min<uint64_t>(d.tot[w], 3ULL * d.bb[w] + d.lmax[w] + 64 + d.tot[w] / 16);
+  }
+  const auto shape_of = [&](uint32_t w) {
+    PoaWideShape s;
+    s.ncap = static_cast<uint32_t>(ncap[w]);
+    s.ecap = static_cast<uint32_t>(std::min<uint64_t>(3 * ncap[w], d.tot[w]));
+    s.lmax = d.lmax[w];
+    s.rows = s.ncap + 1;
+    s.width = (s.lmax + 1 + 31) & ~31u;
+    s.layers = d.kept[w];
+    return s;
+  };
+  const auto widest = [](PoaWideShape a, const PoaWideShape& b) {
+    a.ncap = std::max(a.ncap, b.ncap);
+    a.ecap = std::max(a.ecap, b.ecap);
+    a.lmax = std::max(a.lmax, b.lmax);
+    a.rows = std::max(a.rows, b.rows);
+    a.width = std::max(a.width, b.width);
+    a.layers = std::max(a.layers, b.layers);
+    return a;
+  };
+  const auto stride_of = [](const PoaWideShape& s) {
+    return (MakePoaLayout<PoaWide>(s).bytes + 255) & ~size_t(255);
+  };
+  while (!todo.empty()) {
+    std::vector<size_t> need(n_windows, 0);
+    for (uint32_t w : todo) need[w] = stride_of(shape_of(w));
+    std::stable_sort(todo.begin(), todo.end(),
+                     [&](uint32_t a, uint32_t b) { return need[a] < need[b]; });
+    const size_t budget = PoaScratchBudget(c);
+    if (need[todo.back()] > budget) {
+      throw LimitError("a POA window needs " + std::to_string(need[todo.back()]) +
+                       " bytes of scratch, more than the budget of " +
+                       std::to_string(budget) + " bytes");
+    }
+    // runs [first, first + count) of the sorted windows and their shapes
+    struct Run {
+      size_t first, count;
+      PoaWideShape shape;
+      size_t stride;
+    };
+    std::vector<Run> runs;
+    size_t scratch_bytes = 0;
+    for (size_t i = 0; i < todo.size();) {
+      Run r{i, 1, shape_of(todo[i]), need[todo[i]]};
+      while (i + r.count < todo.size()) {
+        const PoaWideShape s = widest(r.shape, shape_of(todo[i + r.count]));
+        const size_t st = stride_of(s);
+        if (st * (r.count + 1) > budget) break;
+        r.shape = s;
+        r.stride = st;
+        ++r.count;
+      }
+      scratch_bytes = std::max(scratch_bytes, r.stride * r.count);
+      runs.push_back(r);
+      i += r.count;
+    }
+    uint8_t* scratch = c.po_scratch.reserve(scratch_bytes);
+    uint32_t* d_list = c.po_list.reserve(n_windows + 1ULL);
+    RVN_CUDA(cudaMemcpyAsync(d_list, todo.data(), todo.size() * 4, cudaMemcpyHostToDevice, c.stream));
+    for (const Run& r : runs) {
+      PoaKernel<PoaWide><<<static_cast<uint32_t>(r.count), 32, 0, c.stream>>>(
+          static_cast<uint32_t>(r.count), d_list + r.first, d_wf, d_so, d_bases, d_quals,
+          d_sb, d_se, m, n, gap, trim, tgs, r.shape, scratch, r.stride, d_cons, d_coff,
+          d_clen, d_cov, d_status, reinterpret_cast<unsigned long long*>(d_cells));
+      RVN_LAUNCH_CHECK();
+      ++c.launches;
+      ++c.po_route_launches[2];
+    }
+    RVN_CUDA(cudaMemcpyAsync(c.po_h_status.data(), d_status, n_windows, cudaMemcpyDeviceToHost, c.stream));
+    RVN_CUDA(cudaStreamSynchronize(c.stream));  // (also: todo / d_list are reusable)
+    std::vector<uint32_t> again;
+    for (uint32_t w : todo) {
+      if (c.po_h_status[w] != kPoaStatusCapacity) continue;
+      if (ncap[w] >= d.tot[w]) {  // cannot happen: the bound holds every base
+        throw LimitError("a POA graph outgrew the bases of its window");
+      }
+      ncap[w] = std::min<uint64_t>(2 * ncap[w], d.tot[w]);
+      again.push_back(w);
+    }
+    todo.swap(again);
+  }
+}
+
+}  // namespace
+
 // Host driver: windows in batches sized by the scratch budget; windows that
-// outgrow the first-tier capacity are retried with the exact upper bound.
+// outgrow the first-tier capacity are retried with the exact upper bound. With
+// option "poa_wide", the windows past the 16-bit kernels' limits run on the wide one.
 void PoaBatch(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first,
               const uint64_t* h_seq_off, const uint8_t* h_bases, const uint8_t* h_quals,
               const uint32_t* h_seq_begin, const uint32_t* h_seq_end, int m, int n,
@@ -830,8 +1009,9 @@ void PoaBatch(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first,
   c.po_cons_off.assign(n_windows + 1ULL, 0);
   // per window: longest layer, backbone length, all bases - the kernel is chosen
   // PER WINDOW (one long layer must not send a whole batch to the generic kernel)
-  std::vector<uint32_t> w_lmax(n_windows, 1), w_bb(n_windows, 1);
+  std::vector<uint32_t> w_lmax(n_windows, 1), w_bb(n_windows, 1), w_kept(n_windows, 0);
   std::vector<uint64_t> w_tot(n_windows, 1);
+  std::vector<uint8_t> w_wide(n_windows, 0);
   for (uint32_t w = 0; w < n_windows; ++w) {
     const uint32_t s0 = h_win_first[w], s1 = h_win_first[w + 1];
     uint64_t tot = 0, lmax = 0;
@@ -847,10 +1027,16 @@ void PoaBatch(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first,
       }
     }
     // 16-bit node ids, int16 layer positions, 16-bit layer order slots
-    if (tot > 65000) throw LimitError("a POA window holds more than 65000 bases");
-    if (lmax > 32000) throw LimitError("a layer of a POA window holds more than 32000 bases");
-    if (kept > kPoaMaxLayers) throw LimitError("a POA window holds more than 4095 layers");
+    const bool past = tot > 65000 || lmax > 32000 || kept > kPoaMaxLayers;
+    if (c.poa_wide == 2 || (c.poa_wide == 1 && past)) {
+      w_wide[w] = 1;
+    } else {
+      if (tot > 65000) throw LimitError("a POA window holds more than 65000 bases");
+      if (lmax > 32000) throw LimitError("a layer of a POA window holds more than 32000 bases");
+      if (kept > kPoaMaxLayers) throw LimitError("a POA window holds more than 4095 layers");
+    }
     w_lmax[w] = std::max<uint32_t>(w_lmax[w], static_cast<uint32_t>(lmax));
+    w_kept[w] = kept;
     w_tot[w] = std::max<uint64_t>(tot, 1);
     c.po_cons_off[w + 1] = c.po_cons_off[w] + tot;
   }
@@ -866,12 +1052,14 @@ void PoaBatch(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first,
   RVN_CUDA(cudaMemsetAsync(d_status, 0, n_windows + 1ULL, c.stream));
 
   c.po_h_status.assign(n_windows, 0);
+  std::vector<uint8_t> route(n_windows, 0);  // 0 fast, 1 generic, 2 wide
+  for (int k = 0; k < 3; ++k) c.po_route_windows[k] = c.po_route_launches[k] = 0;
   TimerBegin(c, "poa");
   // group 0: every layer fits the register-row kernel; group 1: the generic kernel
   for (int group = 0; group < 2; ++group) {
     std::vector<uint32_t> todo;
     for (uint32_t w = 0; w < n_windows; ++w) {
-      if ((w_lmax[w] + 1 <= kFastCols) == (group == 0)) todo.push_back(w);
+      if (!w_wide[w] && (w_lmax[w] + 1 <= kFastCols) == (group == 0)) todo.push_back(w);
     }
     for (int tier = 0; tier < 2 && !todo.empty(); ++tier) {
       uint32_t lmax = 1, bb_max = 1;
@@ -891,18 +1079,15 @@ void PoaBatch(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first,
       shape.width = (lmax + 1 + 31) & ~31u;
       const size_t fast_smem = ((shape.ncap + 15) & ~15u) + 4ULL * shape.ncap + 16;
       const bool fast = group == 0 && fast_smem <= 220 * 1024;  // the register-row kernel
-      const size_t stride = ((fast ? MakeFastLayout(shape).bytes : MakePoaLayout(shape).bytes) +
+      const size_t stride = ((fast ? MakeFastLayout(shape).bytes
+                                   : MakePoaLayout<PoaNarrow>(shape).bytes) +
                              255) & ~size_t(255);
       if (fast) {
         RVN_CUDA(cudaFuncSetAttribute(PoaKernelFast,
                                       cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       static_cast<int>(fast_smem)));
       }
-      // scratch budget per batch: up to 16 GB, at most half of what the device has
-      // left (the stage-1 buffers of the same context stay resident on an 80 GB card)
-      size_t free_b = 0, total_b = 0;
-      RVN_CUDA(cudaMemGetInfo(&free_b, &total_b));
-      const size_t budget = std::min<size_t>(16ULL << 30, (free_b + c.po_scratch.cap) / 2);
+      const size_t budget = PoaScratchBudget(c);
       const uint32_t batch = static_cast<uint32_t>(
           std::max<size_t>(1, std::min<size_t>(todo.size(), budget / stride)));
       uint8_t* scratch = c.po_scratch.reserve(stride * batch);
@@ -916,14 +1101,16 @@ void PoaBatch(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first,
               tgs, shape, scratch, stride, d_cons, d_coff, d_clen, d_cov, d_status,
               reinterpret_cast<unsigned long long*>(d_cells));
         } else {
-          PoaKernel<<<nb, 32, 0, c.stream>>>(
+          PoaKernel<PoaNarrow><<<nb, 32, 0, c.stream>>>(
               nb, d_list + b0, d_wf, d_so, d_bases, d_quals, d_sb, d_se, m, n, gap, trim,
               tgs, shape, scratch, stride, d_cons, d_coff, d_clen, d_cov, d_status,
               reinterpret_cast<unsigned long long*>(d_cells));
         }
         RVN_LAUNCH_CHECK();
         ++c.launches;
+        ++c.po_route_launches[fast ? 0 : 1];
       }
+      for (uint32_t w : todo) route[w] = fast ? 0 : 1;
       RVN_CUDA(cudaMemcpyAsync(c.po_h_status.data(), d_status, n_windows, cudaMemcpyDeviceToHost, c.stream));
       RVN_CUDA(cudaStreamSynchronize(c.stream));  // (also: todo / d_list are reusable)
       std::vector<uint32_t> again;
@@ -934,6 +1121,23 @@ void PoaBatch(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first,
     }
   }
   TimerEnd(c);
+  // the wide kernel: windows past the 16-bit limits, and those still out of capacity
+  // after the second tier (a graph beyond 65000 nodes or edges, or the int16 guard)
+  std::vector<uint32_t> deep;
+  for (uint32_t w = 0; w < n_windows; ++w) {
+    if (w_wide[w] || (c.poa_wide && c.po_h_status[w] == kPoaStatusCapacity)) {
+      deep.push_back(w);
+      route[w] = 2;
+    }
+  }
+  if (!deep.empty()) {
+    TimerBegin(c, "poa_wide");
+    PoaWideRun(c, deep, PoaWindowDims{w_lmax, w_bb, w_kept, w_tot}, n_windows, d_wf, d_so,
+               d_bases, d_quals, d_sb, d_se, m, n, gap, trim, tgs, d_cons, d_coff, d_clen,
+               d_cov, d_status, d_cells);
+    TimerEnd(c);
+  }
+  for (uint32_t w = 0; w < n_windows; ++w) ++c.po_route_windows[route[w]];
   for (uint32_t w = 0; w < n_windows; ++w) {
     if (c.po_h_status[w] == kPoaStatusCapacity) {
       throw LimitError("a POA graph outgrew 65000 nodes/edges or the int16 score range");

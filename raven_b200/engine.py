@@ -183,6 +183,14 @@ class Engine:
                     coverage=_arr(cov, total if want_coverage else 0, np.uint32),
                     cells=cells.value)
 
+    def poa_routes(self):
+        """Kernels of the last poa_batch: windows that finished on the register-row
+        ("fast"), generic and wide kernels, and each kernel's launches."""
+        win, lau = (C.c_uint32 * 3)(), (C.c_uint32 * 3)()
+        self._check(self.lib.rvn_poa_routes(self.h, win, lau))
+        names = ("fast", "generic", "wide")
+        return dict(zip(names, list(win)), launches=dict(zip(names, list(lau))))
+
     def kmer_complexity(self, read_index, positions, kmer_len):
         """Pile::AddKmers' low-complexity test (pile.cc:64-120): 1 = bin gets marked."""
         ri = np.ascontiguousarray(read_index, dtype=np.uint32)

@@ -27,6 +27,19 @@ void Check(rvn_ctx* ctx, int rc) {
   throw std::runtime_error(msg);
 }
 
+// whether RVN_SET_OPTIONS ("name=value,...") sets option `name`
+bool EnvNamesOption(const std::string& name) {
+  const char* env = std::getenv("RVN_SET_OPTIONS");
+  if (!env) return false;
+  const std::string all(env);
+  for (size_t b = 0; b < all.size();) {
+    const size_t e = std::min(all.find(',', b), all.size());
+    if (all.compare(b, std::min(all.find('=', b), e) - b, name) == 0) return true;
+    b = e + 1;
+  }
+  return false;
+}
+
 struct Hit {  // the overlap kept for one read
   bool valid = false;
   rvn_overlap o{};
@@ -50,6 +63,9 @@ Polisher::Polisher(std::shared_ptr<thread_pool::ThreadPool> thread_pool, double 
     throw std::runtime_error(
         "[racon::Polisher::Create] error: no usable CUDA device (no CPU fallback)");
   }
+  // windows of any depth, like racon: the ones past the 16-bit consensus kernels run
+  // on the wide kernel. RVN_SET_OPTIONS=poa_wide=... (applied by rvn_ctx_create) wins.
+  if (!EnvNamesOption("poa_wide")) Check(ctx_, rvn_set_option(ctx_, "poa_wide", 1));
 }
 
 Polisher::~Polisher() {
@@ -75,7 +91,7 @@ std::vector<std::unique_ptr<biosoup::NucleicAcid>> Polisher::Polish(
     const std::vector<std::unique_ptr<biosoup::NucleicAcid>>& targets,
     const std::vector<std::unique_ptr<biosoup::NucleicAcid>>& sequences,
     bool drop_unpolished) {
-  num_windows_ = num_polished_windows_ = 0;
+  num_windows_ = num_polished_windows_ = num_wide_windows_ = 0;
   poa_seconds_ = 0;
   if (targets.empty() || sequences.empty()) {
     return {};
@@ -330,6 +346,9 @@ std::vector<std::unique_ptr<biosoup::NucleicAcid>> Polisher::Polish(
   const std::uint64_t* cons_off = nullptr;
   const std::uint8_t* status = nullptr;
   Check(ctx_, rvn_poa_results(ctx_, &cons, &cons_off, &status, nullptr, nullptr));
+  std::uint32_t routes[3] = {0, 0, 0};
+  Check(ctx_, rvn_poa_routes(ctx_, routes, nullptr));
+  num_wide_windows_ = routes[2];
   poa_seconds_ = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
   phase_seconds_[3] = Seconds(t_phase);
 

@@ -42,6 +42,7 @@ def _load():
 
 def polish(targets, sequences, q=0.0, e=0.3, w=500, trim=True, m=3, n=-5, g=-4, threads=4):
     """Polished targets (ReadSet with names) and stats: windows, polished windows,
+    windows on the wide consensus kernel (deeper than the 16-bit kernels take),
     seconds in the consensus phase (H2D + POA kernels + D2H), total seconds."""
     lib = _load()
     u64p, u32p, u8p = (C.POINTER(C.c_uint64), C.POINTER(C.c_uint32), C.POINTER(C.c_uint8))
@@ -82,7 +83,8 @@ def polish(targets, sequences, q=0.0, e=0.3, w=500, trim=True, m=3, n=-5, g=-4, 
                            woff, view(lib.rvnh_polish_lens(h), cnt, np.uint32))
         rs.names = lib.rvnh_polish_names(h).decode().split("\n")[:-1]
         st = lib.rvnh_polish_stats(h)
-        stats = dict(windows=int(st[0]), polished_windows=int(st[1]), poa_seconds=st[2],
+        stats = dict(windows=int(st[0]), polished_windows=int(st[1]),
+                     wide_windows=int(st[10]), poa_seconds=st[2],
                      seconds=st[3],
                      phases_s=dict(map=st[4], align=st[5], pack=st[6], consensus=st[7],
                                    stitch=st[8], pieces=st[9]))
