@@ -8,8 +8,8 @@
 //   polisher->Polish(targets, sequences, drop_unpolished)   polish.cc:51
 // This class keeps those signatures. Mapping (ram) and the window consensus
 // (POA) run on the GPU through the C ABI (rvn_minimize / rvn_map /
-// rvn_poa_batch); the read-to-unitig alignment path and the window cutting run
-// on the host pool (next row of SURVEY.md §8f). The cuda_* arguments of the
+// rvn_align_breaking_points / rvn_polish_windows): the alignment paths, the window
+// cuts, racon's layer rules and the window layers are built on the device. The cuda_* arguments of the
 // reference select NVIDIA's cudapoa/cudaaligner inside upstream racon; here the
 // GPU path is always on and they are accepted and ignored.
 #ifndef RACON_POLISHER_HPP_
@@ -49,9 +49,12 @@ class Polisher {
   // windows that ran on the wide (32-bit) consensus kernel: deeper than the 16-bit
   // kernels take (option "poa_wide" of include/raven_b200.h)
   std::uint64_t num_wide_windows() const { return num_wide_windows_; }
+  // batches of windows the consensus ran in (option "poa_batch_bytes")
+  std::uint64_t num_window_batches() const { return num_window_batches_; }
+  // the layer rules, the packing and the consensus (rvn_polish_windows)
   double poa_seconds() const { return poa_seconds_; }
-  // map (GPU), alignment paths + window cuts (GPU), window packing, consensus (GPU),
-  // stitch, layer rules (host pool)
+  // map (GPU), alignment paths + window cuts (GPU), window packing (GPU), consensus
+  // (GPU), stitch, layer rules (GPU)
   const double* phase_seconds() const { return phase_seconds_; }
 
  private:
@@ -65,6 +68,7 @@ class Polisher {
   std::int8_t m_, n_, g_;
   rvn_ctx* ctx_;
   std::uint64_t num_windows_ = 0, num_polished_windows_ = 0, num_wide_windows_ = 0;
+  std::uint64_t num_window_batches_ = 0;
   double poa_seconds_ = 0;
   double phase_seconds_[6] = {0, 0, 0, 0, 0, 0};
 };

@@ -26,6 +26,8 @@
  *                          edlibAlign(read, unitig, NW, EDLIB_TASK_PATH) + the window
  *                          breaking points of racon::Polisher::Polish
  *                                                      RavenLib/src/polish.cc:43-51
+ *   rvn_polish_windows     the window layers and consensus of racon::Polisher::Polish
+ *                                                      RavenLib/src/polish.cc:43-51
  *   rvn_find_overlaps_and_create_piles
  *                          raven::FindOverlapsAndCreatePiles
  *                                                      RavenLib/src/construct.cc:14-121
@@ -307,6 +309,54 @@ int rvn_poa_results(rvn_ctx* ctx, const char** consensus, const uint64_t** cons_
  * (else 3 entries). RVN_ERR_STATE when there are no POA results. */
 int rvn_poa_routes(rvn_ctx* ctx, uint32_t* windows, uint32_t* launches);
 
+/* The window layers and consensus of racon::Polisher::Polish (RavenLib/src/polish.cc:43-51)
+ * after the alignments of rvn_align_breaking_points, with the layers built on the device
+ * from the uploaded reads: no base of a layer passes through the host.
+ * Targets are uploaded reads [0, n_targets); target t owns windows first_window[t] ..
+ * first_window[t+1] - 1, ceil(len_t / window) of them, numbered over the targets in order.
+ * The backbone of window j of target t is its bases [j*window, min((j+1)*window, len_t)).
+ * Alignment a: query = uploaded read q_read[a] (length L), aligned on strand[a] (0 = the
+ * read reverse complemented as a whole) to target t_read[a] (< n_targets); its window
+ * slots bp_off[a] .. bp_off[a+1] - 1 (bp_off[0] = 0) hold 4 breaking points each, as
+ * rvn_align_breaking_points writes them. Per slot x, in order of alignment and slot:
+ *   - skipped if bp[4x] == 0xFFFFFFFF;
+ *   - qb = q_begin[a], or L - (q_begin[a] + q_len[a]) when strand[a] == 0;
+ *     fq = qb + bp[4x+1], lq = qb + bp[4x+3], ft = bp[4x], lt = bp[4x+2];
+ *   - dropped unless (double)(lq - fq) >= 0.02 * window;
+ *   - if the read has block qualities: dropped if avg < q, avg = the sum of Score(x) over
+ *     x in [fq, lq) divided by lq - fq, where Score(x) = block_quality[(f ? L-1-x : x) >> 6]
+ *     and f = reverse_complement[read] XOR (strand[a] == 0) (biosoup's Score of the view
+ *     the reference aligns);
+ *   - ws = (ft / window) * window; dropped if ft - ws >= lt - ws - 1 (unsigned);
+ *   - else a layer of window first_window[t] + ft / window with begin = ft - ws and
+ *     end = lt - ws - 1: bases [fq, lq) of the read in its aligned orientation, qualities
+ *     Score + '!' (a read without qualities: '!' + 1, and no qualities at all when no read
+ *     has any); the backbone's quality is '!'.
+ * A window's layers keep that order. Qualities: block_quality[bq_off[r] .. bq_off[r+1])
+ * for uploaded read r (bq_off has one entry per uploaded read + 1; an empty range = no
+ * qualities, else at least one per 64 bases), or block_quality NULL. reverse_complement:
+ * biosoup's is_reverse_complement per uploaded read, or NULL (all 0); it only turns the
+ * quality index around - the uploaded bases are the read as it reads.
+ * The consensus is rvn_poa_batch's (m, n, g, trim, tgs and its options) over that flat
+ * layout, run on consecutive windows in batches whose device inputs fit a budget: per
+ * window 2 bytes per base (backbone and layers; 3 when some read has qualities), 20 per
+ * sequence and 64; the budget is a quarter of the free device memory (with the batch
+ * buffers the context holds), or option "poa_batch_bytes" when that is not 0; a batch holds
+ * at least one window. *window_batches (may be NULL) = the batches. Results as for
+ * rvn_poa_batch, for every window of the call: rvn_poa_results (no coverage),
+ * rvn_poa_routes (summed over the batches). Phases "poa_layers" (rules and sort) and
+ * "poa_pack" (one per batch) in rvn_get_timings are the device layer build.
+ * RVN_ERR_INVALID for bad indices or coordinates, breaking points outside their read or
+ * their target's windows, too few block qualities, or g >= 0; RVN_ERR_LIMIT as
+ * rvn_poa_batch; RVN_ERR_STATE when the reads were not uploaded. */
+int rvn_polish_windows(rvn_ctx* ctx, uint64_t n_alignments, const uint32_t* q_read,
+                       const uint32_t* q_begin, const uint32_t* q_len, const uint8_t* strand,
+                       const uint32_t* t_read, const uint64_t* bp_off,
+                       const uint32_t* breaking_points, uint32_t n_targets, uint32_t window,
+                       const uint8_t* block_quality, const uint64_t* bq_off,
+                       const uint8_t* reverse_complement, double q, int8_t m, int8_t n, int8_t g,
+                       int trim, int tgs, uint32_t* window_batches);
+
 /* ---- introspection (parity tests, profiling) ---- */
 
 /* Per-read sketches of reads [first,last) exactly as the reference engine's
@@ -375,7 +425,9 @@ int rvn_get_stats(rvn_ctx* ctx, rvn_stats* out);
  * upload); "index_chunk_budget" (bytes: replaces the free device memory in that auto
  * decision, 0 = the free memory); "map_flush_bases" (rvn_map cuts its range into flushes of
  * >= N query bases; 0 = the default, from the device memory; for tests of the flush
- * path, results do not depend on it); "poa_wide" and "poa_scratch_budget" (rvn_poa_batch);
+ * path, results do not depend on it); "poa_wide" and "poa_scratch_budget" (rvn_poa_batch and
+ * rvn_polish_windows); "poa_batch_bytes" (rvn_polish_windows: the device inputs of one window
+ * batch, 0 = the default, from the free device memory; results do not depend on it);
  * "reset_stats".
  * Unknown name or value out of range -> RVN_ERR_INVALID. */
 int rvn_set_option(rvn_ctx* ctx, const char* name, int64_t value);

@@ -57,6 +57,11 @@ SIGNATURES = {
     "rvn_poa_results": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(U64P),
                                   C.POINTER(C.POINTER(C.c_uint8)), C.POINTER(U32P), U64P]),
     "rvn_poa_routes": (C.c_int, [C.c_void_p, U32P, U32P]),
+    "rvn_polish_windows": (C.c_int, [C.c_void_p, C.c_uint64, U32P, U32P, U32P,
+                                     C.POINTER(C.c_uint8), U32P, U64P, U32P, C.c_uint32,
+                                     C.c_uint32, C.POINTER(C.c_uint8), U64P,
+                                     C.POINTER(C.c_uint8), C.c_double, C.c_int8, C.c_int8,
+                                     C.c_int8, C.c_int, C.c_int, U32P]),
     "rvn_kmer_complexity": (C.c_int, [C.c_void_p, U32P, U32P, C.c_uint64, C.c_uint32,
                                       C.POINTER(C.c_uint8)]),
     "rvn_find_overlaps_and_create_piles": (

@@ -727,6 +727,9 @@ void SetOption(Ctx& c, const char* name, int64_t value) {
   } else if (name && std::strcmp(name, "poa_scratch_budget") == 0) {
     if (value < 0) throw InvalidArgument("poa_scratch_budget: bytes, 0 = from the device memory");
     c.poa_scratch_budget = static_cast<uint64_t>(value);
+  } else if (name && std::strcmp(name, "poa_batch_bytes") == 0) {
+    if (value < 0) throw InvalidArgument("poa_batch_bytes: bytes, 0 = from the device memory");
+    c.poa_batch_bytes = static_cast<uint64_t>(value);
   } else if (name && std::strcmp(name, "reset_stats") == 0) {
     std::memset(&c.stats, 0, sizeof(c.stats));
     c.launches = 0;
@@ -1150,6 +1153,30 @@ RVN_API int rvn_poa_routes(rvn_ctx* ctx, uint32_t* windows, uint32_t* launches) 
       if (windows) windows[k] = c.po_route_windows[k];
       if (launches) launches[k] = c.po_route_launches[k];
     }
+  });
+}
+
+RVN_API int rvn_polish_windows(rvn_ctx* ctx, uint64_t n_alignments, const uint32_t* q_read,
+                               const uint32_t* q_begin, const uint32_t* q_len,
+                               const uint8_t* strand, const uint32_t* t_read,
+                               const uint64_t* bp_off, const uint32_t* breaking_points,
+                               uint32_t n_targets, uint32_t window,
+                               const uint8_t* block_quality, const uint64_t* bq_off,
+                               const uint8_t* reverse_complement, double q, int8_t m, int8_t n,
+                               int8_t g, int trim, int tgs, uint32_t* window_batches) {
+  return Guard(ctx, [&](Ctx& c) {
+    if (!bp_off || (block_quality && !bq_off)) throw InvalidArgument("null argument");
+    if (n_alignments && (!q_read || !q_begin || !q_len || !strand || !t_read ||
+                         (bp_off[n_alignments] && !breaking_points))) {
+      throw InvalidArgument("null argument");
+    }
+    TimerReset(c);
+    PolishArgs a{n_alignments, q_read, q_begin, q_len, strand, t_read, bp_off, breaking_points,
+                 n_targets, window, block_quality, bq_off, reverse_complement, q, m, n, g,
+                 trim != 0, tgs != 0};
+    PolishWindows(c, a);
+    if (window_batches) *window_batches = c.po_batches;
+    TimerCollect(c);
   });
 }
 

@@ -257,6 +257,15 @@ struct Ctx {
   uint64_t poa_scratch_budget = 0;
   // windows and launches of the last rvn_poa_batch per kernel: fast, generic, wide
   uint32_t po_route_windows[3] = {0, 0, 0}, po_route_launches[3] = {0, 0, 0};
+  // rvn_polish_windows (layers.cu): per alignment and per breaking-point slot, the
+  // window key and slot order of the stable sort, per window its kept layers and their
+  // bases, per window of a batch its source; option "poa_batch_bytes" (0 = from the
+  // free device memory) bounds the flat inputs of one window batch
+  DevBuf<uint8_t> pl_aln, pl_bq, pl_win;
+  DevBuf<uint32_t> pl_bp, pl_key[2], pl_cnt, pl_seq_len;
+  DevBuf<uint64_t> pl_ord[2], pl_bases, pl_err;
+  uint64_t poa_batch_bytes = 0;
+  uint32_t po_batches = 0;  // window batches of the last rvn_polish_windows
 
   // ---- stage-1 results ----
   PinBuf<rvn_overlap> st_ovl;  // pinned: the D2H of the results runs at link speed
@@ -486,10 +495,43 @@ void PileAddLayersDevice(Ctx& c, uint16_t* d_data, const uint64_t* d_off, uint64
                          uint32_t first = 0);
 
 // ---- poa.cu ---- racon window consensus over a flat batch of windows
+// the flat layout of a batch of windows in device memory (rvn_poa_batch's arguments)
+struct PoaInput {
+  const uint32_t* win_first = nullptr;
+  const uint64_t* seq_off = nullptr;
+  const uint8_t* bases = nullptr;
+  const uint8_t* quals = nullptr;  // null: no qualities
+  const uint32_t* seq_begin = nullptr;
+  const uint32_t* seq_end = nullptr;
+};
+// the consensus of windows already on the device; h_*: host copies of the tables
+void PoaRun(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first, const uint64_t* h_seq_off,
+            const uint32_t* h_seq_begin, const uint32_t* h_seq_end, const PoaInput& d, int m,
+            int n, int gap, bool trim, bool tgs, bool want_coverage);
 void PoaBatch(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first,
               const uint64_t* h_seq_off, const uint8_t* h_bases, const uint8_t* h_quals,
               const uint32_t* h_seq_begin, const uint32_t* h_seq_end, int m, int n,
               int gap, bool trim, bool tgs, bool want_coverage);
+
+// ---- layers.cu ---- racon's layers of every window built on the device from the
+// uploaded reads and the breaking points, then PoaRun over batches of windows
+// (include/raven_b200.h, rvn_polish_windows)
+struct PolishArgs {
+  uint64_t n_aln;
+  const uint32_t *q_read, *q_begin, *q_len;
+  const uint8_t* strand;
+  const uint32_t* t_read;
+  const uint64_t* bp_off;
+  const uint32_t* bp;
+  uint32_t n_targets, window;
+  const uint8_t* bq;
+  const uint64_t* bq_off;
+  const uint8_t* rc;
+  double q;
+  int m, n, gap;
+  bool trim, tgs;
+};
+void PolishWindows(Ctx& c, const PolishArgs& a);
 
 // Pile::AddKmers low-complexity test for (read index, position) pairs
 void KmerComplexity(Ctx& c, const uint32_t* h_read_idx, const uint32_t* h_pos,

@@ -977,33 +977,24 @@ void PoaWideRun(Ctx& c, std::vector<uint32_t> todo, const PoaWindowDims& d,
 
 }  // namespace
 
-// Host driver: windows in batches sized by the scratch budget; windows that
-// outgrow the first-tier capacity are retried with the exact upper bound. With
-// option "poa_wide", the windows past the 16-bit kernels' limits run on the wide one.
-void PoaBatch(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first,
-              const uint64_t* h_seq_off, const uint8_t* h_bases, const uint8_t* h_quals,
-              const uint32_t* h_seq_begin, const uint32_t* h_seq_end, int m, int n,
-              int gap, bool trim, bool tgs, bool want_coverage) {
+// Host driver of windows whose flat layout is on the device (`d`); h_* are the host
+// copies of its window and sequence tables. Windows in batches sized by the scratch
+// budget; windows that outgrow the first-tier capacity are retried with the exact
+// upper bound. With option "poa_wide", the windows past the 16-bit kernels' limits run
+// on the wide one. Results (compacted) land in c.po_out_*, c.po_h_status, c.po_route_*.
+void PoaRun(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first, const uint64_t* h_seq_off,
+            const uint32_t* h_seq_begin, const uint32_t* h_seq_end, const PoaInput& d, int m,
+            int n, int gap, bool trim, bool tgs, bool want_coverage) {
   c.poa_valid = false;
   if (gap >= 0) {
     throw InvalidArgument("[racon::Polisher::Create] error: gap penalty must be negative");
   }
-  const uint32_t n_seqs = n_windows ? h_win_first[n_windows] : 0;
-  const uint64_t n_bases = n_seqs ? h_seq_off[n_seqs] : 0;
-  TimerBegin(c, "poa_h2d");
-  uint32_t* d_wf = c.po_win_first.reserve(n_windows + 2ULL);
-  uint64_t* d_so = c.po_seq_off.reserve(n_seqs + 2ULL);
-  uint8_t* d_bases = c.po_bases.reserve(n_bases + 16);
-  uint8_t* d_quals = h_quals ? c.po_quals.reserve(n_bases + 16) : nullptr;
-  uint32_t* d_sb = c.po_seq_begin.reserve(n_seqs + 2ULL);
-  uint32_t* d_se = c.po_seq_end.reserve(n_seqs + 2ULL);
-  RVN_CUDA(cudaMemcpyAsync(d_wf, h_win_first, (n_windows + 1ULL) * 4, cudaMemcpyHostToDevice, c.stream));
-  RVN_CUDA(cudaMemcpyAsync(d_so, h_seq_off, (n_seqs + 1ULL) * 8, cudaMemcpyHostToDevice, c.stream));
-  RVN_CUDA(cudaMemcpyAsync(d_bases, h_bases, n_bases, cudaMemcpyHostToDevice, c.stream));
-  if (h_quals) RVN_CUDA(cudaMemcpyAsync(d_quals, h_quals, n_bases, cudaMemcpyHostToDevice, c.stream));
-  RVN_CUDA(cudaMemcpyAsync(d_sb, h_seq_begin, n_seqs * 4ULL, cudaMemcpyHostToDevice, c.stream));
-  RVN_CUDA(cudaMemcpyAsync(d_se, h_seq_end, n_seqs * 4ULL, cudaMemcpyHostToDevice, c.stream));
-  TimerEnd(c);
+  const uint32_t* d_wf = d.win_first;
+  const uint64_t* d_so = d.seq_off;
+  const uint8_t* d_bases = d.bases;
+  const uint8_t* d_quals = d.quals;
+  const uint32_t* d_sb = d.seq_begin;
+  const uint32_t* d_se = d.seq_end;
 
   // output slots: a consensus never has more bases than the window holds
   c.po_cons_off.assign(n_windows + 1ULL, 0);
@@ -1178,6 +1169,42 @@ void PoaBatch(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first,
   c.po_n_windows = n_windows;
   c.po_has_cov = want_coverage;
   c.poa_valid = true;
+}
+
+// rvn_poa_batch: the host's flat layout to the device, then PoaRun.
+void PoaBatch(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first,
+              const uint64_t* h_seq_off, const uint8_t* h_bases, const uint8_t* h_quals,
+              const uint32_t* h_seq_begin, const uint32_t* h_seq_end, int m, int n,
+              int gap, bool trim, bool tgs, bool want_coverage) {
+  c.poa_valid = false;
+  if (gap >= 0) {
+    throw InvalidArgument("[racon::Polisher::Create] error: gap penalty must be negative");
+  }
+  const uint32_t n_seqs = n_windows ? h_win_first[n_windows] : 0;
+  const uint64_t n_bases = n_seqs ? h_seq_off[n_seqs] : 0;
+  TimerBegin(c, "poa_h2d");
+  PoaInput d;
+  uint32_t* d_wf = c.po_win_first.reserve(n_windows + 2ULL);
+  uint64_t* d_so = c.po_seq_off.reserve(n_seqs + 2ULL);
+  uint8_t* d_bases = c.po_bases.reserve(n_bases + 16);
+  uint8_t* d_quals = h_quals ? c.po_quals.reserve(n_bases + 16) : nullptr;
+  uint32_t* d_sb = c.po_seq_begin.reserve(n_seqs + 2ULL);
+  uint32_t* d_se = c.po_seq_end.reserve(n_seqs + 2ULL);
+  RVN_CUDA(cudaMemcpyAsync(d_wf, h_win_first, (n_windows + 1ULL) * 4, cudaMemcpyHostToDevice, c.stream));
+  RVN_CUDA(cudaMemcpyAsync(d_so, h_seq_off, (n_seqs + 1ULL) * 8, cudaMemcpyHostToDevice, c.stream));
+  RVN_CUDA(cudaMemcpyAsync(d_bases, h_bases, n_bases, cudaMemcpyHostToDevice, c.stream));
+  if (h_quals) RVN_CUDA(cudaMemcpyAsync(d_quals, h_quals, n_bases, cudaMemcpyHostToDevice, c.stream));
+  RVN_CUDA(cudaMemcpyAsync(d_sb, h_seq_begin, n_seqs * 4ULL, cudaMemcpyHostToDevice, c.stream));
+  RVN_CUDA(cudaMemcpyAsync(d_se, h_seq_end, n_seqs * 4ULL, cudaMemcpyHostToDevice, c.stream));
+  TimerEnd(c);
+  d.win_first = d_wf;
+  d.seq_off = d_so;
+  d.bases = d_bases;
+  d.quals = d_quals;
+  d.seq_begin = d_sb;
+  d.seq_end = d_se;
+  PoaRun(c, n_windows, h_win_first, h_seq_off, h_seq_begin, h_seq_end, d, m, n, gap, trim, tgs,
+         want_coverage);
 }
 
 }  // namespace rvn

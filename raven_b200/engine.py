@@ -273,6 +273,39 @@ class Engine:
             bp.ctypes.data_as(U32P)))
         return dist, off, bp
 
+    def polish_windows(self, q_read, q_begin, q_len, strand, t_read, bp_off, bp, n_targets,
+                       window=500, block_quality=None, bq_off=None, reverse_complement=None,
+                       q=0.0, m=3, n=-5, g=-4, trim=True, tgs=True):
+        """racon's layers of every window of targets [0, n_targets) built on the device from
+        the uploaded reads and the breaking points (align_breaking_points), and their
+        consensus in window batches (rvn_polish_windows): consensus, offsets and status per
+        window, and the window batches."""
+        a = [np.ascontiguousarray(x, dtype=np.uint32) for x in (q_read, q_begin, q_len, t_read)]
+        st = np.ascontiguousarray(strand, dtype=np.uint8)
+        off = np.ascontiguousarray(bp_off, dtype=np.uint64)
+        b = np.ascontiguousarray(bp, dtype=np.uint32)
+        u8p = C.POINTER(C.c_uint8)
+        bq = None if block_quality is None else np.ascontiguousarray(block_quality, np.uint8)
+        bqo = None if bq_off is None else np.ascontiguousarray(bq_off, np.uint64)
+        rc = (None if reverse_complement is None
+              else np.ascontiguousarray(reverse_complement, np.uint8))
+        batches = C.c_uint32(0)
+        self._check(self.lib.rvn_polish_windows(
+            self.h, a[0].size, a[0].ctypes.data_as(U32P), a[1].ctypes.data_as(U32P),
+            a[2].ctypes.data_as(U32P), st.ctypes.data_as(u8p), a[3].ctypes.data_as(U32P),
+            off.ctypes.data_as(U64P), b.ctypes.data_as(U32P), n_targets, window,
+            None if bq is None else bq.ctypes.data_as(u8p),
+            None if bqo is None else bqo.ctypes.data_as(U64P),
+            None if rc is None else rc.ctypes.data_as(u8p), float(q), m, n, g, int(trim),
+            int(tgs), C.byref(batches)))
+        cons, coff, sts = C.c_void_p(), U64P(), C.POINTER(C.c_uint8)()
+        self._check(self.lib.rvn_poa_results(self.h, C.byref(cons), C.byref(coff),
+                                             C.byref(sts), None, None))
+        nw = int(sum((int(x) + window - 1) // window for x in self._keep[2][:n_targets]))
+        cons_off = _arr(coff, nw + 1, np.uint64)
+        return dict(consensus=_arr(cons, int(cons_off[-1]) if nw else 0, np.uint8),
+                    cons_off=cons_off, status=_arr(sts, nw, np.uint8), batches=batches.value)
+
     def debug_sort_pairs(self, keys, vals=None, begin_bit=0, end_bit=None, descending=False):
         """The engine's stable radix sort (csrc/radix.cu) on host arrays; returns copies."""
         k = np.ascontiguousarray(keys).copy()

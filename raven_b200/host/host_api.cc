@@ -42,8 +42,8 @@ struct PolishResult {
   std::string names, error;
   // windows, polished windows, POA seconds, total seconds, then the phases of
   // Polish: map, alignment paths, window packing, consensus, stitch, layer rules;
-  // then the windows that ran on the wide consensus kernel
-  double stats[11] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  // then the windows that ran on the wide consensus kernel, the window batches
+  double stats[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 };
 
 }  // namespace
@@ -84,6 +84,7 @@ RVNH_API void* rvnh_polish(const std::uint64_t* t_words, const std::uint64_t* t_
         std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     for (int i = 0; i < 6; ++i) res->stats[4 + i] = polisher->phase_seconds()[i];
     res->stats[10] = static_cast<double>(polisher->num_wide_windows());
+    res->stats[11] = static_cast<double>(polisher->num_window_batches());
   } catch (const std::exception& ex) {
     res->error = ex.what();
     if (res->error.empty()) res->error = "error";

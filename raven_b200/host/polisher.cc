@@ -2,15 +2,14 @@
 // Reference contract: RavenLib/src/polish.cc:43-51; behaviour of the stages:
 // SURVEY.md App. A.4. GPU: mapping (rvn_minimize/rvn_filter/rvn_map), the global
 // alignment paths of the reads (edlibAlign NW PATH) cut at the windows
-// (rvn_align_breaking_points) and the per-window consensus (rvn_poa_batch). Host
-// pool: best overlap per read, racon's per-layer rules, window assembly, stitching.
+// (rvn_align_breaking_points), racon's per-layer rules, the window layers and their
+// consensus (rvn_polish_windows). Host: best overlap per read, stitching.
 #include "racon/polisher.hpp"
 
 #include <algorithm>
 #include <chrono>
 #include <cstdlib>
 #include <cstring>
-#include <future>
 #include <stdexcept>
 #include <string>
 
@@ -43,12 +42,6 @@ bool EnvNamesOption(const std::string& name) {
 struct Hit {  // the overlap kept for one read
   bool valid = false;
   rvn_overlap o{};
-};
-
-struct Piece {  // one layer: read segment [qb, qe) laid over a window
-  std::uint64_t window;
-  std::uint32_t read, qb, qe, begin, end;
-  bool strand;
 };
 
 }  // namespace
@@ -91,7 +84,7 @@ std::vector<std::unique_ptr<biosoup::NucleicAcid>> Polisher::Polish(
     const std::vector<std::unique_ptr<biosoup::NucleicAcid>>& targets,
     const std::vector<std::unique_ptr<biosoup::NucleicAcid>>& sequences,
     bool drop_unpolished) {
-  num_windows_ = num_polished_windows_ = num_wide_windows_ = 0;
+  num_windows_ = num_polished_windows_ = num_wide_windows_ = num_window_batches_ = 0;
   poa_seconds_ = 0;
   if (targets.empty() || sequences.empty()) {
     return {};
@@ -160,14 +153,13 @@ std::vector<std::unique_ptr<biosoup::NucleicAcid>> Polisher::Polish(
 
   phase_seconds_[0] = Seconds(t_phase);
 
-  // ---- 2. GPU: alignment paths cut at the windows (rvn_align_breaking_points),
-  //         host pool: the per-window rules of racon -> layer pieces ----
+  // ---- 2. GPU: alignment paths cut at the windows (rvn_align_breaking_points) ----
   std::vector<std::uint64_t> first_window(T + 1ULL, 0);
   for (std::uint32_t i = 0; i < T; ++i) {
     first_window[i + 1] = first_window[i] + (targets[i]->inflated_len + w_ - 1) / w_;
   }
   std::vector<std::uint32_t> coverage(T, 0);
-  std::vector<std::uint32_t> a_read, a_qread, a_qbegin, a_qlen, a_tread, a_tbegin, a_tlen;
+  std::vector<std::uint32_t> a_qread, a_qbegin, a_qlen, a_tread, a_tbegin, a_tlen;
   std::vector<std::uint8_t> a_strand;
   std::vector<std::uint64_t> bp_off{0};
   for (std::uint32_t k = 0; k < S; ++k) {
@@ -176,7 +168,6 @@ std::vector<std::unique_ptr<biosoup::NucleicAcid>> Polisher::Polish(
     const double ql = o.lhs_end - o.lhs_begin, tl = o.rhs_end - o.rhs_begin;
     if (1 - std::min(ql, tl) / std::max(ql, tl) > e_) continue;
     ++coverage[o.rhs_id];
-    a_read.push_back(k);
     a_qread.push_back(T + k);
     a_qbegin.push_back(o.lhs_begin);
     a_qlen.push_back(o.lhs_end - o.lhs_begin);
@@ -188,7 +179,7 @@ std::vector<std::unique_ptr<biosoup::NucleicAcid>> Polisher::Polish(
         o.rhs_end > o.rhs_begin ? (o.rhs_end - 1) / w_ - o.rhs_begin / w_ + 1 : 0;
     bp_off.push_back(bp_off.back() + windows);
   }
-  const std::size_t A = a_read.size();
+  const std::size_t A = a_qread.size();
   std::vector<std::int32_t> a_dist(A);
   std::vector<std::uint32_t> bp(4 * bp_off.back() + 4);
   // (batches of about 2^29 query bases bound the device scratch of the alignment:
@@ -212,136 +203,22 @@ std::vector<std::unique_ptr<biosoup::NucleicAcid>> Polisher::Polish(
   }
   phase_seconds_[1] = Seconds(t_phase);
 
-  std::vector<std::future<std::vector<Piece>>> futures;
-  const std::size_t a_chunk = std::max<std::size_t>(64, A / 1024 + 1);
-  for (std::size_t a0 = 0; a0 < A; a0 += a_chunk) {
-    futures.emplace_back(thread_pool_->Submit(
-        [&](std::size_t a0, std::size_t a1) {
-          std::vector<Piece> pieces;
-          for (std::size_t a = a0; a < a1; ++a) {
-            const std::uint32_t k = a_read[a];
-            const auto& seq = *sequences[k];
-            biosoup::NucleicAcid view(seq);
-            // query positions are those of the aligned orientation of the read
-            std::uint32_t qb = a_qbegin[a];
-            if (!a_strand[a]) {
-              view.ReverseAndComplement();
-              qb = seq.inflated_len - (a_qbegin[a] + a_qlen[a]);
-            }
-            for (std::uint64_t s = bp_off[a]; s < bp_off[a + 1]; ++s) {
-              if (bp[4 * s] == 0xFFFFFFFFu) continue;  // no aligned pair in this window
-              const std::uint32_t ft = bp[4 * s], fq = qb + bp[4 * s + 1], lt = bp[4 * s + 2],
-                                  lq = qb + bp[4 * s + 3];
-              if (!(lq - fq >= 0.02 * w_)) continue;
-              if (!view.block_quality.empty()) {
-                double avg = 0;
-                for (std::uint32_t x = fq; x < lq; ++x) avg += view.Score(x);
-                avg /= lq - fq;
-                if (avg < q_) continue;
-              }
-              const std::uint32_t ws = (ft / w_) * w_;
-              if (ft - ws >= lt - ws - 1) continue;  // racon skips begin == end
-              pieces.push_back(Piece{first_window[a_tread[a]] + ft / w_, k, fq, lq, ft - ws,
-                                     lt - ws - 1, a_strand[a] != 0});
-            }
-          }
-          return pieces;
-        },
-        a0, std::min(A, a0 + a_chunk)));
+  // ---- 3. GPU: racon's layer rules, the layers of every window and their consensus,
+  //         in batches of windows (rvn_polish_windows) ----
+  std::vector<std::uint8_t> bq, rc(T + S, 0);
+  std::vector<std::uint64_t> bq_off(T + S + 1ULL, 0);
+  for (std::uint32_t i = 0; i < T + S; ++i) {
+    const auto& s = i < T ? *targets[i] : *sequences[i - T];
+    rc[i] = s.is_reverse_complement ? 1 : 0;
+    if (i >= T) bq.insert(bq.end(), s.block_quality.begin(), s.block_quality.end());
+    bq_off[i + 1] = bq.size();
   }
-  std::vector<Piece> pieces;
-  for (auto& f : futures) {
-    auto p = f.get();
-    pieces.insert(pieces.end(), p.begin(), p.end());
-  }
-  phase_seconds_[5] = Seconds(t_phase);
-
-  // ---- 3. windows in the flat layout of rvn_poa_batch ----
-  const std::uint64_t n_windows = first_window[T];
-  std::vector<std::uint32_t> layers_of(n_windows + 1, 0);
-  for (const auto& p : pieces) ++layers_of[p.window + 1];
-  std::vector<std::uint32_t> win_first(n_windows + 1, 0);
-  for (std::uint64_t w = 0; w < n_windows; ++w) {
-    win_first[w + 1] = win_first[w] + 1 + layers_of[w + 1];
-  }
-  const std::uint32_t n_seqs = win_first[n_windows];
-  std::vector<std::uint64_t> seq_off(n_seqs + 1ULL, 0);
-  std::vector<std::uint32_t> seq_begin(n_seqs, 0), seq_end(n_seqs, 0), slot(n_windows, 0);
-  // sizes first (arrival order of the layers = order of `pieces`)
-  std::vector<std::uint32_t> seq_len(n_seqs, 0);
-  {
-    std::uint64_t w = 0;
-    for (std::uint32_t i = 0; i < T; ++i) {
-      for (std::uint32_t j = 0; j < targets[i]->inflated_len; j += w_, ++w) {
-        seq_len[win_first[w]] = std::min(j + w_, targets[i]->inflated_len) - j;
-      }
-    }
-  }
-  std::vector<std::uint32_t> piece_seq(pieces.size());
-  for (std::size_t x = 0; x < pieces.size(); ++x) {
-    const auto& p = pieces[x];
-    const std::uint32_t s = win_first[p.window] + 1 + slot[p.window]++;
-    piece_seq[x] = s;
-    seq_len[s] = p.qe - p.qb;
-    seq_begin[s] = p.begin;
-    seq_end[s] = p.end;
-  }
-  for (std::uint32_t s = 0; s < n_seqs; ++s) seq_off[s + 1] = seq_off[s] + seq_len[s];
-  std::string bases(seq_off[n_seqs], 'A'), quals;
-  bool any_quality = false;
-  for (const auto& s : sequences) any_quality = any_quality || !s->block_quality.empty();
-  if (any_quality) quals.assign(seq_off[n_seqs], '!');
-  {
-    std::uint64_t w = 0;
-    for (std::uint32_t i = 0; i < T; ++i) {
-      for (std::uint32_t j = 0; j < targets[i]->inflated_len; j += w_, ++w) {
-        const std::uint32_t s = win_first[w];
-        const std::string bb = targets[i]->InflateData(j, seq_len[s]);
-        std::memcpy(&bases[seq_off[s]], bb.data(), bb.size());
-      }
-    }
-  }
-  // pieces of one read are contiguous (the futures were collected in read order):
-  // one (reverse complemented) view per read, reads spread over the pool
-  {
-    std::vector<std::future<void>> fills;
-    const std::size_t chunk = std::max<std::size_t>(256, pieces.size() / 1024 + 1);
-    for (std::size_t x0 = 0; x0 < pieces.size();) {
-      std::size_t x1 = std::min(pieces.size(), x0 + chunk);
-      while (x1 < pieces.size() && pieces[x1].read == pieces[x1 - 1].read) ++x1;
-      fills.emplace_back(thread_pool_->Submit(
-          [&](std::size_t x0, std::size_t x1) {
-            for (std::size_t x = x0; x < x1;) {
-              const std::uint32_t read = pieces[x].read;
-              biosoup::NucleicAcid view(*sequences[read]);
-              if (!pieces[x].strand) view.ReverseAndComplement();
-              for (; x < x1 && pieces[x].read == read; ++x) {
-                const auto& p = pieces[x];
-                const std::string d = view.InflateData(p.qb, p.qe - p.qb);
-                std::memcpy(&bases[seq_off[piece_seq[x]]], d.data(), d.size());
-                if (!any_quality) continue;
-                if (!view.block_quality.empty()) {
-                  const std::string qv = view.InflateQuality(p.qb, p.qe - p.qb);
-                  std::memcpy(&quals[seq_off[piece_seq[x]]], qv.data(), qv.size());
-                } else {
-                  std::memset(&quals[seq_off[piece_seq[x]]], '!' + 1, p.qe - p.qb);  // weight 1
-                }
-              }
-            }
-          },
-          x0, x1));
-      x0 = x1;
-    }
-    for (auto& f : fills) f.get();
-  }
-  phase_seconds_[2] = Seconds(t_phase);
-
-  // ---- 4. GPU: consensus of every window ----
   const auto t0 = std::chrono::steady_clock::now();
-  Check(ctx_, rvn_poa_batch(ctx_, static_cast<std::uint32_t>(n_windows), win_first.data(),
-                            seq_off.data(), bases.data(),
-                            any_quality ? quals.data() : nullptr, seq_begin.data(),
-                            seq_end.data(), m_, n_, g_, trim_, tgs, 0));
+  std::uint32_t batches = 0;
+  Check(ctx_, rvn_polish_windows(ctx_, A, a_qread.data(), a_qbegin.data(), a_qlen.data(),
+                                 a_strand.data(), a_tread.data(), bp_off.data(), bp.data(), T, w_,
+                                 bq.empty() ? nullptr : bq.data(), bq_off.data(), rc.data(), q_,
+                                 m_, n_, g_, trim_, tgs, &batches));
   const char* cons = nullptr;
   const std::uint64_t* cons_off = nullptr;
   const std::uint8_t* status = nullptr;
@@ -349,10 +226,24 @@ std::vector<std::unique_ptr<biosoup::NucleicAcid>> Polisher::Polish(
   std::uint32_t routes[3] = {0, 0, 0};
   Check(ctx_, rvn_poa_routes(ctx_, routes, nullptr));
   num_wide_windows_ = routes[2];
+  num_window_batches_ = batches;
   poa_seconds_ = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-  phase_seconds_[3] = Seconds(t_phase);
+  // the device time of the layer rules and of the packing (rvn_get_timings)
+  double layers_s = 0, pack_s = 0;
+  const char* const* names = nullptr;
+  const float* ms = nullptr;
+  std::uint32_t n_phases = 0;
+  Check(ctx_, rvn_get_timings(ctx_, &names, &ms, &n_phases));
+  for (std::uint32_t i = 0; i < n_phases; ++i) {
+    if (std::strcmp(names[i], "poa_layers") == 0) layers_s += ms[i] / 1000;
+    if (std::strcmp(names[i], "poa_pack") == 0) pack_s += ms[i] / 1000;
+  }
+  const double consensus_s = Seconds(t_phase);
+  phase_seconds_[5] = layers_s;
+  phase_seconds_[2] = pack_s;
+  phase_seconds_[3] = std::max(0.0, consensus_s - layers_s - pack_s);
 
-  // ---- 5. stitch ----
+  // ---- 4. stitch ----
   std::vector<std::unique_ptr<biosoup::NucleicAcid>> dst;
   for (std::uint32_t i = 0; i < T; ++i) {
     const std::uint64_t w0 = first_window[i], w1 = first_window[i + 1];

@@ -2,8 +2,9 @@
 ``racon::Polisher::Create(pool, q, e, w, trim, m, n, g, ...)->Polish(targets,
 sequences, false)`` (RavenLib/src/polish.cc:43-51) through
 raven_b200/libraven_b200_host.so (raven_b200/host/host_api.cc).  GPU: read-to-target
-mapping and the window consensus (POA); host pool: alignment paths and window
-cutting.  There is no CPU path."""
+mapping, alignment paths and window cuts, racon's layer rules, the window layers and
+their consensus (POA); host: best overlap per read and stitching.  There is no CPU
+path."""
 from __future__ import annotations
 
 import ctypes as C
@@ -42,8 +43,9 @@ def _load():
 
 def polish(targets, sequences, q=0.0, e=0.3, w=500, trim=True, m=3, n=-5, g=-4, threads=4):
     """Polished targets (ReadSet with names) and stats: windows, polished windows,
-    windows on the wide consensus kernel (deeper than the 16-bit kernels take),
-    seconds in the consensus phase (H2D + POA kernels + D2H), total seconds."""
+    windows on the wide consensus kernel (deeper than the 16-bit kernels take), the
+    window batches of the consensus, seconds in the consensus phase (device layer
+    build + POA kernels + D2H), total seconds."""
     lib = _load()
     u64p, u32p, u8p = (C.POINTER(C.c_uint64), C.POINTER(C.c_uint32), C.POINTER(C.c_uint8))
 
@@ -84,7 +86,8 @@ def polish(targets, sequences, q=0.0, e=0.3, w=500, trim=True, m=3, n=-5, g=-4, 
         rs.names = lib.rvnh_polish_names(h).decode().split("\n")[:-1]
         st = lib.rvnh_polish_stats(h)
         stats = dict(windows=int(st[0]), polished_windows=int(st[1]),
-                     wide_windows=int(st[10]), poa_seconds=st[2],
+                     wide_windows=int(st[10]), window_batches=int(st[11]),
+                     poa_seconds=st[2],
                      seconds=st[3],
                      phases_s=dict(map=st[4], align=st[5], pack=st[6], consensus=st[7],
                                    stitch=st[8], pieces=st[9]))
