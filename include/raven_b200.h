@@ -378,12 +378,25 @@ int rvn_map_hits(rvn_ctx* ctx, const uint64_t** group,
                  uint64_t* n_hits);
 
 /* The engine's stable LSD radix sort (raven_b200/csrc/radix.cu - it orders the
- * minimizer index, construct.cc:42-43) on host arrays, in place: keys of 4 or 8
- * bytes, values of 0 (u32 keys only), 4 or 8 bytes, key bits [begin_bit,
- * end_bit); equal keys keep their input order. */
+ * minimizer index, construct.cc:42-43), in place: keys of 4 or 8 bytes, values of
+ * 0 (u32 keys only), 4 or 8 bytes, key bits [begin_bit, end_bit), n < 2^32 - 1;
+ * equal keys keep their input order. keys and vals are both host or both device
+ * memory; device arrays are sorted where they are, with one more buffer per array. */
 int rvn_debug_sort_pairs(rvn_ctx* ctx, int key_bytes, int val_bytes, void* keys,
                          void* vals, uint64_t n, int begin_bit, int end_bit,
                          int descending);
+
+/* The engine's unstable radix partition of u32 keys on bits [begin_bit, end_bit)
+ * (1 to 10 bits), in place: the keys of digit d end in keys[bin_start[d],
+ * bin_start[d + 1]) in any order (bin_start: 1024 entries, n for the digits past
+ * the bit range). keys and bin_start are host or device memory, each on its own. */
+int rvn_debug_partition_keys(rvn_ctx* ctx, uint32_t* keys, uint64_t n, int begin_bit,
+                             int end_bit, uint32_t* bin_start);
+
+/* The engine's exclusive scan of u32 counts into u64 offsets: out[i] = in[0] + ... +
+ * in[i - 1] for i in [0, n] (n + 1 entries). in and out are host or device memory,
+ * each on its own. */
+int rvn_debug_exclusive_scan(rvn_ctx* ctx, const uint32_t* in, uint64_t n, uint64_t* out);
 
 int rvn_get_stats(rvn_ctx* ctx, rvn_stats* out);
 
@@ -428,6 +441,11 @@ int rvn_get_stats(rvn_ctx* ctx, rvn_stats* out);
  * path, results do not depend on it); "poa_wide" and "poa_scratch_budget" (rvn_poa_batch and
  * rvn_polish_windows); "poa_batch_bytes" (rvn_polish_windows: the device inputs of one window
  * batch, 0 = the default, from the free device memory; results do not depend on it);
+ * "radix_portion_tiles" (a radix sort or partition over more than about 2^30 records
+ * runs in portions, the last tile of each handing the running bin ends to the next;
+ * N > 0 cuts portions of N tiles - 8192 records for u32 keys, 4096 for u64 keys -
+ * or of as few more as keep the launches of a sort within 64; 0 = the default, the
+ * longest portion; for tests of the portion path, results do not depend on it);
  * "reset_stats".
  * Unknown name or value out of range -> RVN_ERR_INVALID. */
 int rvn_set_option(rvn_ctx* ctx, const char* name, int64_t value);

@@ -90,6 +90,9 @@ SIGNATURES = {
                                             U64P, C.POINTER(C.c_int32), U32P]),
     "rvn_debug_sort_pairs": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                        C.c_uint64, C.c_int, C.c_int, C.c_int]),
+    "rvn_debug_partition_keys": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int,
+                                           C.c_int, C.c_void_p]),
+    "rvn_debug_exclusive_scan": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     "rvn_get_stats": (C.c_int, [C.c_void_p, C.POINTER(Stats)]),
     "rvn_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int64]),
     "rvn_get_timings": (C.c_int, [C.c_void_p, C.POINTER(C.POINTER(C.c_char_p)),

@@ -730,6 +730,9 @@ void SetOption(Ctx& c, const char* name, int64_t value) {
   } else if (name && std::strcmp(name, "poa_batch_bytes") == 0) {
     if (value < 0) throw InvalidArgument("poa_batch_bytes: bytes, 0 = from the device memory");
     c.poa_batch_bytes = static_cast<uint64_t>(value);
+  } else if (name && std::strcmp(name, "radix_portion_tiles") == 0) {
+    if (value < 0) throw InvalidArgument("radix_portion_tiles: tiles, 0 = the longest portion");
+    c.radix_portion_tiles = value;
   } else if (name && std::strcmp(name, "reset_stats") == 0) {
     std::memset(&c.stats, 0, sizeof(c.stats));
     c.launches = 0;
@@ -1382,7 +1385,19 @@ RVN_API int rvn_align_breaking_points(rvn_ctx* ctx, uint64_t n_pairs, const uint
   });
 }
 
-// the engine's radix sort on host arrays (parity tests of radix.cu)
+// whether p is device memory: the debug entry points below take host or device arrays
+static bool OnDevice(const void* p) {
+  cudaPointerAttributes a{};
+  if (!p || cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();  // (clears the error of a pointer CUDA does not know)
+    return false;
+  }
+  return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+}
+
+// the engine's radix sort, in place (parity tests of radix.cu). Host arrays travel
+// through three device buffers per array; device arrays are the sort's source and its
+// buffer b, so that only buffer a is allocated.
 RVN_API int rvn_debug_sort_pairs(rvn_ctx* ctx, int key_bytes, int val_bytes, void* keys,
                                  void* vals, uint64_t n, int begin_bit, int end_bit,
                                  int descending) {
@@ -1394,42 +1409,106 @@ RVN_API int rvn_debug_sort_pairs(rvn_ctx* ctx, int key_bytes, int val_bytes, voi
     if (begin_bit < 0 || end_bit > 8 * key_bytes || begin_bit > end_bit) {
       throw InvalidArgument("bit range out of bounds");
     }
+    if (n >= 0xFFFFFFFFULL) throw LimitError("radix sort of 2^32 or more records");
     if (n && (!keys || (val_bytes && !vals))) throw InvalidArgument("null arrays");
+    const bool dev = n && OnDevice(keys);
+    if (val_bytes && n && OnDevice(vals) != dev) {
+      throw InvalidArgument("keys and values both on the device or both on the host");
+    }
+    const size_t kbytes = static_cast<size_t>(key_bytes) * n, vbytes = static_cast<size_t>(val_bytes) * n;
     DevBuf<uint8_t> ks, ka, kb, vs, va, vb;
-    const size_t kb_ = static_cast<size_t>(key_bytes) * n + 16, vb_ = static_cast<size_t>(val_bytes) * n + 16;
-    ks.reserve(kb_); ka.reserve(kb_); kb.reserve(kb_);
-    vs.reserve(vb_); va.reserve(vb_); vb.reserve(vb_);
-    RVN_CUDA(cudaMemcpyAsync(ks.get(), keys, static_cast<size_t>(key_bytes) * n, cudaMemcpyHostToDevice, c.stream));
-    if (val_bytes) {
-      RVN_CUDA(cudaMemcpyAsync(vs.get(), vals, static_cast<size_t>(val_bytes) * n, cudaMemcpyHostToDevice, c.stream));
+    uint8_t *k_src, *k_a, *k_b, *v_src, *v_a, *v_b;
+    k_a = ka.reserve(kbytes + 16);
+    v_a = va.reserve(vbytes + 16);
+    if (dev) {
+      k_src = k_b = static_cast<uint8_t*>(keys);
+      v_src = v_b = val_bytes ? static_cast<uint8_t*>(vals) : vb.reserve(16);
+    } else {
+      k_src = ks.reserve(kbytes + 16);
+      k_b = kb.reserve(kbytes + 16);
+      v_src = vs.reserve(vbytes + 16);
+      v_b = vb.reserve(vbytes + 16);
+      RVN_CUDA(cudaMemcpyAsync(k_src, keys, kbytes, cudaMemcpyHostToDevice, c.stream));
+      if (val_bytes) RVN_CUDA(cudaMemcpyAsync(v_src, vals, vbytes, cudaMemcpyHostToDevice, c.stream));
     }
     int where;
     const bool desc = descending != 0;
     if (val_bytes == 0) {
-      where = RadixSortKeys(c, (const uint32_t*)ks.get(), (uint32_t*)ka.get(), (uint32_t*)kb.get(), n,
+      where = RadixSortKeys(c, (const uint32_t*)k_src, (uint32_t*)k_a, (uint32_t*)k_b, n,
                             begin_bit, end_bit);
     } else if (key_bytes == 4 && val_bytes == 8) {
-      where = RadixSortPairs(c, (const uint32_t*)ks.get(), (uint32_t*)ka.get(), (uint32_t*)kb.get(),
-                             (const uint64_t*)vs.get(), (uint64_t*)va.get(), (uint64_t*)vb.get(), n,
+      where = RadixSortPairs(c, (const uint32_t*)k_src, (uint32_t*)k_a, (uint32_t*)k_b,
+                             (const uint64_t*)v_src, (uint64_t*)v_a, (uint64_t*)v_b, n,
                              begin_bit, end_bit, desc);
     } else if (key_bytes == 8 && val_bytes == 8) {
-      where = RadixSortPairs(c, (const uint64_t*)ks.get(), (uint64_t*)ka.get(), (uint64_t*)kb.get(),
-                             (const uint64_t*)vs.get(), (uint64_t*)va.get(), (uint64_t*)vb.get(), n,
+      where = RadixSortPairs(c, (const uint64_t*)k_src, (uint64_t*)k_a, (uint64_t*)k_b,
+                             (const uint64_t*)v_src, (uint64_t*)v_a, (uint64_t*)v_b, n,
                              begin_bit, end_bit, desc);
     } else if (key_bytes == 4 && val_bytes == 4) {
-      where = RadixSortPairs(c, (const uint32_t*)ks.get(), (uint32_t*)ka.get(), (uint32_t*)kb.get(),
-                             (const uint32_t*)vs.get(), (uint32_t*)va.get(), (uint32_t*)vb.get(), n,
+      where = RadixSortPairs(c, (const uint32_t*)k_src, (uint32_t*)k_a, (uint32_t*)k_b,
+                             (const uint32_t*)v_src, (uint32_t*)v_a, (uint32_t*)v_b, n,
                              begin_bit, end_bit, desc);
     } else {
-      where = RadixSortPairs(c, (const uint64_t*)ks.get(), (uint64_t*)ka.get(), (uint64_t*)kb.get(),
-                             (const uint32_t*)vs.get(), (uint32_t*)va.get(), (uint32_t*)vb.get(), n,
+      where = RadixSortPairs(c, (const uint64_t*)k_src, (uint64_t*)k_a, (uint64_t*)k_b,
+                             (const uint32_t*)v_src, (uint32_t*)v_a, (uint32_t*)v_b, n,
                              begin_bit, end_bit, desc);
     }
-    const uint8_t* rk = where < 0 ? ks.get() : (where == 0 ? ka.get() : kb.get());
-    const uint8_t* rv = where < 0 ? vs.get() : (where == 0 ? va.get() : vb.get());
-    RVN_CUDA(cudaMemcpyAsync(keys, rk, static_cast<size_t>(key_bytes) * n, cudaMemcpyDeviceToHost, c.stream));
-    if (val_bytes) {
-      RVN_CUDA(cudaMemcpyAsync(vals, rv, static_cast<size_t>(val_bytes) * n, cudaMemcpyDeviceToHost, c.stream));
+    const uint8_t* rk = where < 0 ? k_src : (where == 0 ? k_a : k_b);
+    const uint8_t* rv = where < 0 ? v_src : (where == 0 ? v_a : v_b);
+    if (rk != keys) {  // (device arrays: only a result in buffer a moves)
+      RVN_CUDA(cudaMemcpyAsync(keys, rk, kbytes, cudaMemcpyDefault, c.stream));
+      if (val_bytes) RVN_CUDA(cudaMemcpyAsync(vals, rv, vbytes, cudaMemcpyDefault, c.stream));
+    }
+    RVN_CUDA(cudaStreamSynchronize(c.stream));
+  });
+}
+
+// the engine's unstable radix partition (RadixPartitionKeys), in place: keys (u32) and
+// bin_start (1024 entries) on the host or on the device, each on its own
+RVN_API int rvn_debug_partition_keys(rvn_ctx* ctx, uint32_t* keys, uint64_t n, int begin_bit,
+                                     int end_bit, uint32_t* bin_start) {
+  return Guard(ctx, [&](Ctx& c) {
+    if (begin_bit < 0 || end_bit > 32 || end_bit - begin_bit < 1 || end_bit - begin_bit > 10) {
+      throw InvalidArgument("1 to 10 key bits inside 32");
+    }
+    if (n >= 0xFFFFFFFFULL) throw LimitError("radix partition of 2^32 or more records");
+    if ((n && !keys) || !bin_start) throw InvalidArgument("null arrays");
+    const size_t bytes = sizeof(uint32_t) * n;
+    DevBuf<uint32_t> src_buf, dst_buf, start_buf;
+    const bool dev = n && OnDevice(keys);
+    uint32_t* src = dev ? keys : src_buf.reserve(n + 1);
+    uint32_t* dst = dst_buf.reserve(n + 1);  // (the pass cannot write over its source)
+    uint32_t* start = OnDevice(bin_start) ? bin_start : start_buf.reserve(1024);
+    if (!dev && n) RVN_CUDA(cudaMemcpyAsync(src, keys, bytes, cudaMemcpyHostToDevice, c.stream));
+    RadixPartitionKeys(c, src, dst, n, begin_bit, end_bit, start);
+    if (n) RVN_CUDA(cudaMemcpyAsync(keys, dst, bytes, cudaMemcpyDefault, c.stream));
+    if (start != bin_start) {
+      RVN_CUDA(cudaMemcpyAsync(bin_start, start, 1024 * sizeof(uint32_t), cudaMemcpyDeviceToHost,
+                               c.stream));
+    }
+    RVN_CUDA(cudaStreamSynchronize(c.stream));
+  });
+}
+
+// the engine's exclusive scan (ExclusiveScanU32): out[i] = in[0] + ... + in[i - 1] for
+// i in [0, n]; in and out on the host or on the device, each on its own
+RVN_API int rvn_debug_exclusive_scan(rvn_ctx* ctx, const uint32_t* in, uint64_t n,
+                                     uint64_t* out) {
+  return Guard(ctx, [&](Ctx& c) {
+    if ((n && !in) || !out) throw InvalidArgument("null arrays");
+    DevBuf<uint32_t> in_buf;
+    DevBuf<uint64_t> out_buf;
+    const uint32_t* d_in = in;
+    if (n && !OnDevice(in)) {
+      d_in = in_buf.reserve(n);
+      RVN_CUDA(cudaMemcpyAsync(const_cast<uint32_t*>(d_in), in, sizeof(uint32_t) * n,
+                               cudaMemcpyHostToDevice, c.stream));
+    }
+    uint64_t* d_out = OnDevice(out) ? out : out_buf.reserve(n + 1);
+    ExclusiveScanU32(c, d_in, d_out, n);
+    if (d_out != out) {
+      RVN_CUDA(cudaMemcpyAsync(out, d_out, sizeof(uint64_t) * (n + 1), cudaMemcpyDeviceToHost,
+                               c.stream));
     }
     RVN_CUDA(cudaStreamSynchronize(c.stream));
   });

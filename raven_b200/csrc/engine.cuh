@@ -152,6 +152,9 @@ struct Ctx {
   bool i_sorted_ids = false;  // postings of a key are in ascending read-id order
   bool ids_ascending = true;  // read ids never decrease with the read index
   DevBuf<uint8_t> sort_tmp;
+  // option "radix_portion_tiles": a radix sort or partition runs in portions of at
+  // most that many tiles (0: the longest portion its status words allow)
+  int64_t radix_portion_tiles = 0;
 
   // ---- map ----
   DevBuf<uint32_t> m_cnt, m_first;

@@ -481,6 +481,20 @@ PassPlan MakePlan(int begin_bit, int end_bit) {
   return plan;
 }
 
+// Tiles per portion of a sort or partition over `tiles` tiles of `tile` records. A
+// status word counts below 2^30, so a portion holds at most (2^30 - 1) / tile tiles;
+// the last tile of a portion hands the running bin ends to the next one. Option
+// "radix_portion_tiles" (> 0) cuts portions of that many tiles instead, so that the
+// handoff runs at small sizes, but never more portions than the kMaxPasses * 8
+// tickets allow over n_passes passes.
+uint64_t PortionTiles(const Ctx& c, uint64_t tile, uint64_t tiles, int n_passes) {
+  const uint64_t cap = ((1ULL << 30) - 1) / tile;
+  const uint64_t want =
+      c.radix_portion_tiles > 0 ? std::min<uint64_t>(c.radix_portion_tiles, cap) : cap;
+  const uint64_t per_pass = kMaxPasses * 8 / n_passes;
+  return std::min(cap, std::max(want, (tiles + per_pass - 1) / per_pass));
+}
+
 template <typename KeyT, typename ValT, bool HAS_VAL>
 int SortImpl(Ctx& c, const KeyT* src_keys, KeyT* keys_a, KeyT* keys_b, const ValT* src_vals,
              ValT* vals_a, ValT* vals_b, uint64_t n, int begin_bit, int end_bit,
@@ -491,9 +505,8 @@ int SortImpl(Ctx& c, const KeyT* src_keys, KeyT* keys_a, KeyT* keys_b, const Val
   using Smem = PassSmem<KeyT, ValT, HAS_VAL>;
   constexpr uint64_t kTile = Smem::kTile;
   const KeyT flip = descending ? static_cast<KeyT>(~static_cast<KeyT>(0)) : static_cast<KeyT>(0);
-  // a status word counts below 2^30: longer inputs go portion by portion, the
-  // last tile of a portion hands the running bin ends to the next one
-  const uint64_t portion = ((1ULL << 30) - 1) / kTile * kTile;
+  // longer inputs go portion by portion (PortionTiles)
+  const uint64_t portion = PortionTiles(c, kTile, (n + kTile - 1) / kTile, plan.n_passes) * kTile;
   const uint64_t n_portions = (n + portion - 1) / portion;
   const uint64_t max_tiles = (std::min(n, portion) + kTile - 1) / kTile;
   // scratch: [hist: passes*kBins u64][bin bases: 2 x passes*kBins u32][tickets][status]
@@ -602,7 +615,7 @@ void RadixPartitionKeys(Ctx& c, const uint32_t* src, uint32_t* dst, uint64_t n, 
   plan.bits[0] = end_bit - begin_bit;
   constexpr uint64_t kTile = kThreads * Items<uint32_t>::value;
   // status words count below 2^30: portion by portion, as in SortImpl
-  const uint64_t portion = ((1ULL << 30) - 1) / kTile * kTile;
+  const uint64_t portion = PortionTiles(c, kTile, (n + kTile - 1) / kTile, 1) * kTile;
   const uint64_t n_portions = (n + portion - 1) / portion;
   const uint64_t max_tiles = (std::min(n, portion) + kTile - 1) / kTile;
   const size_t hist_bytes = sizeof(uint64_t) * kBins;
@@ -629,7 +642,7 @@ void RadixPartitionKeys(Ctx& c, const uint32_t* src, uint32_t* dst, uint64_t n, 
   RadixScanBinsKernel<<<1, kBins, 0, c.stream>>>(hist, 1, bases[0]);
   RVN_LAUNCH_CHECK();
   c.launches += 2;
-  // (bases[0] is overwritten from the third portion on)
+  // (the second portion overwrites bases[0] with its bin ends)
   RVN_CUDA(cudaMemcpyAsync(bin_start, bases[0], base_bytes, cudaMemcpyDeviceToDevice, c.stream));
   RVN_CUDA(cudaFuncSetAttribute(PartitionPass, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 static_cast<int>(sizeof(PartitionSmem))));

@@ -33,6 +33,22 @@ def _arr(ptr, n, dtype):
     return np.frombuffer(buf, dtype=dtype).copy()
 
 
+def _is_tensor(x):
+    return hasattr(x, "data_ptr") and hasattr(x, "element_size")
+
+
+def _tensor_ptr(t):
+    """device address of a torch tensor for a call on the context's own stream, which
+    nothing orders after torch's: waits for the work queued on torch's current stream
+    (the writes of t). The debug calls that take tensors synchronise their stream before
+    they return, so torch's later reads see their results."""
+    if not (t.is_cuda and t.is_contiguous()):
+        raise ValueError("a contiguous CUDA tensor")
+    import torch
+    torch.cuda.current_stream(t.device).synchronize()
+    return t.data_ptr()
+
+
 class Engine:
     def __init__(self, device: int = 0, stream: int | None = None):
         self.lib = _lib.load()
@@ -307,15 +323,47 @@ class Engine:
                     cons_off=cons_off, status=_arr(sts, nw, np.uint8), batches=batches.value)
 
     def debug_sort_pairs(self, keys, vals=None, begin_bit=0, end_bit=None, descending=False):
-        """The engine's stable radix sort (csrc/radix.cu) on host arrays; returns copies."""
-        k = np.ascontiguousarray(keys).copy()
-        v = None if vals is None else np.ascontiguousarray(vals).copy()
-        end_bit = 8 * k.itemsize if end_bit is None else end_bit
-        self._check(self.lib.rvn_debug_sort_pairs(
-            self.h, k.itemsize, 0 if v is None else v.itemsize, k.ctypes.data_as(C.c_void_p),
-            None if v is None else v.ctypes.data_as(C.c_void_p), k.size, begin_bit, end_bit,
-            int(descending)))
+        """The engine's stable radix sort (csrc/radix.cu). numpy arrays: returns sorted
+        copies. Contiguous CUDA tensors (torch, 4- or 8-byte elements taken as unsigned):
+        sorted in place and returned."""
+        if _is_tensor(keys):
+            k, v = keys, vals
+            kb, vb = k.element_size(), 0 if v is None else v.element_size()
+            kp, vp, n = _tensor_ptr(k), None if v is None else _tensor_ptr(v), k.numel()
+        else:
+            k = np.ascontiguousarray(keys).copy()
+            v = None if vals is None else np.ascontiguousarray(vals).copy()
+            kb, vb = k.itemsize, 0 if v is None else v.itemsize
+            kp, vp, n = k.ctypes.data, None if v is None else v.ctypes.data, k.size
+        end_bit = 8 * kb if end_bit is None else end_bit
+        self._check(self.lib.rvn_debug_sort_pairs(self.h, kb, vb, kp, vp, n, begin_bit, end_bit,
+                                                  int(descending)))
         return k, v
+
+    def debug_partition_keys(self, keys, begin_bit, end_bit):
+        """The engine's unstable radix partition of u32 keys on bits [begin_bit, end_bit)
+        (csrc/radix.cu, 1 to 10 bits): the partitioned keys (a copy of a numpy array, a
+        contiguous 4-byte CUDA tensor in place) and the first position of every one of
+        the 1024 digits (numpy)."""
+        start = np.zeros(1024, np.uint32)
+        if _is_tensor(keys):
+            assert keys.element_size() == 4
+            k, kp, n = keys, _tensor_ptr(keys), keys.numel()
+        else:
+            k = np.ascontiguousarray(keys, dtype=np.uint32).copy()
+            kp, n = k.ctypes.data, k.size
+        self._check(self.lib.rvn_debug_partition_keys(self.h, kp, n, begin_bit, end_bit,
+                                                      start.ctypes.data))
+        return k, start
+
+    def debug_exclusive_scan(self, values):
+        """The engine's exclusive scan of u32 counts (csrc/scan.cu) on a host array: the
+        n + 1 u64 offsets."""
+        v = np.ascontiguousarray(values, dtype=np.uint32)
+        out = np.zeros(v.size + 1, np.uint64)
+        self._check(self.lib.rvn_debug_exclusive_scan(self.h, v.ctypes.data, v.size,
+                                                      out.ctypes.data))
+        return out
 
     # ---- bookkeeping ----
     def set_option(self, name, value):
