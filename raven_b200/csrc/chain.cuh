@@ -143,25 +143,33 @@ struct ColumnLis {
   }
 };
 
-// Binary insertion sort of elements [0, n) by operator<, get(i) reading element i
-// and set(i, v) writing it: stable, and one comparison for an element in order.
+// Shell sort of elements [0, n) by operator<, get(i) reading element i and set(i, v)
+// writing it (Ciura's gaps, then a plain insertion pass). Not stable: the callers' keys
+// tie only on bitwise-equal hits. A pair's hits arrive in no order, and the gapped passes
+// move each of them a few times where an insertion sort moves about n / 4 per element.
 template <typename Get, typename Set>
-RVN_HD void InsertionSort(uint32_t n, const Get& get, const Set& set) {
-  for (uint32_t a = 1; a < n; ++a) {
-    const auto v = get(a);
-    if (!(v < get(a - 1))) continue;
-    uint32_t lo = 0, hi = a - 1;  // the first element above v lies in [lo, hi]
-    while (lo < hi) {
-      const uint32_t mid = (lo + hi) >> 1;
-      if (v < get(mid)) {
-        hi = mid;
-      } else {
-        lo = mid + 1;
+RVN_HD void ShellSort(uint32_t n, const Get& get, const Set& set) {
+  auto pass = [&](uint32_t gap) {
+    for (uint32_t a = gap; a < n; ++a) {
+      const auto v = get(a);
+      uint32_t b = a;
+      for (; b >= gap; b -= gap) {
+        const auto u = get(b - gap);
+        if (!(v < u)) break;
+        set(b, u);
       }
+      if (b != a) set(b, v);
     }
-    for (uint32_t b = a; b > lo; --b) set(b, get(b - 1));
-    set(lo, v);
-  }
+  };
+  if (n > 1750) pass(1750);
+  if (n > 701) pass(701);
+  if (n > 301) pass(301);
+  if (n > 132) pass(132);
+  if (n > 57) pass(57);
+  if (n > 23) pass(23);
+  if (n > 10) pass(10);
+  if (n > 4) pass(4);
+  pass(1);
 }
 
 struct DiagPos {
@@ -176,17 +184,29 @@ struct DiagPos {
 template <typename Emit>
 RVN_HD void ChainPairSerial(const Column& c, uint32_t m, uint32_t gid, uint32_t lhs_id,
                             const ChainParams& cp, Emit&& emit) {
-  InsertionSort(m, [&](uint32_t i) { return DiagPos{c.d(i), c.p(i)}; },
-                [&](uint32_t i, DiagPos v) {
-                  c.d(i) = v.d;
-                  c.p(i) = v.p;
-                });
+  // A pair whose diagonals all lie within the bandwidth is one window, hence one band of
+  // all its hits, which the band step puts in position order anyway: the (diagonal,
+  // positions) sort is only needed when the pair spans more than the bandwidth.
+  uint32_t dmin = 0xFFFFFFFFu, dmax = 0;
+  for (uint32_t i = 0; i < m; ++i) {
+    const uint32_t d = c.d(i);
+    dmin = d < dmin ? d : dmin;
+    dmax = d > dmax ? d : dmax;
+  }
+  const bool one_band = m == 0 || dmax - dmin <= cp.bandwidth;
+  if (!one_band) {
+    ShellSort(m, [&](uint32_t i) { return DiagPos{c.d(i), c.p(i)}; },
+                  [&](uint32_t i, DiagPos v) {
+                    c.d(i) = v.d;
+                    c.p(i) = v.p;
+                  });
+  }
   const bool strand = gid & 1;
   const uint32_t rhs_id = gid >> 1;
   // one band [jb, ie): position order, then the chain rules
   auto band = [&](uint32_t jb, uint32_t ie) {
     const uint32_t len = ie - jb;
-    InsertionSort(len, [&](uint32_t i) { return c.p(jb + i); },
+    ShellSort(len, [&](uint32_t i) { return c.p(jb + i); },
                   [&](uint32_t i, uint64_t v) { c.p(jb + i) = v; });
     const ColumnLis lis{c, jb};
     const uint32_t longest =
@@ -196,6 +216,10 @@ RVN_HD void ChainPairSerial(const Column& c, uint32_t m, uint32_t gid, uint32_t 
                           emit(MakeOverlap(lhs_id, rhs_id, strand, cp.k, first, last, score));
                         });
   };
+  if (one_band) {  // (the window loop below would give the band [0, m) for m >= 4)
+    if (m >= 4) band(0, m);
+    return;
+  }
   // the reference's window loop; index m plays the stop dummy
   bool open = false;
   uint32_t ob = 0, oe = 0;

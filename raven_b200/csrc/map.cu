@@ -591,7 +591,7 @@ __device__ uint32_t ChainRead(const ChainWork<IdxT>& wk, uint32_t n,
 constexpr uint32_t kChainSmemCap = 65535;  // hits per read on the split path (16-bit offsets)
 constexpr uint32_t kSplitMaxTable = 8192;  // pair hash table entries per read, at most
 constexpr uint32_t kPairMaxHits = 8191;    // hits of one pair PairChainKernel holds on chip
-constexpr uint32_t kThreadPairMax = 48;   // larger (rhs, strand) pairs get a CTA each
+constexpr uint32_t kThreadPairMax = 63;   // larger (rhs, strand) pairs get a CTA each
 
 // ---------------------------------------------------------------------------
 // Fast path, two kernels.
@@ -1250,10 +1250,10 @@ constexpr int kSplitClasses = sizeof(kSplitBounds) / sizeof(kSplitBounds[0]);
 // kPairBounds[b + 1] < hits <= kPairBounds[b]; a CTA per pair (PairChainKernel, shared
 // memory by class) above kThreadPairMax, a thread per pair from there on
 // (GroupChainKernel: shared memory per CTA = threads x class bound x 12 B)
-constexpr uint32_t kPairBounds[] = {8191, 4095, 2047, 1023, 511, 255, 127, 63,
-                                    kThreadPairMax, 32, 24, 16, 8};
+constexpr uint32_t kPairBounds[] = {8191, 4095, 2047, 1023, 511, 255, 127,
+                                    kThreadPairMax, 48, 32, 24, 16, 8};
 constexpr uint32_t kPairClasses = sizeof(kPairBounds) / sizeof(kPairBounds[0]);
-constexpr uint32_t kFirstThreadClass = 8;
+constexpr uint32_t kFirstThreadClass = 7;
 static_assert(kPairBounds[kFirstThreadClass] == kThreadPairMax,
               "pairs of up to kThreadPairMax hits get a thread each");
 constexpr int kGroupSmemLimit = 200 * 1024;        // GroupChainKernel's dynamic shared memory
