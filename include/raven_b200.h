@@ -31,6 +31,10 @@
  *   rvn_find_overlaps_and_create_piles
  *                          raven::FindOverlapsAndCreatePiles
  *                                                      RavenLib/src/construct.cc:14-121
+ *   rvn_find_overlaps_and_repetitive_regions
+ *                          the map, Pile::AddKmers and identity-filter part of
+ *                          raven::FindOverlapsAndRepetetiveRegions
+ *                                                      RavenLib/src/construct.cc:352-424
  *
  * The C++ facade over this ABI (include/ram/minimizer_engine.hpp and
  * raven_b200/host/) keeps the reference's class and function signatures, so
@@ -223,6 +227,43 @@ int rvn_align_breaking_points(rvn_ctx* ctx, uint64_t n_pairs, const uint32_t* q_
                               const uint32_t* t_begin, const uint32_t* t_len, uint32_t window,
                               const uint64_t* bp_off, int32_t* distance,
                               uint32_t* breaking_points);
+
+/* raven::FindOverlapsAndRepetetiveRegions up to its classification loop
+ * (RavenLib/src/construct.cc:352-424; the loop, :430-455, and what follows it stay with
+ * the caller). The caller uploads the reads in the reference's sorted order (valid
+ * piles first, then by id, construct.cc:325-334), with their ids (rvn_reads_upload_ids);
+ * n_valid is that order's s (construct.cc:343-349: 0 when no pile is invalid, and then
+ * nothing is mapped). region_begin[i] / region_end[i]: Pile::begin() / end() of valid
+ * read i, in bases.
+ * Schedule, as the reference's: index batches [j, i + 1) of the valid reads, cut when
+ * they reach 1U << 30 bases (option "stage2_batch_bases" forces a smaller cut), each an
+ * untiered full-sketch index (Minimize) filtered at `frequency` (Filter); then every
+ * valid read of [0, i + 1) is mapped (avoid equal, avoid symmetric, no minhash, filtered
+ * positions kept: construct.cc:377-381) in rvn_map's flushes. On the device, per flush:
+ *  - the filtered positions that pass Pile::AddKmers' complexity test (pile.cc:64-120)
+ *    set bit position >> 4 of their read's bitmap, ORed over all batches;
+ *  - identity != 0: each overlap is clipped to the valid regions (raven::OverlapUpdate,
+ *    overlap_utils.cc:14-60) and kept iff 1 - ed / max(len) >= identity (edlibAlign of
+ *    the clipped substrings, construct.cc:385-424); identity == 0: overlaps unchanged.
+ * Results by rvn_stage2_results. */
+int rvn_find_overlaps_and_repetitive_regions(rvn_ctx* ctx, double frequency, double identity,
+                                             uint32_t n_valid, const uint32_t* region_begin,
+                                             const uint32_t* region_end);
+/* Results of the last rvn_find_overlaps_and_repetitive_regions call:
+ *  - overlaps: the final (clipped, kept) overlaps of every batch in the order the
+ *    reference's classification loop consumes them: batch by batch, query read by query
+ *    read, in emission order; overlap_off (n_valid + 1): a batch that ends at valid read i
+ *    holds overlaps [overlap_off[i], overlap_off[i + 1]) (an empty range for every other
+ *    read);
+ *  - kmer_bits: per valid read i the words [kmer_off[i], kmer_off[i + 1]) (n_valid + 1
+ *    offsets), bit b of the read at word b >> 5, bit b & 31: Pile::kmers_[b], of
+ *    (len >> 4) + 1 bits;
+ *  - kmer_touched[i] = 1 iff some batch reported a filtered position of read i, i.e. iff
+ *    the reference resized kmers_ (pile.cc:67-72; it may stay all zero);
+ *  - n_mapped: the overlaps the map produced, before the clip and the identity filter. */
+int rvn_stage2_results(rvn_ctx* ctx, const rvn_overlap** overlaps, const uint64_t** overlap_off,
+                       const uint32_t** kmer_bits, const uint64_t** kmer_off,
+                       const uint8_t** kmer_touched, uint64_t* n_mapped);
 
 /* The estimates behind option "stage1_window" -1 (auto) for a stage-1 call over the
  * uploaded reads with these arguments (0 = the defaults, as in
@@ -438,7 +479,10 @@ int rvn_get_stats(rvn_ctx* ctx, rvn_stats* out);
  * upload); "index_chunk_budget" (bytes: replaces the free device memory in that auto
  * decision, 0 = the free memory); "map_flush_bases" (rvn_map cuts its range into flushes of
  * >= N query bases; 0 = the default, from the device memory; for tests of the flush
- * path, results do not depend on it); "poa_wide" and "poa_scratch_budget" (rvn_poa_batch and
+ * path, results do not depend on it); "stage2_batch_bases" (rvn_find_overlaps_and_repetitive_
+ * regions cuts its index batches at >= N bases instead of the reference's 1U << 30; 0 = the
+ * reference's cut; for tests of the multi-batch path: it changes what the reference's
+ * schedule would compute at that cut); "poa_wide" and "poa_scratch_budget" (rvn_poa_batch and
  * rvn_polish_windows); "poa_batch_bytes" (rvn_polish_windows: the device inputs of one window
  * batch, 0 = the default, from the free device memory; results do not depend on it);
  * "radix_portion_tiles" (a radix sort or partition over more than about 2^30 records

@@ -26,6 +26,7 @@
 #include "raven/graph/overlap_utils.h"
 #include "raven/pile.h"
 #include "raven_b200.h"
+#include "raven_b200/overlap_clip.hpp"
 #include "thread_pool/thread_pool.hpp"
 
 namespace raven_b200 {
@@ -169,24 +170,6 @@ inline void TrimAndAnnotatePiles(
 
 namespace detail {
 
-// Largest edit distance the identity filter still keeps for substrings whose
-// longer one has `longest` bases: the reference drops an overlap iff
-// 1. - double(ed) / longest < identity (construct.cc:195-204). Both operations
-// are monotone in ed, so the decision is "ed <= bound" - computed here with the
-// SAME double arithmetic, which makes a bounded distance search exact.
-inline std::int32_t IdentityBound(double identity, std::size_t longest) {
-  if (longest == 0) return -1;
-  auto keeps = [&](std::int64_t ed) {
-    const double score = 1. - static_cast<double>(ed) / longest;
-    return !(score < identity);
-  };
-  std::int64_t e = static_cast<std::int64_t>((1. - identity) * static_cast<double>(longest)) + 2;
-  e = std::min<std::int64_t>(std::max<std::int64_t>(e, 0), static_cast<std::int64_t>(longest));
-  while (e >= 0 && !keeps(e)) --e;
-  while (e >= 0 && e < static_cast<std::int64_t>(longest) && keeps(e + 1)) ++e;
-  return static_cast<std::int32_t>(e);  // -1: nothing passes
-}
-
 // keep[i] = 1 iff overlap i passes the identity filter; the reads are addressed
 // through index_of(id) = position in the set uploaded to the engine
 template <typename IndexOf>
@@ -208,7 +191,7 @@ std::vector<char> IdentityFilter(ram::MinimizerEngine& engine,
     rb[i] = o.rhs_begin;
     rl[i] = o.rhs_end - o.rhs_begin;
     st[i] = o.strand ? 1 : 0;
-    limit[i] = IdentityBound(identity, std::max(ll[i], rl[i]));
+    limit[i] = rvn::IdentityBound(identity, std::max(ll[i], rl[i]));
     if (limit[i] < 0) limit[i] = 0;  // (decided below; the search stays bounded)
   }
   std::lock_guard<std::mutex> lock(engine.mutex());
@@ -270,19 +253,41 @@ inline void ResolveContainedReads(
   raven::ResolveContainedReads(piles, overlaps, sequences, thread_pool, 0);
 }
 
+namespace detail {
+
+// Pile::AddKmers' result moved into a pile through the same door as PileDoor: kmers_
+// takes the device's bits, resized as the reference resizes it (pile.cc:67-72), so a
+// touched pile whose k-mers all fail the complexity test keeps an all-zero kmers_.
+struct KmerDoor {
+  const std::uint32_t* bits;
+  template <typename... Ts>
+  void operator()(std::uint32_t&, std::uint32_t&, std::uint32_t&, std::uint16_t&, bool&, bool&,
+                  bool&, bool&, std::vector<std::uint16_t>& data, std::vector<bool>& kmers,
+                  Ts&...) {
+    if (kmers.empty()) kmers.resize(data.size() + 1, false);
+    for (std::size_t b = 0; b < data.size() + 1; ++b) {
+      if (bits[b >> 5] >> (b & 31) & 1u) kmers[b] = true;
+    }
+  }
+};
+
+}  // namespace detail
+
 // raven::FindOverlapsAndRepetetiveRegions (RavenLib/src/construct.cc:316-491)
-// with the reference's exact signature: per batch of >= 1 GiB of valid reads ONE
-// device call maps every read so far (full sketches, filtered positions kept),
-// Pile::AddKmers takes the filtered positions, the identity filter is one batched
-// edit-distance call, the classification loop (OverlapUpdate / GetOverlapType /
-// longest per pair, :430-455) is the reference's, on the host.
+// with the reference's exact signature: the map of every batch, Pile::AddKmers and the
+// identity filter are ONE device call (rvn_find_overlaps_and_repetitive_regions) over
+// the valid reads; the k-mer marks move into the piles, and the classification loop
+// (OverlapUpdate / GetOverlapType / longest per pair, :430-455) is the reference's, on
+// the host. The k-mers are the engine's k long: the reference's only caller passes that
+// k as kmer_len (construct.cc:661-688).
 inline void FindOverlapsAndRepetetiveRegions(
     const std::shared_ptr<thread_pool::ThreadPool>& /*thread_pool*/,
-    ram::MinimizerEngine& engine, double freq, std::uint8_t kmer_len, double identity,
+    ram::MinimizerEngine& engine, double freq, std::uint8_t /*kmer_len*/, double identity,
     const std::vector<std::unique_ptr<raven::Pile>>& piles,
     std::vector<std::vector<biosoup::Overlap>>& overlaps,
     std::vector<std::unique_ptr<biosoup::NucleicAcid>>& sequences) {
   biosoup::Timer timer;
+  timer.Start();
   std::sort(sequences.begin(), sequences.end(),
             [&](const std::unique_ptr<biosoup::NucleicAcid>& lhs,
                 const std::unique_ptr<biosoup::NucleicAcid>& rhs) -> bool {
@@ -290,12 +295,6 @@ inline void FindOverlapsAndRepetetiveRegions(
                      (piles[lhs->id]->is_invalid() == piles[rhs->id]->is_invalid() &&
                       lhs->id < rhs->id);
             });
-  // id -> position in the sorted vector (= position in the uploaded set)
-  std::uint32_t max_id = 0;
-  for (const auto& it : sequences) max_id = std::max(max_id, it->id);
-  std::vector<std::uint32_t> sequences_map(static_cast<std::size_t>(max_id) + 1, 0);
-  for (std::uint32_t i = 0; i < sequences.size(); ++i) sequences_map[sequences[i]->id] = i;
-
   std::uint32_t s = 0;  // (stays 0 when no read is invalid: construct.cc:343-349)
   for (std::uint32_t i = 0; i < sequences.size(); ++i) {
     if (piles[sequences[i]->id]->is_invalid()) {
@@ -303,57 +302,44 @@ inline void FindOverlapsAndRepetetiveRegions(
       break;
     }
   }
-
   overlaps.resize(sequences.size() + 1);
-  if (s > 0) engine.Upload(sequences.begin(), sequences.begin() + s);
-  rvn_ctx* ctx = engine.context();
-  auto check = [&](int rc) {
-    if (rc == RVN_ERR_INVALID) throw std::invalid_argument(rvn_last_error(ctx));
-    if (rc != RVN_OK) throw std::runtime_error(rvn_last_error(ctx));
-  };
-  std::size_t bytes = 0;
-  for (std::uint32_t i = 0, j = 0; i < s; ++i) {
-    bytes += sequences[i]->inflated_len;
-    if (i != s - 1 && bytes < (1U << 30)) continue;
-    bytes = 0;
-    timer.Start();
-    std::vector<biosoup::Overlap> mapped;  // all Map results of the batch, query order
+  if (s > 0) {
+    engine.Upload(sequences.begin(), sequences.begin() + s);
+    std::vector<std::uint32_t> begin(s), end(s);
+    for (std::uint32_t i = 0; i < s; ++i) {
+      begin[i] = piles[sequences[i]->id]->begin();
+      end[i] = piles[sequences[i]->id]->end();
+    }
+    std::vector<biosoup::Overlap> mapped;  // final results of all batches, in loop order
     {
       std::lock_guard<std::mutex> lock(engine.mutex());
-      check(rvn_minimize(ctx, j, i + 1, 0));
-      std::uint32_t occ = 0;
-      check(rvn_filter(ctx, freq, &occ));
-      check(rvn_map(ctx, 0, i + 1, 1, 1, 0, 1));
+      rvn_ctx* ctx = engine.context();
+      auto check = [&](int rc) {
+        if (rc == RVN_ERR_INVALID) throw std::invalid_argument(rvn_last_error(ctx));
+        if (rc != RVN_OK) throw std::runtime_error(rvn_last_error(ctx));
+      };
+      check(rvn_find_overlaps_and_repetitive_regions(ctx, freq, identity, s, begin.data(),
+                                                     end.data()));
       const rvn_overlap* o = nullptr;
-      const std::uint64_t *off = nullptr, *foff = nullptr;
-      const std::uint32_t* f = nullptr;
-      std::uint64_t n = 0;
-      check(rvn_map_results(ctx, &o, &off, &n, &f, &foff));
-      mapped.reserve(n);
-      for (std::uint32_t k = 0; k < i + 1; ++k) {
-        const std::vector<std::uint32_t> filtered(f + foff[k], f + foff[k + 1]);
-        piles[sequences[k]->id]->AddKmers(filtered, kmer_len, sequences[k]);  // :382-383
-        for (std::uint64_t e = off[k]; e < off[k + 1]; ++e) {
-          mapped.emplace_back(o[e].lhs_id, o[e].lhs_begin, o[e].lhs_end, o[e].rhs_id,
-                              o[e].rhs_begin, o[e].rhs_end, o[e].score, o[e].strand != 0);
-        }
+      const std::uint64_t *ooff = nullptr, *koff = nullptr;
+      const std::uint32_t* bits = nullptr;
+      const std::uint8_t* touched = nullptr;
+      std::uint64_t n_mapped = 0;
+      check(rvn_stage2_results(ctx, &o, &ooff, &bits, &koff, &touched, &n_mapped));
+      for (std::uint32_t i = 0; i < s; ++i) {  // :382-383
+        if (!touched[i]) continue;
+        detail::KmerDoor door{bits + koff[i]};
+        auto visit = cereal::fields(door);
+        cereal::access::member_serialize(visit, *piles[sequences[i]->id]);
+      }
+      mapped.reserve(ooff[s]);
+      for (std::uint64_t e = 0; e < ooff[s]; ++e) {
+        mapped.emplace_back(o[e].lhs_id, o[e].lhs_begin, o[e].lhs_end, o[e].rhs_id,
+                            o[e].rhs_begin, o[e].rhs_end, o[e].score, o[e].strand != 0);
       }
     }
-    if (identity != 0) {  // :385-424, batched
-      std::vector<biosoup::Overlap> upd;
-      for (auto& o : mapped) {
-        if (raven::OverlapUpdate(o, piles)) upd.emplace_back(o);
-      }
-      const auto keep = detail::IdentityFilter(
-          engine, upd, identity, [&](std::uint32_t id) { return sequences_map[id]; });
-      mapped.clear();
-      for (std::size_t x = 0; x < upd.size(); ++x) {
-        if (keep[x]) mapped.emplace_back(upd[x]);
-      }
-    }
-    std::cerr << "[raven::Graph::Construct] minimized + mapped valid sequences (GPU) " << j
-              << " - " << i + 1 << " / " << s << " " << std::fixed << timer.Stop() << "s"
-              << std::endl;
+    std::cerr << "[raven::Graph::Construct] minimized + mapped valid sequences (GPU) " << s
+              << " " << std::fixed << timer.Stop() << "s" << std::endl;
     for (auto& jt : mapped) {  // :430-455
       if (!raven::OverlapUpdate(jt, piles)) continue;
       const std::uint32_t type = raven::GetOverlapType(jt, piles);
@@ -374,7 +360,6 @@ inline void FindOverlapsAndRepetetiveRegions(
         }
       }
     }
-    j = i + 1;
   }
 
   for (const auto& pile : piles) {  // :465-469

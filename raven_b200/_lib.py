@@ -67,6 +67,11 @@ SIGNATURES = {
     "rvn_find_overlaps_and_create_piles": (
         C.c_int, [C.c_void_p, C.c_double, C.c_uint64, C.c_int, C.c_uint64,
                   C.c_uint64]),
+    "rvn_find_overlaps_and_repetitive_regions": (
+        C.c_int, [C.c_void_p, C.c_double, C.c_double, C.c_uint32, U32P, U32P]),
+    "rvn_stage2_results": (C.c_int, [C.c_void_p, C.POINTER(OVLP), C.POINTER(U64P),
+                                     C.POINTER(U32P), C.POINTER(U64P),
+                                     C.POINTER(C.POINTER(C.c_uint8)), U64P]),
     "rvn_stage1_footprint": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64,
                                        U64P, U64P, U64P]),
     "rvn_index_footprint": (C.c_int, [C.c_void_p, C.c_uint64, U64P, U64P]),

@@ -4,6 +4,7 @@
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <memory>
 
 #include <unistd.h>
@@ -258,13 +259,25 @@ uint64_t MapFlushBases(const Ctx& c, uint64_t range_bases, bool join) {
 // rvn_map: MapRange flush by flush, each flush's overlaps, offsets and filtered positions
 // appended to the pinned host results, so that they read as one MapRange over the range.
 // One flush (and keep_hits, whose hits are those of one piece) is exactly that MapRange.
+// each (stage 2): called with (first read, reads) after every flush, whose results it
+// takes from the device (c.m_ovl, c.m_ovl_off, c.r_n_ovl, c.m_filtered); nothing is
+// gathered on the host.
 void MapFlushes(Ctx& c, uint32_t first, uint32_t last, bool avoid_equal, bool avoid_symmetric,
-                bool minhash, bool want_filtered) {
+                bool minhash, bool want_filtered,
+                const std::function<void(uint32_t, uint32_t)>& each = nullptr) {
   uint64_t bases = 0;
   for (uint32_t r = first; r < last; ++r) bases += c.h_len[r];
   const bool join = c.self_join && minhash && avoid_equal && avoid_symmetric && !want_filtered &&
                     first >= c.i_first && last <= c.i_last;
   const std::vector<uint32_t> cuts = ChunkCuts(c, first, last, MapFlushBases(c, bases, join));
+  if (each) {
+    for (size_t i = 0; i + 1 < cuts.size(); ++i) {
+      MapRange(c, cuts[i], cuts[i + 1], avoid_equal, avoid_symmetric, minhash, want_filtered,
+               /*fetch=*/false);
+      each(cuts[i], cuts[i + 1] - cuts[i]);
+    }
+    return;
+  }
   if (c.keep_hits || cuts.size() <= 2) {
     MapRange(c, first, last, avoid_equal, avoid_symmetric, minhash, want_filtered);
     return;
@@ -306,6 +319,110 @@ void MapFlushes(Ctx& c, uint32_t first, uint32_t last, bool avoid_equal, bool av
   c.m_first_read = first;
   c.m_last_read = last;
   c.r_valid = true;
+}
+
+// raven::FindOverlapsAndRepetetiveRegions' device work (construct.cc:352-424) over the
+// first n valid reads of the uploaded set, in the reference's sorted order: index
+// batches [j, i + 1) cut by the reference's rule (bytes < 1U << 30; option
+// "stage2_batch_bases" forces a smaller batch), each an untiered full-sketch index
+// filtered at freq, then every read of [0, i + 1) mapped with (avoid equal, avoid
+// symmetric, no minhash, filtered positions) in rvn_map's flushes. Per flush, on the
+// device: the filtered positions mark the k-mer bitmaps (Pile::AddKmers), and with
+// identity != 0 the overlaps are clipped to the valid regions (rbeg, rend: Pile::begin()
+// and end() per valid read) and filtered by edit distance. Only the final overlaps, and
+// at the end the bitmaps and touched flags, go to the pinned host results.
+void Stage2(Ctx& c, double freq, double identity, uint32_t n, const uint32_t* h_rbeg,
+            const uint32_t* h_rend) {
+  if (n > c.n_reads) throw InvalidArgument("more valid reads than uploaded reads");
+  if (n && (!h_rbeg || !h_rend)) throw InvalidArgument("null regions");
+  if (n && (c.res_first > 0 || c.res_last < n)) {
+    throw StateError("the bases of the valid reads were not uploaded");
+  }
+  c.s2_valid = false;
+  uint32_t max_id = 0;
+  for (uint32_t i = 0; i < n; ++i) {
+    if (h_rbeg[i] > h_rend[i] || h_rend[i] > c.h_len[i]) {
+      throw InvalidArgument("region outside its read");
+    }
+    max_id = std::max(max_id, c.h_ids[i]);
+  }
+  // read id -> position in the uploaded set (construct.cc:331-337's sequences_map)
+  std::vector<uint32_t> pos_of(max_id + 1ULL, 0);
+  for (uint32_t i = 0; i < n; ++i) pos_of[c.h_ids[i]] = i;
+  uint64_t* boff = c.s2_bit_off_h.reserve(n + 1ULL);
+  boff[0] = 0;
+  for (uint32_t i = 0; i < n; ++i) boff[i + 1] = boff[i] + ((c.h_len[i] >> 4) + 1 + 31) / 32;
+  uint32_t* d_pos_of = c.s2_pos_of.reserve(pos_of.size());
+  uint32_t* d_rbeg = c.s2_rbeg.reserve(n + 1ULL);
+  uint32_t* d_rend = c.s2_rend.reserve(n + 1ULL);
+  uint64_t* d_boff = c.s2_bit_off.reserve(n + 1ULL);
+  uint32_t* d_bits = c.s2_bits.reserve(boff[n] + 1);
+  uint8_t* d_touched = c.s2_touched.reserve(n + 1ULL);
+  RVN_CUDA(cudaMemcpyAsync(d_pos_of, pos_of.data(), pos_of.size() * 4, cudaMemcpyHostToDevice,
+                           c.stream));
+  if (n) {
+    RVN_CUDA(cudaMemcpyAsync(d_rbeg, h_rbeg, n * 4ULL, cudaMemcpyHostToDevice, c.stream));
+    RVN_CUDA(cudaMemcpyAsync(d_rend, h_rend, n * 4ULL, cudaMemcpyHostToDevice, c.stream));
+  }
+  RVN_CUDA(cudaMemcpyAsync(d_boff, boff, (n + 1ULL) * 8, cudaMemcpyHostToDevice, c.stream));
+  RVN_CUDA(cudaMemsetAsync(d_bits, 0, (boff[n] + 1) * 4, c.stream));
+  RVN_CUDA(cudaMemsetAsync(d_touched, 0, n + 1ULL, c.stream));
+
+  uint64_t* ooff = c.s2_ovl_off.reserve(n + 1ULL);
+  ooff[0] = 0;
+  c.s2_ovl.reserve_keep(1, 0);
+  uint64_t total = 0, mapped = 0;
+  auto flush = [&](uint32_t r0, uint32_t m) {
+    Stage2KmerMarks(c, r0, m, c.prm.k);
+    const uint64_t nm = c.r_n_ovl;
+    mapped += nm;
+    const rvn_overlap* src = c.m_ovl.get();
+    uint64_t kept = nm;
+    if (identity != 0) {  // with identity 0 the overlaps pass unchanged (construct.cc:385)
+      rvn_overlap* dst = c.s2_kept.reserve(nm + 1);
+      uint64_t* dst_off = c.s2_kept_off.reserve(m + 1ULL);
+      kept = Stage2ClipFilter(c, c.m_ovl.get(), c.m_ovl_off.get(), m, nm, identity, dst, dst_off);
+      src = dst;
+    }
+    rvn_overlap* o = c.s2_ovl.reserve_keep(total + kept + 1, total);
+    RVN_CUDA(cudaMemcpyAsync(o + total, src, kept * sizeof(rvn_overlap), cudaMemcpyDeviceToHost,
+                             c.stream));
+    RVN_CUDA(cudaStreamSynchronize(c.stream));
+    total += kept;
+  };
+  const uint64_t cut = c.stage2_batch_bases ? c.stage2_batch_bases : (1ULL << 30);
+  struct HostFiltered {  // the filtered positions stay on the device for the whole call
+    Ctx& c;
+    explicit HostFiltered(Ctx& x) : c(x) { c.m_filtered_host = false; }
+    ~HostFiltered() { c.m_filtered_host = true; }
+  } keep_on_device(c);
+  uint64_t bytes = 0;
+  for (uint32_t i = 0, j = 0; i < n; ++i) {
+    bytes += c.h_len[i];
+    ooff[i + 1] = total;
+    if (i != n - 1 && bytes < cut) continue;
+    bytes = 0;
+    // rvn_minimize(j, i + 1, 0) and rvn_filter(freq)
+    const uint64_t chunk = IndexChunk(c, MinimizeFootprint(c, j, i + 1, 0));
+    if (chunk) {
+      BuildIndexChunked(c, j, i + 1, false, chunk, 0, /*tiers=*/false);
+    } else {
+      BuildIndex(c, j, i + 1, false);
+    }
+    FilterIndex(c, freq);
+    if (chunk) ReleaseIndexBuild(c);
+    MapFlushes(c, 0, i + 1, true, true, false, true, flush);
+    ooff[i + 1] = total;
+    j = i + 1;
+  }
+  uint32_t* bits = c.s2_bits_h.reserve(boff[n] + 1);
+  uint8_t* touched = c.s2_touched_h.reserve(n + 1ULL);
+  RVN_CUDA(cudaMemcpyAsync(bits, d_bits, boff[n] * 4, cudaMemcpyDeviceToHost, c.stream));
+  RVN_CUDA(cudaMemcpyAsync(touched, d_touched, n, cudaMemcpyDeviceToHost, c.stream));
+  RVN_CUDA(cudaStreamSynchronize(c.stream));
+  c.s2_n_valid = n;
+  c.s2_mapped = mapped;
+  c.s2_valid = true;
 }
 
 // Option "stage1_window" -1 (auto): windowed only when the resident estimate exceeds
@@ -721,6 +838,9 @@ void SetOption(Ctx& c, const char* name, int64_t value) {
   } else if (name && std::strcmp(name, "map_flush_bases") == 0) {
     if (value < 0) throw InvalidArgument("map_flush_bases: bases, 0 = from the device memory");
     c.map_flush_bases = static_cast<uint64_t>(value);
+  } else if (name && std::strcmp(name, "stage2_batch_bases") == 0) {
+    if (value < 0) throw InvalidArgument("stage2_batch_bases: bases, 0 = the reference's 2^30");
+    c.stage2_batch_bases = static_cast<uint64_t>(value);
   } else if (name && std::strcmp(name, "poa_wide") == 0) {
     if (value < 0 || value > 2) throw InvalidArgument("poa_wide: 0, 1 or 2");
     c.poa_wide = value;
@@ -1205,6 +1325,31 @@ RVN_API int rvn_find_overlaps_and_create_piles(rvn_ctx* ctx, double frequency,
     Stage1(c, frequency, max_overlaps, minhash != 0, index_batch_bases,
            query_batch_bases);
   }, /*sketches_first=*/true);
+}
+
+RVN_API int rvn_find_overlaps_and_repetitive_regions(rvn_ctx* ctx, double frequency,
+                                                     double identity, uint32_t n_valid,
+                                                     const uint32_t* region_begin,
+                                                     const uint32_t* region_end) {
+  return Guard(ctx, [&](Ctx& c) {
+    Stage2(c, frequency, identity, n_valid, region_begin, region_end);
+    TimerCollect(c);
+  }, /*sketches_first=*/true);
+}
+
+RVN_API int rvn_stage2_results(rvn_ctx* ctx, const rvn_overlap** overlaps,
+                               const uint64_t** overlap_off, const uint32_t** kmer_bits,
+                               const uint64_t** kmer_off, const uint8_t** kmer_touched,
+                               uint64_t* n_mapped) {
+  return Guard(ctx, [&](Ctx& c) {
+    if (!c.s2_valid) throw StateError("no stage-2 results");
+    if (overlaps) *overlaps = c.s2_ovl.get();
+    if (overlap_off) *overlap_off = c.s2_ovl_off.get();
+    if (kmer_bits) *kmer_bits = c.s2_bits_h.get();
+    if (kmer_off) *kmer_off = c.s2_bit_off_h.get();
+    if (kmer_touched) *kmer_touched = c.s2_touched_h.get();
+    if (n_mapped) *n_mapped = c.s2_mapped;
+  });
 }
 
 RVN_API int rvn_stage1_footprint(rvn_ctx* ctx, uint64_t max_overlaps,

@@ -20,21 +20,13 @@
 #include <algorithm>
 #include <numeric>
 
+#include "../../include/raven_b200/overlap_clip.hpp"
 #include "engine.cuh"
 #include "myers.cuh"
 
 namespace rvn {
 
 namespace {
-
-struct PairDesc {
-  uint64_t q_word;   // first word of the lhs read in `words`
-  uint64_t t_word;   // first word of the rhs read
-  uint32_t q_begin, q_len;
-  uint32_t t_begin, t_len;
-  uint32_t strand;   // 1 = same strand; 0 = rhs substring reverse complemented
-  uint32_t slot;     // index of the pair in the caller's arrays
-};
 
 // match mask of query block b (rows 64b .. 64b+63 of the lhs substring)
 __device__ __forceinline__ uint64_t BlockEq(const uint64_t* __restrict__ qw, uint64_t q_words,
@@ -198,7 +190,91 @@ void LaunchTier(Ctx& c, const PairDesc* d_pairs, const uint32_t* d_list, uint32_
   ++c.launches;
 }
 
+// tier cost of every listed pair (lhs + rhs bases): the list runs longest first, so
+// the lanes of a warp carry similar work
+__global__ void PairCostKernel(const PairDesc* __restrict__ pairs, const uint32_t* __restrict__ list,
+                               uint32_t n, uint32_t* __restrict__ cost) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const PairDesc d = pairs[list[i]];
+  cost[i] = d.q_len + d.t_len;
+}
+
+// pairs of the list still open after a tier of band k: not found within the band and
+// allowed to look further; the longest lhs of them into *max_q_len
+__global__ void OpenPairsKernel(const PairDesc* __restrict__ pairs, const uint32_t* __restrict__ list,
+                                uint32_t n, int k, const int32_t* __restrict__ limit,
+                                const int32_t* __restrict__ out, uint32_t* __restrict__ flag,
+                                uint32_t* __restrict__ max_q_len) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const PairDesc d = pairs[list[i]];
+  const int lim = limit[d.slot];
+  const bool open = out[d.slot] < 0 && !(lim >= 0 && lim <= k);
+  flag[i] = open ? 1u : 0u;
+  if (open) atomicMax(max_q_len, d.q_len);
+}
+
+// dst[pos[i]] = src[i] where flag[i] (a stable compaction by an exclusive scan of flag)
+template <typename T>
+__global__ void CompactKernel(const T* __restrict__ src, const uint32_t* __restrict__ flag,
+                              const uint64_t* __restrict__ pos, uint64_t n, T* __restrict__ dst) {
+  const uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i < n && flag[i]) dst[pos[i]] = src[i];
+}
+
 }  // namespace
+
+void MyersTiers(Ctx& c, const PairDesc* d_pairs, uint32_t* d_list, uint32_t n,
+                const int32_t* d_limit, int32_t* d_out) {
+  if (n == 0) return;
+  uint32_t* key = c.e_key.reserve(n);
+  uint32_t* key2 = c.e_key2.reserve(n);
+  uint32_t* list2 = c.e_list2.reserve(n);
+  uint32_t* flag = c.e_flag.reserve(n + 1ULL);
+  uint64_t* pos = c.e_scan.reserve(n + 2ULL);
+  PairCostKernel<<<CeilDiv(n, 256), 256, 0, c.stream>>>(d_pairs, d_list, n, key);
+  RVN_LAUNCH_CHECK();
+  ++c.launches;
+  // (the sort's sources may alias its buffers b)
+  const int w = RadixSortPairs(c, key, key2, key, d_list, list2, d_list, n, 0, 32,
+                               /*descending=*/true);
+  uint32_t* list = w == 0 ? list2 : d_list;
+  uint32_t* spare = w == 0 ? d_list : list2;
+  static const int kTierK[4] = {64, 192, 448, 960};
+  uint32_t m = n, max_q_len = 0;
+  for (int tier = 0; tier <= 4 && m > 0; ++tier) {
+    if (tier == 0) LaunchTier<4, 128>(c, d_pairs, list, m, kTierK[0], d_limit, d_out);
+    if (tier == 1) LaunchTier<8, 128>(c, d_pairs, list, m, kTierK[1], d_limit, d_out);
+    if (tier == 2) LaunchTier<16, 64>(c, d_pairs, list, m, kTierK[2], d_limit, d_out);
+    if (tier == 3) LaunchTier<32, 64>(c, d_pairs, list, m, kTierK[3], d_limit, d_out);
+    if (tier == 4) {
+      // unbanded: scratch for the vectors of every query block of every pair in flight
+      const uint32_t max_blocks = std::max(1u, (max_q_len + 63) / 64);
+      const uint64_t threads = static_cast<uint64_t>(CeilDiv(m, 64)) * 64;
+      uint64_t* scratch = c.m_scratch64.reserve(2ULL * max_blocks * threads + 16);
+      FullMyersKernel<<<CeilDiv(m, 64), 64, 0, c.stream>>>(c.d_words.get(), d_pairs, list, m,
+                                                          max_blocks, scratch, d_out,
+                                                          c.n_words + 2);
+      RVN_LAUNCH_CHECK();
+      ++c.launches;
+      break;
+    }
+    RVN_CUDA(cudaMemsetAsync(flag + m, 0, sizeof(uint32_t), c.stream));  // (the max below)
+    OpenPairsKernel<<<CeilDiv(m, 256), 256, 0, c.stream>>>(d_pairs, list, m, kTierK[tier],
+                                                           d_limit, d_out, flag, flag + m);
+    ExclusiveScanU32(c, flag, pos, m);
+    CompactKernel<uint32_t><<<CeilDiv(m, 256), 256, 0, c.stream>>>(list, flag, pos, m, spare);
+    RVN_LAUNCH_CHECK();
+    c.launches += 2;
+    uint64_t open = 0;
+    RVN_CUDA(cudaMemcpyAsync(&max_q_len, flag + m, sizeof(uint32_t), cudaMemcpyDeviceToHost,
+                             c.stream));
+    open = ReadU64(c, pos + m);
+    std::swap(list, spare);
+    m = static_cast<uint32_t>(open);
+  }
+}
 
 // Global edit distances of n substring pairs of the uploaded reads. limit[i] >= 0:
 // distances above it are reported as -1 (the caller only needs "beyond").
@@ -223,63 +299,129 @@ void EditDistanceBatch(Ctx& c, uint64_t n, const uint32_t* lhs_read, const uint3
                     rhs_len[i], strand[i] ? 1u : 0u, static_cast<uint32_t>(i)};
   }
   TimerBegin(c, "edit_distance");
-  DevBuf<PairDesc> d_pairs;
-  DevBuf<uint32_t> d_list;
-  DevBuf<int32_t> d_out, d_limit;
-  d_pairs.reserve(n);
-  d_list.reserve(n);
-  d_out.reserve(n);
-  d_limit.reserve(n);
+  PairDesc* d_pairs = c.e_pairs.reserve(n);
+  uint32_t* d_list = c.e_list.reserve(n);
+  int32_t* d_out = c.e_dist.reserve(n);
+  int32_t* d_limit = c.e_limit.reserve(n);
   std::vector<int32_t> h_limit(n), h_out(n, -1);
-  for (uint64_t i = 0; i < n; ++i) h_limit[i] = limit ? limit[i] : -1;
-  RVN_CUDA(cudaMemcpyAsync(d_pairs.get(), h.data(), n * sizeof(PairDesc), cudaMemcpyHostToDevice,
-                           c.stream));
-  RVN_CUDA(cudaMemcpyAsync(d_limit.get(), h_limit.data(), n * 4, cudaMemcpyHostToDevice, c.stream));
-
-  // work list, longest pairs first (lanes of a warp then carry similar work)
-  std::vector<uint32_t> todo(n);
-  std::iota(todo.begin(), todo.end(), 0u);
-  auto cost = [&](uint32_t i) { return static_cast<uint64_t>(h[i].q_len) + h[i].t_len; };
-  std::sort(todo.begin(), todo.end(), [&](uint32_t a, uint32_t b) { return cost(a) > cost(b); });
-
-  static const int kTierK[4] = {64, 192, 448, 960};
-  for (int tier = 0; tier <= 4 && !todo.empty(); ++tier) {
-    const uint32_t m = static_cast<uint32_t>(todo.size());
-    RVN_CUDA(cudaMemcpyAsync(d_list.get(), todo.data(), m * 4ULL, cudaMemcpyHostToDevice, c.stream));
-    if (tier == 0) LaunchTier<4, 128>(c, d_pairs.get(), d_list.get(), m, kTierK[0], d_limit.get(), d_out.get());
-    if (tier == 1) LaunchTier<8, 128>(c, d_pairs.get(), d_list.get(), m, kTierK[1], d_limit.get(), d_out.get());
-    if (tier == 2) LaunchTier<16, 64>(c, d_pairs.get(), d_list.get(), m, kTierK[2], d_limit.get(), d_out.get());
-    if (tier == 3) LaunchTier<32, 64>(c, d_pairs.get(), d_list.get(), m, kTierK[3], d_limit.get(), d_out.get());
-    if (tier == 4) {
-      // unbanded: scratch for the vectors of every query block of every pair in flight
-      uint32_t max_blocks = 1;
-      for (uint32_t i : todo) max_blocks = std::max(max_blocks, (h[i].q_len + 63) / 64);
-      const uint64_t threads = static_cast<uint64_t>(CeilDiv(m, 64)) * 64;
-      uint64_t* scratch = c.m_scratch64.reserve(2ULL * max_blocks * threads + 16);
-      FullMyersKernel<<<CeilDiv(m, 64), 64, 0, c.stream>>>(c.d_words.get(), d_pairs.get(),
-                                                          d_list.get(), m, max_blocks, scratch,
-                                                          d_out.get(), c.n_words + 2);
-      RVN_LAUNCH_CHECK();
-      ++c.launches;
-    }
-    RVN_CUDA(cudaMemcpyAsync(h_out.data(), d_out.get(), n * 4, cudaMemcpyDeviceToHost, c.stream));
-    RVN_CUDA(cudaStreamSynchronize(c.stream));
-    // pairs still open: not found within this tier's band and allowed to look further
-    std::vector<uint32_t> next;
-    for (uint32_t i : todo) {
-      if (h_out[i] >= 0 || tier == 4) continue;
-      const int lim = h_limit[i];
-      if (lim >= 0 && lim <= kTierK[tier]) continue;  // beyond the caller's bound: stays -1
-      next.push_back(i);
-    }
-    todo.swap(next);
+  std::vector<uint32_t> h_list(n);
+  for (uint64_t i = 0; i < n; ++i) {
+    h_limit[i] = limit ? limit[i] : -1;
+    h_list[i] = static_cast<uint32_t>(i);
   }
+  RVN_CUDA(cudaMemcpyAsync(d_pairs, h.data(), n * sizeof(PairDesc), cudaMemcpyHostToDevice,
+                           c.stream));
+  RVN_CUDA(cudaMemcpyAsync(d_limit, h_limit.data(), n * 4, cudaMemcpyHostToDevice, c.stream));
+  RVN_CUDA(cudaMemcpyAsync(d_list, h_list.data(), n * 4, cudaMemcpyHostToDevice, c.stream));
+  RVN_CUDA(cudaMemsetAsync(d_out, 0xFF, n * 4, c.stream));
+  MyersTiers(c, d_pairs, d_list, static_cast<uint32_t>(n), d_limit, d_out);
+  RVN_CUDA(cudaMemcpyAsync(h_out.data(), d_out, n * 4, cudaMemcpyDeviceToHost, c.stream));
+  RVN_CUDA(cudaStreamSynchronize(c.stream));
   TimerEnd(c);
   for (uint64_t i = 0; i < n; ++i) {
     int32_t v = h_out[i];
     if (limit && limit[i] >= 0 && v > limit[i]) v = -1;
     out[i] = v;
   }
+}
+
+// ---------------------------------------------------------------------------
+// Stage 2's clip and identity filter on the device (construct.cc:385-424): the map's
+// overlaps of a flush never leave the device before they are final.
+// ---------------------------------------------------------------------------
+namespace {
+
+// one thread per overlap: OverlapUpdate against the valid regions (reads by their
+// position in the uploaded set, pos_of[id]), and the edit-distance pair of a clipped one
+__global__ void ClipKernel(const rvn_overlap* __restrict__ ovl, uint64_t n,
+                           const uint32_t* __restrict__ pos_of, const uint32_t* __restrict__ rbeg,
+                           const uint32_t* __restrict__ rend, const uint64_t* __restrict__ woff,
+                           double identity, rvn_overlap* __restrict__ clipped,
+                           PairDesc* __restrict__ pairs, int32_t* __restrict__ limit,
+                           int32_t* __restrict__ dist, uint32_t* __restrict__ flag) {
+  const uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  rvn_overlap o = ovl[i];
+  const uint32_t lp = pos_of[o.lhs_id], rp = pos_of[o.rhs_id];
+  const bool ok = OverlapClip(o.lhs_begin, o.lhs_end, o.rhs_begin, o.rhs_end, o.strand != 0,
+                              PileRegion{rbeg[lp], rend[lp], false},
+                              PileRegion{rbeg[rp], rend[rp], false});
+  clipped[i] = o;
+  flag[i] = ok ? 1u : 0u;
+  dist[i] = -1;
+  if (!ok) return;
+  const uint32_t ll = o.lhs_end - o.lhs_begin, rl = o.rhs_end - o.rhs_begin;
+  pairs[i] = PairDesc{woff[lp], woff[rp], o.lhs_begin, ll, o.rhs_begin, rl,
+                      o.strand ? 1u : 0u, static_cast<uint32_t>(i)};
+  const int32_t b = IdentityBound(identity, ll > rl ? ll : rl);
+  limit[i] = b < 0 ? 0 : b;  // (decided below; the search stays bounded)
+}
+
+// keep = clipped and 1 - ed / max(len) >= identity (construct.cc:407-413)
+__global__ void KeepKernel(const rvn_overlap* __restrict__ clipped, uint64_t n,
+                           const int32_t* __restrict__ dist, double identity,
+                           uint32_t* __restrict__ flag) {
+  const uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n || !flag[i]) return;
+  const rvn_overlap o = clipped[i];
+  const uint32_t ll = o.lhs_end - o.lhs_begin, rl = o.rhs_end - o.rhs_begin;
+  const int32_t d = dist[i];
+  const double score = 1. - static_cast<double>(d) / static_cast<double>(ll > rl ? ll : rl);
+  flag[i] = (d >= 0 && !(score < identity)) ? 1u : 0u;
+}
+
+__global__ void IotaListKernel(const uint32_t* __restrict__ flag, const uint64_t* __restrict__ pos,
+                               uint64_t n, uint32_t* __restrict__ list) {
+  const uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i < n && flag[i]) list[pos[i]] = static_cast<uint32_t>(i);
+}
+
+// per read of the flush: the first kept overlap (the scan at its first overlap)
+__global__ void KeptOffsetsKernel(const uint64_t* __restrict__ pos, const uint64_t* __restrict__ off,
+                                  uint32_t nr, uint64_t* __restrict__ out_off) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r <= nr) out_off[r] = pos[off[r]];
+}
+
+}  // namespace
+
+uint64_t Stage2ClipFilter(Ctx& c, const rvn_overlap* d_ovl, const uint64_t* d_off, uint32_t nr,
+                          uint64_t n, double identity, rvn_overlap* d_out, uint64_t* d_out_off) {
+  if (n >= 0xFFFFFFFFULL) throw LimitError("2^32 or more overlaps in one flush");
+  TimerBegin(c, "stage2_filter");
+  rvn_overlap* clipped = c.e_ovl.reserve(n + 1);
+  PairDesc* pairs = c.e_pairs.reserve(n + 1);
+  int32_t* limit = c.e_limit.reserve(n + 1);
+  int32_t* dist = c.e_dist.reserve(n + 1);
+  uint32_t* flag = c.e_sflag.reserve(n + 1);
+  uint32_t* list = c.e_list.reserve(n + 1);
+  uint64_t* pos = c.e_sscan.reserve(n + 2);
+  uint64_t kept = 0;
+  if (n > 0) {
+    const uint32_t blocks = CeilDiv(n, 256);
+    ClipKernel<<<blocks, 256, 0, c.stream>>>(d_ovl, n, c.s2_pos_of.get(), c.s2_rbeg.get(),
+                                             c.s2_rend.get(), c.d_woff.get(), identity, clipped,
+                                             pairs, limit, dist, flag);
+    ExclusiveScanU32(c, flag, pos, n);
+    IotaListKernel<<<blocks, 256, 0, c.stream>>>(flag, pos, n, list);
+    RVN_LAUNCH_CHECK();
+    c.launches += 2;
+    const uint64_t m = ReadU64(c, pos + n);
+    MyersTiers(c, pairs, list, static_cast<uint32_t>(m), limit, dist);
+    KeepKernel<<<blocks, 256, 0, c.stream>>>(clipped, n, dist, identity, flag);
+    ExclusiveScanU32(c, flag, pos, n);
+    CompactKernel<rvn_overlap><<<blocks, 256, 0, c.stream>>>(clipped, flag, pos, n, d_out);
+    RVN_LAUNCH_CHECK();
+    c.launches += 3;
+  } else {
+    RVN_CUDA(cudaMemsetAsync(pos, 0, sizeof(uint64_t), c.stream));
+  }
+  KeptOffsetsKernel<<<CeilDiv(nr + 1ULL, 256), 256, 0, c.stream>>>(pos, d_off, nr, d_out_off);
+  RVN_LAUNCH_CHECK();
+  ++c.launches;
+  kept = n > 0 ? ReadU64(c, pos + n) : 0;
+  TimerEnd(c);
+  return kept;
 }
 
 }  // namespace rvn

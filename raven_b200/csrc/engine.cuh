@@ -43,6 +43,16 @@ struct Window {
   }
 };
 
+// one substring pair of the edit-distance tiers (editdist.cu)
+struct PairDesc {
+  uint64_t q_word;   // first word of the lhs read in `words`
+  uint64_t t_word;   // first word of the rhs read
+  uint32_t q_begin, q_len;
+  uint32_t t_begin, t_len;
+  uint32_t strand;   // 1 = same strand; 0 = rhs substring reverse complemented
+  uint32_t slot;     // index of the pair in the caller's arrays
+};
+
 struct PhaseTimer {
   std::vector<const char*> names;
   std::vector<float> ms;
@@ -184,6 +194,9 @@ struct Ctx {
   DevBuf<uint64_t> m_ovl_off;
   DevBuf<uint64_t> m_counter;
   DevBuf<uint32_t> m_filtered;
+  DevBuf<uint64_t> m_filtered_off;  // per query read (+1): its slice of m_filtered
+  uint64_t m_n_filtered = 0;
+  bool m_filtered_host = true;  // FilteredPositions also copies them to r_filtered
   DevBuf<uint64_t> m_filt_off;
   DevBuf<uint64_t> scan_tmp;
   uint64_t m_hits = 0;
@@ -239,6 +252,9 @@ struct Ctx {
   // option "map_flush_bases": rvn_map works its query range in flushes of >= N bases;
   // 0 (default) = from the usable device memory, at most the reference's 2^30
   uint64_t map_flush_bases = 0;
+  // option "stage2_batch_bases": rvn_find_overlaps_and_repetitive_regions cuts its index
+  // batches at >= N bases; 0 (default) = the reference's 2^30
+  uint64_t stage2_batch_bases = 0;
   PinBuf<rvn_overlap> w_rows;  // kmax records per read
   PinBuf<uint32_t> w_cnt;      // kept records per read
   DevBuf<uint64_t> w_pile_off, w_row_off;  // per slot (+1) of the current window
@@ -285,6 +301,28 @@ struct Ctx {
   int64_t stage1_stream = 1;
   cudaStream_t d2h_stream = nullptr;
   cudaEvent_t d2h_ready = nullptr, d2h_done = nullptr;
+
+  // ---- stage 2 (capi.cu Stage2): per valid read its pile region, the k-mer marks (one
+  // bit per pile bin and one past the end, bins + 1 bits in whole u32 words) and the
+  // touched flag, resident for the whole call; the kept overlaps of every batch ----
+  DevBuf<uint32_t> s2_pos_of, s2_rbeg, s2_rend, s2_bits;
+  DevBuf<uint64_t> s2_bit_off;
+  DevBuf<uint8_t> s2_touched;
+  DevBuf<rvn_overlap> s2_kept;
+  DevBuf<uint64_t> s2_kept_off;
+  PinBuf<rvn_overlap> s2_ovl;
+  PinBuf<uint64_t> s2_ovl_off, s2_bit_off_h;
+  PinBuf<uint32_t> s2_bits_h;
+  PinBuf<uint8_t> s2_touched_h;
+  // edit-distance tiers and the clip/filter of one flush (editdist.cu)
+  DevBuf<PairDesc> e_pairs;
+  DevBuf<uint32_t> e_list, e_list2, e_key, e_key2, e_flag, e_sflag;
+  DevBuf<int32_t> e_limit, e_dist;
+  DevBuf<uint64_t> e_scan, e_sscan;
+  DevBuf<rvn_overlap> e_ovl;
+  uint32_t s2_n_valid = 0;
+  uint64_t s2_mapped = 0;
+  bool s2_valid = false;
 
   // ---- read ownership of the stage-1 tail: read r is owned iff r % own_mod ==
   // own_rem (1 / 0 = every read: the single-GPU path) ----
@@ -488,7 +526,28 @@ void EditDistanceBatch(Ctx& c, uint64_t n, const uint32_t* lhs_read, const uint3
                        const uint32_t* rhs_begin, const uint32_t* rhs_len,
                        const uint8_t* strand, const int32_t* limit, int32_t* out);
 
+// The device half of the edit-distance tiers: distances of the n pairs listed in d_list
+// (indices into d_pairs, in any order; the list is reordered), out[slot] per pair: the
+// distance, or -1 when it exceeds the pair's limit (limit[slot] >= 0) - above the limit a
+// distance may also come back exact. max_q_len: the longest lhs substring of the pairs.
+void MyersTiers(Ctx& c, const PairDesc* d_pairs, uint32_t* d_list, uint32_t n,
+                const int32_t* d_limit, int32_t* d_out);
+
+// Stage 2's clip and identity filter (construct.cc:385-424) of the flush's n overlaps,
+// grouped by query read (d_off, nr + 1 entries): OverlapClip against the pile regions of
+// c.s2_rbeg / c.s2_rend, the edit distance of each clipped overlap that keeps one, and the
+// kept clipped overlaps compacted stably into d_out with per-read offsets d_out_off.
+// Returns how many were kept.
+uint64_t Stage2ClipFilter(Ctx& c, const rvn_overlap* d_ovl, const uint64_t* d_off, uint32_t nr,
+                          uint64_t n, double identity, rvn_overlap* d_out, uint64_t* d_out_off);
+
 // ---- pile.cu ----
+// Pile::AddKmers (pile.cc:64-120) for the filtered positions the last MapRange left on
+// the device (c.m_filtered, c.m_filtered_off) of query reads [first, first + nr): marks
+// bit pos >> 4 of the read's bitmap in c.s2_bits when the k-mer passes the complexity
+// test, and sets the touched flag of every read with a filtered position.
+void Stage2KmerMarks(Ctx& c, uint32_t first, uint32_t nr, uint32_t k);
+
 // data: device u16 bins of the piles of window `w` in slot order, off: their device
 // u64 offsets (w.size() + 1), `bins` of them in all. No overlap may name a pile of a
 // slot below `first`: the coverage pass skips those piles, and neither reads nor

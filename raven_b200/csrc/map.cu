@@ -1108,11 +1108,13 @@ void FilteredPositions(Ctx& c, const uint8_t* filt, const uint64_t* qo, uint64_t
   RVN_LAUNCH_CHECK();
   c.launches += 2;
   // per-read offsets of the filtered list
-  uint64_t* froff = c.m_ovl_off.reserve(nr + 2ULL);
+  uint64_t* froff = c.m_filtered_off.reserve(nr + 2ULL);
   GatherU64<<<CeilDiv(nr + 1ULL, kThreads), kThreads, 0, c.stream>>>(
       fpos, read_off, q_begin, nr + 1ULL, froff);
   RVN_LAUNCH_CHECK();
   ++c.launches;
+  c.m_n_filtered = n_filtered;
+  if (!c.m_filtered_host) return;  // (stage 2 consumes them on the device)
   uint32_t* hf = c.r_filtered.reserve(n_filtered + 1);
   RVN_CUDA(cudaMemcpyAsync(hf, fout, n_filtered * sizeof(uint32_t),
                            cudaMemcpyDeviceToHost, c.stream));
@@ -1237,6 +1239,7 @@ HitCounts ProbeHits(Ctx& c, uint32_t first, uint32_t last, bool avoid_equal,
 
   c.r_filt_off.reserve(nr + 2ULL);
   for (uint32_t i = 0; i <= nr; ++i) c.r_filt_off.get()[i] = 0;
+  c.m_n_filtered = 0;
   if (want_filtered && n_q > 0) {
     FilteredPositions(c, filt, qo, q_begin, n_q, d_read_off + off_base_read, nr);
   }

@@ -149,18 +149,9 @@ __device__ uint32_t CompressPairs(uint8_t* c, uint32_t n, uint32_t first_single)
   return m;
 }
 
-__global__ void KmerComplexityKernel(const uint64_t* __restrict__ words,
-                                     const uint64_t* __restrict__ woff,
-                                     const uint32_t* __restrict__ lens,
-                                     const uint32_t* __restrict__ read_idx,
-                                     const uint32_t* __restrict__ pos, uint64_t n,
-                                     uint32_t k, uint8_t* __restrict__ keep) {
-  const uint64_t t = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (t >= n) return;
-  const uint32_t r = read_idx[t];
-  const uint32_t p = pos[t];
-  const uint32_t len = lens[r];
-  const uint64_t* w = words + woff[r];
+// the test of one k-mer: true iff the reference marks kmers_[p >> 4]
+__device__ bool KmerPasses(const uint64_t* __restrict__ w, uint32_t len, uint32_t p,
+                           uint32_t k) {
   uint8_t c[32];
   uint32_t m = 0;
   // InflateData(p, k) clamps at the read end
@@ -172,16 +163,49 @@ __global__ void KmerComplexityKernel(const uint64_t* __restrict__ words,
     if (i == 0 || c[i] != c[i - 1]) c[q++] = c[i];
   }
   m = q;
-  bool ok = m >= need;
-  if (ok) {  // (2) 2-mers at even offsets
-    m = CompressPairs(c, m, 0);
-    ok = m >= need;
+  if (m < need) return false;
+  m = CompressPairs(c, m, 0);  // (2) 2-mers at even offsets
+  if (m < need) return false;
+  m = CompressPairs(c, m, 1);  // (3) 2-mers at odd offsets
+  return m >= need;
+}
+
+__global__ void KmerComplexityKernel(const uint64_t* __restrict__ words,
+                                     const uint64_t* __restrict__ woff,
+                                     const uint32_t* __restrict__ lens,
+                                     const uint32_t* __restrict__ read_idx,
+                                     const uint32_t* __restrict__ pos, uint64_t n,
+                                     uint32_t k, uint8_t* __restrict__ keep) {
+  const uint64_t t = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  const uint32_t r = read_idx[t];
+  keep[t] = KmerPasses(words + woff[r], lens[r], pos[t], k) ? 1 : 0;
+}
+
+// One thread per filtered position of the flush's nr query reads (from read `first` on):
+// its read by binary search in the per-read offsets, then the test and the mark.
+__global__ void KmerMarksKernel(const uint64_t* __restrict__ words,
+                                const uint64_t* __restrict__ woff,
+                                const uint32_t* __restrict__ lens,
+                                const uint32_t* __restrict__ pos,
+                                const uint64_t* __restrict__ read_off, uint32_t first,
+                                uint32_t nr, uint64_t n, uint32_t k,
+                                const uint64_t* __restrict__ bit_off,
+                                uint32_t* __restrict__ bits, uint8_t* __restrict__ touched) {
+  const uint64_t t = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  uint32_t lo = 0, hi = nr;  // the read i with read_off[i] <= t < read_off[i + 1]
+  while (hi - lo > 1) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (read_off[mid] <= t) lo = mid; else hi = mid;
   }
-  if (ok) {  // (3) 2-mers at odd offsets
-    m = CompressPairs(c, m, 1);
-    ok = m >= need;
+  const uint32_t r = first + lo;
+  const uint32_t p = pos[t];
+  touched[r] = 1;
+  if (KmerPasses(words + woff[r], lens[r], p, k)) {
+    const uint32_t bin = p >> 4;
+    atomicOr(bits + bit_off[r] + (bin >> 5), 1u << (bin & 31));
   }
-  keep[t] = ok ? 1 : 0;
 }
 
 // Pile::FindValidRegion(coverage) + Pile::FindMedian (pile.cc:122-172) of fresh piles
@@ -267,6 +291,18 @@ void KmerComplexity(Ctx& c, const uint32_t* h_read_idx, const uint32_t* h_pos,
   ++c.launches;
   RVN_CUDA(cudaMemcpyAsync(h_keep, d_keep, n, cudaMemcpyDeviceToHost, c.stream));
   RVN_CUDA(cudaStreamSynchronize(c.stream));
+}
+
+void Stage2KmerMarks(Ctx& c, uint32_t first, uint32_t nr, uint32_t k) {
+  const uint64_t n = c.m_n_filtered;
+  if (n == 0) return;
+  TimerBegin(c, "stage2_kmers");
+  KmerMarksKernel<<<CeilDiv(n, 256), 256, 0, c.stream>>>(
+      c.d_words.get(), c.d_woff.get(), c.d_len.get(), c.m_filtered.get(), c.m_filtered_off.get(),
+      first, nr, n, k, c.s2_bit_off.get(), c.s2_bits.get(), c.s2_touched.get());
+  RVN_LAUNCH_CHECK();
+  ++c.launches;
+  TimerEnd(c);
 }
 
 // valid regions and medians of the piles of the last stage-1 call: on the device

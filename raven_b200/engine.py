@@ -61,6 +61,7 @@ class Engine:
                 "(raven_b200 has no CPU fallback)")
         self.h = h
         self.n_reads = 0
+        self._s2_n = 0
         self._keep = None
 
     def close(self):
@@ -80,14 +81,26 @@ class Engine:
         self._check(self.lib.rvn_engine_configure(self.h, k, w, bandwidth, chain,
                                                   matches, gap))
 
-    def upload(self, rs, resident=None):
+    def upload(self, rs, resident=None, ids=None):
         """resident = (first, last): copy only the bases of those reads to the
-        device (a rank of a partitioned run sketches its own range)."""
+        device (a rank of a partitioned run sketches its own range). ids: the reads'
+        ids (biosoup::NucleicAcid::id, the overlaps' lhs_id / rhs_id), default their
+        positions."""
         words = np.ascontiguousarray(rs.words, dtype=np.uint64)
         woff = np.ascontiguousarray(rs.word_off, dtype=np.uint64)
         lens = np.ascontiguousarray(rs.lens, dtype=np.uint32)
         self._keep = (words, woff, lens)
-        if resident is None:
+        if ids is not None:
+            if resident is not None:
+                raise ValueError("ids and resident do not combine")
+            ids = np.ascontiguousarray(ids, dtype=np.uint32)
+            if ids.size != rs.n:
+                raise ValueError("one id per read")
+            self._keep += (ids,)
+            self._check(self.lib.rvn_reads_upload_ids(
+                self.h, words.ctypes.data_as(U64P), woff.ctypes.data_as(U64P),
+                lens.ctypes.data_as(U32P), ids.ctypes.data_as(U32P), rs.n))
+        elif resident is None:
             self._check(self.lib.rvn_reads_upload(
                 self.h, words.ctypes.data_as(U64P), woff.ctypes.data_as(U64P),
                 lens.ctypes.data_as(U32P), rs.n))
@@ -239,6 +252,49 @@ class Engine:
         return dict(overlaps=_arr(o, int(ovl_off[-1]) * 8, np.uint32).reshape(-1, 8),
                     ovl_off=ovl_off, pile=_arr(p, int(pile_off[-1]), np.uint16),
                     pile_off=pile_off, num_mapped=nm.value)
+
+    # ---- raven::FindOverlapsAndRepetetiveRegions ----
+    def find_overlaps_and_repetitive_regions(self, freq, identity, n_valid, region_begin,
+                                             region_end, fetch=True):
+        """The map, Pile::AddKmers and identity-filter part of stage 2 (construct.cc:
+        352-424) over the first n_valid uploaded reads, which must be the valid reads in
+        the reference's sorted order, uploaded with their ids. region_begin / region_end:
+        Pile::begin() / end() of each valid read, in bases."""
+        rb = np.ascontiguousarray(region_begin, dtype=np.uint32)
+        re_ = np.ascontiguousarray(region_end, dtype=np.uint32)
+        if rb.size < n_valid or re_.size < n_valid:
+            raise ValueError("one region per valid read")
+        self._check(self.lib.rvn_find_overlaps_and_repetitive_regions(
+            self.h, float(freq), float(identity), int(n_valid), rb.ctypes.data_as(U32P),
+            re_.ctypes.data_as(U32P)))
+        self._s2_n = int(n_valid)
+        return self.stage2_results() if fetch else None
+
+    def stage2_results(self):
+        """Results of the last find_overlaps_and_repetitive_regions call: the final
+        overlaps in the order the classification loop takes them (rows of 8 u32) and
+        ovl_off (a batch ending at valid read i holds rows [ovl_off[i], ovl_off[i+1])),
+        per valid read its k-mer marks (kmers[i]: bool array of (len >> 4) + 1 bits, the
+        reference's Pile::kmers_) and whether the reference resized kmers_ (touched), and
+        the number of overlaps mapped before the clip and the identity filter."""
+        o, off, bits, koff = OVLP(), U64P(), U32P(), U64P()
+        touched, nm = C.POINTER(C.c_uint8)(), C.c_uint64(0)
+        self._check(self.lib.rvn_stage2_results(self.h, C.byref(o), C.byref(off),
+                                                C.byref(bits), C.byref(koff),
+                                                C.byref(touched), C.byref(nm)))
+        n = self._s2_n
+        ovl_off = _arr(off, n + 1, np.uint64)
+        kmer_off = _arr(koff, n + 1, np.uint64)
+        words = _arr(bits, int(kmer_off[-1]), np.uint32)
+        lens = np.asarray(self._keep[2][:n], dtype=np.uint64)
+        kmers = []
+        for i in range(n):
+            w = words[int(kmer_off[i]):int(kmer_off[i + 1])]
+            b = np.unpackbits(w.view(np.uint8), bitorder="little").astype(bool)
+            kmers.append(b[:int(lens[i] >> 4) + 1])
+        return dict(overlaps=_arr(o, int(ovl_off[-1]) * 8, np.uint32).reshape(-1, 8),
+                    ovl_off=ovl_off, kmer_bits=words, kmer_off=kmer_off, kmers=kmers,
+                    touched=_arr(touched, n, np.uint8).astype(bool), num_mapped=nm.value)
 
     # ---- edlibAlign(..., edlibDefaultAlignConfig()) of the identity filter ----
     def edit_distance_batch(self, lhs_read, lhs_begin, lhs_len, rhs_read, rhs_begin, rhs_len,

@@ -46,6 +46,31 @@ def make_reads(genome_len=100_000, n_reads=200, mean_len=5000, seed=1, sub=0.03,
     return seqio.pack_codes(seqs)
 
 
+def repeat_genome(genome_len=200_000, families=4, family_len=2000, copies=8,
+                  tandem_every=5000, tandem_len=120, seed=1, divergence=0.01):
+    """A random genome with planted repeats: `families` interspersed families of
+    `copies` near-identical copies (substitutions at `divergence`), and a short tandem
+    repeat (dinucleotide, trinucleotide or homopolymer run of tandem_len bases) every
+    tandem_every bases. Their minimizers are the frequent ones stage 2 filters: the
+    families' k-mers pass Pile::AddKmers' complexity test, the tandem repeats' fail it."""
+    rng = np.random.default_rng(seed)
+    g = rng.integers(0, 4, genome_len, dtype=np.uint8)
+    for _ in range(families):
+        fam = rng.integers(0, 4, family_len, dtype=np.uint8)
+        for _ in range(copies):
+            c = fam.copy()
+            hit = rng.random(family_len) < divergence
+            c[hit] = (c[hit] + rng.integers(1, 4, int(hit.sum()))) % 4
+            if rng.random() < 0.5:
+                c = (3 - c[::-1]).astype(np.uint8)
+            at = int(rng.integers(0, genome_len - family_len))
+            g[at:at + family_len] = c
+    for at in range(tandem_every // 2, genome_len - tandem_len, tandem_every):
+        unit = rng.integers(0, 4, int(rng.integers(1, 4)), dtype=np.uint8)
+        g[at:at + tandem_len] = np.resize(unit, tandem_len)
+    return g
+
+
 def random_reads(lengths, seed=1):
     """Unrelated random reads of given lengths (edge-case tests)."""
     rng = np.random.default_rng(seed)
