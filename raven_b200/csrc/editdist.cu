@@ -242,24 +242,31 @@ void MyersTiers(Ctx& c, const PairDesc* d_pairs, uint32_t* d_list, uint32_t n,
   uint32_t* list = w == 0 ? list2 : d_list;
   uint32_t* spare = w == 0 ? d_list : list2;
   static const int kTierK[4] = {64, 192, 448, 960};
+  // one phase per tier that runs: the timings tell how far a call's pairs went
+  static const char* const kTierPhase[5] = {"myers_k64", "myers_k192", "myers_k448",
+                                            "myers_k960", "myers_full"};
   uint32_t m = n, max_q_len = 0;
   for (int tier = 0; tier <= 4 && m > 0; ++tier) {
-    if (tier == 0) LaunchTier<4, 128>(c, d_pairs, list, m, kTierK[0], d_limit, d_out);
-    if (tier == 1) LaunchTier<8, 128>(c, d_pairs, list, m, kTierK[1], d_limit, d_out);
-    if (tier == 2) LaunchTier<16, 64>(c, d_pairs, list, m, kTierK[2], d_limit, d_out);
-    if (tier == 3) LaunchTier<32, 64>(c, d_pairs, list, m, kTierK[3], d_limit, d_out);
     if (tier == 4) {
       // unbanded: scratch for the vectors of every query block of every pair in flight
       const uint32_t max_blocks = std::max(1u, (max_q_len + 63) / 64);
       const uint64_t threads = static_cast<uint64_t>(CeilDiv(m, 64)) * 64;
       uint64_t* scratch = c.m_scratch64.reserve(2ULL * max_blocks * threads + 16);
+      TimerBegin(c, kTierPhase[4]);
       FullMyersKernel<<<CeilDiv(m, 64), 64, 0, c.stream>>>(c.d_words.get(), d_pairs, list, m,
                                                           max_blocks, scratch, d_out,
                                                           c.n_words + 2);
       RVN_LAUNCH_CHECK();
       ++c.launches;
+      TimerEnd(c);
       break;
     }
+    TimerBegin(c, kTierPhase[tier]);
+    if (tier == 0) LaunchTier<4, 128>(c, d_pairs, list, m, kTierK[0], d_limit, d_out);
+    if (tier == 1) LaunchTier<8, 128>(c, d_pairs, list, m, kTierK[1], d_limit, d_out);
+    if (tier == 2) LaunchTier<16, 64>(c, d_pairs, list, m, kTierK[2], d_limit, d_out);
+    if (tier == 3) LaunchTier<32, 64>(c, d_pairs, list, m, kTierK[3], d_limit, d_out);
+    TimerEnd(c);
     RVN_CUDA(cudaMemsetAsync(flag + m, 0, sizeof(uint32_t), c.stream));  // (the max below)
     OpenPairsKernel<<<CeilDiv(m, 256), 256, 0, c.stream>>>(d_pairs, list, m, kTierK[tier],
                                                            d_limit, d_out, flag, flag + m);

@@ -487,6 +487,14 @@ class Engine:
         self._check(self.lib.rvn_get_timings(self.h, C.byref(names), None, C.byref(n)))
         return sum(names[i] == b"map_flush" for i in range(n.value))
 
+    def phases(self):
+        """The phases since the last "reset_stats" in the order they ran, one name per
+        occurrence (timings() sums them by name)."""
+        names = C.POINTER(C.c_char_p)()
+        n = C.c_uint32(0)
+        self._check(self.lib.rvn_get_timings(self.h, C.byref(names), None, C.byref(n)))
+        return [names[i].decode() for i in range(n.value)]
+
     def stats(self):
         s = Stats()
         self._check(self.lib.rvn_get_stats(self.h, C.byref(s)))

@@ -277,6 +277,48 @@ class Reference(_Flat):
         return self.unbag(bag, dict(pile=np.uint16))["pile"]
 
 
+class ReferenceStage2(_Flat):
+    """The reference's stage 2 over given valid regions (oracle/_ref/libraven_ref_stage2.so)."""
+
+    PATH = os.path.join(ORACLE_DIR, "_ref", "libraven_ref_stage2.so")
+
+    @classmethod
+    def available(cls):
+        return os.path.exists(cls.PATH)
+
+    def __init__(self):
+        super().__init__(self.PATH, "refs2")
+        L = self.lib
+        L.ref_stage2.restype = C.c_void_p
+        L.ref_stage2.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_double, C.c_double,
+                                 C.c_uint32, _U32P, _U32P, _U8P]
+
+    def stage2(self, rs, k, w, freq, identity, region_begin, region_end, invalid, threads=1):
+        """raven::FindOverlapsAndRepetetiveRegions over fresh piles of the reads of `rs`
+        (ids 0..n-1) with the given valid regions (in bins) and invalid flags: valid (the
+        sorted valid ids it maps, the first s), s, overlaps (overlaps.back() at the end),
+        per pile kmers (Pile::kmers_), touched (kmers_ resized) and contained."""
+        rb = np.ascontiguousarray(region_begin, dtype=np.uint32)
+        re_ = np.ascontiguousarray(region_end, dtype=np.uint32)
+        inv = np.ascontiguousarray(invalid, dtype=np.uint8)
+        if not rb.size == re_.size == inv.size == rs.n:
+            raise ValueError("one region and flag per read")
+        reads = self.reads(rs)
+        bag = self.lib.ref_stage2(reads.h, k, w, freq, identity, threads, _ptr(rb, _U32P),
+                                  _ptr(re_, _U32P), _ptr(inv, _U8P))
+        r = self.unbag(bag, dict(valid=np.uint32, s=np.uint32, overlaps=np.uint32,
+                                 kmers=np.uint8, kmer_off=np.uint64, touched=np.uint8,
+                                 contained=np.uint8))
+        off = r.pop("kmer_off")
+        flat = r.pop("kmers").astype(bool)
+        r["kmers"] = [flat[int(off[i]):int(off[i + 1])] for i in range(rs.n)]
+        r["s"] = int(r["s"][0])
+        r["overlaps"] = r["overlaps"].reshape(-1, 8)
+        r["touched"] = r["touched"].astype(bool)
+        r["contained"] = r["contained"].astype(bool)
+        return r
+
+
 def ref_pile_trim(ref, pile, pile_off, coverage=4):
     """Pile::FindValidRegion(coverage) + FindMedian of the compiled reference (oracle/_ref)
     on the given histograms: begin, end, median, invalid per pile and the trimmed data."""
