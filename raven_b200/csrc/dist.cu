@@ -651,13 +651,11 @@ void DistStage1Begin(Ctx& c, uint32_t parts, uint32_t rank) {
   c.ds_results_valid = false;
   const uint32_t n = c.n_reads;
   c.st_valid = false;
-  c.st_pile_off.assign(n + 1ULL, 0);
-  for (uint32_t i = 0; i < n; ++i) c.st_pile_off[i + 1] = c.st_pile_off[i] + (c.h_len[i] >> 4);
-  const uint64_t total_bins = c.st_pile_off[n];
+  const uint64_t total_bins = c.h_pile_off[n];
   uint16_t* d_pile = c.p_data.reserve(total_bins + 1);
   uint64_t* d_poff = c.p_off.reserve(n + 1ULL);
   RVN_CUDA(cudaMemsetAsync(d_pile, 0, (total_bins + 1) * 2, c.stream));
-  RVN_CUDA(cudaMemcpyAsync(d_poff, c.st_pile_off.data(), (n + 1ULL) * 8, cudaMemcpyHostToDevice,
+  RVN_CUDA(cudaMemcpyAsync(d_poff, c.h_pile_off.data(), (n + 1ULL) * 8, cudaMemcpyHostToDevice,
                            c.stream));
   GatherReset(c);
   c.st_mapped = 0;
@@ -716,20 +714,17 @@ void DistStage1Add(Ctx& c, const rvn_overlap* d_ovl, uint64_t n_ovl, uint32_t n_
 
   // ---- the reference's flush schedule over the merged list ----
   uint64_t* d_rel = c.ds_rel_off.reserve(n + 2ULL);
-  uint64_t bases = 0;
-  for (uint32_t k = 0, k0 = 0; k < n_query; ++k) {
-    bases += c.h_len[k];
-    if (k != n_query - 1 && bases < qb) continue;
-    bases = 0;
-    const uint64_t b = h_off[k0], e = h_off[k + 1];
+  const std::vector<uint32_t> cuts = ChunkCuts(c, 0, n_query, qb);
+  for (size_t i = 0; i + 1 < cuts.size(); ++i) {
+    const uint32_t k0 = cuts[i], k1 = cuts[i + 1];
+    const uint64_t b = h_off[k0], e = h_off[k1];
     if (e > b) {
-      RelativeOffsets<<<CeilDiv(k + 2 - k0, kThreads), kThreads, 0, c.stream>>>(qoff, k0,
-                                                                              k + 2 - k0, d_rel);
-      PileAddLayersDevice(c, c.p_data.get(), c.p_off.get(), c.st_pile_off[n], Window::All(n),
+      RelativeOffsets<<<CeilDiv(k1 + 1 - k0, kThreads), kThreads, 0, c.stream>>>(qoff, k0,
+                                                                               k1 + 1 - k0, d_rel);
+      PileAddLayersDevice(c, c.p_data.get(), c.p_off.get(), c.h_pile_off[n], Window::All(n),
                           merged + b, e - b);
-      GatherFlush(c, merged + b, d_rel, e - b, k0, k + 1, kmax, Window::All(n));
+      GatherFlush(c, merged + b, d_rel, e - b, k0, k1, kmax, Window::All(n));
     }
-    k0 = k + 1;
   }
 }
 

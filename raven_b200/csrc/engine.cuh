@@ -9,6 +9,7 @@
 //   overlaps   rvn_overlap[]     32 B records grouped by query read
 #pragma once
 
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -89,6 +90,9 @@ struct Ctx {
   DevBuf<uint32_t> d_len, d_ids;
   std::vector<uint64_t> h_woff;
   std::vector<uint32_t> h_len, h_ids;
+  // first pile bin of every read (len >> 4 bins), n_reads + 1 entries (before the first
+  // upload too: a context starts as an empty read set)
+  std::vector<uint64_t> h_pile_off{0};
   bool ids_identity = true;  // id == index (needed by the device-side gather)
   uint32_t res_first = 0, res_last = 0;  // reads whose bases are in HBM
   // sketch tiles: tile_off[r] = first tile of read r (depends on k)
@@ -233,7 +237,7 @@ struct Ctx {
   DevBuf<uint32_t> g_cnt, g_kept, g_key, g_idx, g_key2, g_idx2, g_rhs_cnt,
       g_total_cnt;
 
-  // ---- windowed stage 1 (capi.cu): piles and lists of all reads on the host,
+  // ---- windowed stage 1 (stage.cu): piles and lists of all reads on the host,
   // a flush's window of them on the device ----
   // option "stage1_window": 0 resident, 1 windowed, -1 (default) windowed only when
   // the resident estimate exceeds the free device memory ("stage1_window_budget"
@@ -290,7 +294,6 @@ struct Ctx {
   PinBuf<rvn_overlap> st_ovl;  // pinned: the D2H of the results runs at link speed
   PinBuf<uint64_t> st_ovl_off;
   PinBuf<uint16_t> st_pile;
-  std::vector<uint64_t> st_pile_off;
   uint64_t st_mapped = 0;
   bool st_valid = false;
   bool st_piles_on_device = false;  // c.p_data / c.p_off still hold the piles of that call
@@ -302,7 +305,7 @@ struct Ctx {
   cudaStream_t d2h_stream = nullptr;
   cudaEvent_t d2h_ready = nullptr, d2h_done = nullptr;
 
-  // ---- stage 2 (capi.cu Stage2): per valid read its pile region, the k-mer marks (one
+  // ---- stage 2 (stage.cu Stage2): per valid read its pile region, the k-mer marks (one
   // bit per pile bin and one past the end, bins + 1 bits in whole u32 words) and the
   // touched flag, resident for the whole call; the kept overlaps of every batch ----
   DevBuf<uint32_t> s2_pos_of, s2_rbeg, s2_rend, s2_bits;
@@ -415,6 +418,8 @@ uint64_t MaxMicromizerValue(Ctx& c, uint32_t first, uint32_t last);
 // c.i_org_alt, at k <= 15, w = 5 straight from the sketch kernel (SketchAppend).
 uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash,
                            uint64_t chunk, uint64_t tmax, bool tiers = true);
+// bases of reads [first, last)
+uint64_t ReadBases(const Ctx& c, uint32_t first, uint32_t last);
 // reads [first, last) cut into ranges of >= chunk bases at read boundaries, by the rule
 // that cuts index batches (construct.cc:36-44): boundaries first, ..., last
 std::vector<uint32_t> ChunkCuts(const Ctx& c, uint32_t first, uint32_t last, uint64_t chunk);
@@ -555,6 +560,30 @@ void Stage2KmerMarks(Ctx& c, uint32_t first, uint32_t nr, uint32_t k);
 void PileAddLayersDevice(Ctx& c, uint16_t* d_data, const uint64_t* d_off, uint64_t bins,
                          const Window& w, const rvn_overlap* d_ovl, uint64_t n_ovl,
                          uint32_t first = 0);
+
+// ---- stage.cu ---- the overlap stages' host drivers
+// raven::FindOverlapsAndCreatePiles: index batches of >= ib bases, query flushes of >= qb
+// bases (0: the reference's 2^32 and 2^30)
+void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib, uint64_t qb);
+// raven::FindOverlapsAndRepetetiveRegions' device work over the first n uploaded reads,
+// with their valid regions [h_rbeg, h_rend)
+void Stage2(Ctx& c, double freq, double identity, uint32_t n, const uint32_t* h_rbeg,
+            const uint32_t* h_rend);
+// rvn_map over reads [first, last) in flushes; each: called after every flush instead of
+// gathering its results on the host (stage 2)
+void MapFlushes(Ctx& c, uint32_t first, uint32_t last, bool avoid_equal, bool avoid_symmetric,
+                bool minhash, bool want_filtered,
+                const std::function<void(uint32_t, uint32_t)>& each = nullptr);
+// rvn_minimize and rvn_filter (returns the occurrence threshold)
+void Minimize(Ctx& c, uint32_t first, uint32_t last, bool minhash);
+uint32_t Filter(Ctx& c, double freq);
+// the estimates rvn_stage1_footprint, rvn_index_footprint and rvn_minimize_footprint
+// return, into the outputs that are not null
+void Stage1Footprints(const Ctx& c, uint64_t kmax, uint64_t ib, uint64_t qb,
+                      uint64_t* resident, uint64_t* windowed_device, uint64_t* windowed_host);
+void IndexFootprints(const Ctx& c, uint64_t ib, uint64_t* one_shot, uint64_t* chunked);
+void MinimizeFootprints(const Ctx& c, uint32_t first, uint32_t last, uint64_t* one_shot,
+                        uint64_t* chunked, uint64_t* chunk);
 
 // ---- poa.cu ---- racon window consensus over a flat batch of windows
 // the flat layout of a batch of windows in device memory (rvn_poa_batch's arguments)

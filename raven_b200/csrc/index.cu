@@ -610,12 +610,10 @@ void BuildIndex(Ctx& c, uint32_t first, uint32_t last, bool minhash, uint64_t va
     src_org = c.q_org.get();
     n = c.q_n;
   }
-  uint64_t bases = 0;
-  for (uint32_t r = first; r < last; ++r) bases += c.h_len[r];
   c.i_first = first;
   c.i_last = last;
-  BuildIndexFrom(c, src_val, src_org, n, bases, minhash ? ~0ULL : value_limit,
-                 /*count_bare=*/true);
+  BuildIndexFrom(c, src_val, src_org, n, ReadBases(c, first, last),
+                 minhash ? ~0ULL : value_limit, /*count_bare=*/true);
   c.i_sorted_ids = c.ids_ascending;
   c.i_from_sketch = !minhash;
 }
@@ -869,6 +867,12 @@ void BuildIndexImpl(Ctx& c, ValView src_val, const uint64_t* src_org, uint64_t n
 
 }  // namespace
 
+uint64_t ReadBases(const Ctx& c, uint32_t first, uint32_t last) {
+  uint64_t bases = 0;
+  for (uint32_t r = first; r < last; ++r) bases += c.h_len[r];
+  return bases;
+}
+
 std::vector<uint32_t> ChunkCuts(const Ctx& c, uint32_t first, uint32_t last, uint64_t chunk) {
   std::vector<uint32_t> cuts{first};
   uint64_t bases = 0;
@@ -899,8 +903,7 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
   unsigned long long* vhist = reinterpret_cast<unsigned long long*>(c.t_hist.reserve(kCapBins));
   RVN_CUDA(cudaMemsetAsync(vhist, 0, kCapBins * sizeof(uint64_t), c.stream));
 
-  uint64_t bases = 0;
-  for (uint32_t r = first; r < last; ++r) bases += c.h_len[r];
+  const uint64_t bases = ReadBases(c, first, last);
   if (minhash) {
     // one sweep: each chunk's micromizers are appended to the sort's second buffers,
     // sized by the len / k micromizers a read has at most

@@ -1613,9 +1613,7 @@ void MapRange(Ctx& c, uint32_t first, uint32_t last, bool avoid_equal,
   c.m_last_read = last;
   c.r_valid = fetch;
 
-  uint64_t qbases = 0;
-  for (uint32_t r = first; r < last; ++r) qbases += c.h_len[r];
-  c.stats.query_bases += qbases;
+  c.stats.query_bases += ReadBases(c, first, last);
   c.stats.query_records += n_q;
   c.stats.hits += n_hits;
   c.stats.overlaps += n_ovl;

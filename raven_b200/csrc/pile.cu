@@ -326,7 +326,7 @@ void StagePileRegions(Ctx& c, uint32_t coverage, uint32_t* h_begin, uint32_t* h_
     RVN_LAUNCH_CHECK();
     ++c.launches;
   } else {
-    const std::vector<uint64_t>& off = c.st_pile_off;
+    const std::vector<uint64_t>& off = c.h_pile_off;
     uint64_t* d_off = c.p_off.reserve(n + 1ULL);
     RVN_CUDA(cudaMemcpyAsync(d_off, off.data(), (n + 1ULL) * 8, cudaMemcpyHostToDevice,
                              c.stream));

@@ -907,6 +907,12 @@ size_t SketchSmemBytes(uint32_t w, size_t hash_bytes) {
 
 }  // namespace
 
+void WaitUpload(Ctx& c) {
+  if (!c.up_pending) return;
+  RVN_CUDA(cudaStreamWaitEvent(c.stream, c.up_events[c.up_chunks - 1], 0));
+  c.up_pending = false;
+}
+
 void EnsureTiles(Ctx& c) {
   if (c.tiles_k == c.prm.k && c.h_tile_off.size() == c.n_reads + 1ULL) return;
   c.h_tile_off.assign(c.n_reads + 1ULL, 0);
