@@ -130,6 +130,13 @@ int rvn_reads_upload_ids(rvn_ctx* ctx, const uint64_t* words,
                          const uint64_t* word_off, const uint32_t* lens,
                          const uint32_t* ids, uint32_t n_reads);
 
+/* Where the packed bases of the current upload live (option "host_bases"): *on_host = 1
+ * when they stay in the context's pinned host copy and the sketch kernels read them from a
+ * staging window, 0 when the device holds the whole set; *device_word_bytes = the device
+ * bytes of packed words held for them (the staging window, or the whole set). Either
+ * output may be NULL. */
+int rvn_reads_residency(rvn_ctx* ctx, int* on_host, uint64_t* device_word_bytes);
+
 /* Minimize(reads[first..last), minhash): sketch and index. The index holds every record
  * (full sketches may probe it). Option "index_chunk_bases" applies: built in chunks, no
  * sketch of the whole range is held, and the rvn_filter that follows frees the build's
@@ -449,7 +456,25 @@ int rvn_get_stats(rvn_ctx* ctx, rvn_stats* out);
  * rvn_reads_upload* returns while the packed bases still travel - in chunks, on a
  * copy stream - and the sketch kernel of the next call starts on the reads that
  * have arrived; the caller must keep `words` unchanged until the next call on the
- * context has returned; meant for pinned host memory); "stage1_window" (where
+ * context has returned; meant for pinned host memory; ignored when the bases stay on the
+ * host); "host_bases" (where rvn_reads_upload and rvn_reads_upload_ids keep the packed
+ * bases: 0 = on the device for as long as the upload lives; 1 = in a pinned host copy the
+ * context makes during the upload (the caller may change its words once the call returns),
+ * and every sketch copies the words of its read range - an index batch, one chunk of a
+ * chunked build, or one map flush - into one of two device halves of a staging window,
+ * the drivers copying the next range while the current one is sketched and the kernels
+ * that read no bases run; -1 = auto, the default: on the host only when the windowed,
+ * chunked stage-1 estimate of the reference's schedule (2^32-base index batches, 2^30-base
+ * flushes, max_overlaps 32) exceeds the usable device memory with the bases on the device
+ * and fits with the staging window instead. rvn_reads_upload_range always keeps them on the
+ * device. rvn_edit_distance_batch, rvn_align_breaking_points, rvn_polish_windows,
+ * rvn_kmer_complexity and rvn_find_overlaps_and_repetitive_regions read bases at random
+ * positions: on a context whose bases are on the host they first copy the whole set to the
+ * device (which then holds it until the next upload), or return RVN_ERR_LIMIT naming the
+ * bytes when it does not fit. Results are identical in every mode; phase "stage_bases" in
+ * rvn_get_timings is the copy time no kernel hid; rvn_reads_residency tells where the bases
+ * are); "host_bases_budget" (bytes: replaces the usable device memory in the auto decision
+ * and in that fit test, 0 = the free memory); "stage1_window" (where
  * rvn_find_overlaps_and_create_piles keeps the piles and overlap lists of all reads:
  * 0 = on the device for the whole pass; 1 = windowed: in pinned host memory, and
  * each flush brings only the reads it touches - its queries and the current index

@@ -41,6 +41,7 @@ SIGNATURES = {
     "rvn_reads_upload_range": (C.c_int, [C.c_void_p, U64P, U64P, U32P, C.c_uint32,
                                          C.c_uint32, C.c_uint32]),
     "rvn_reads_upload_ids": (C.c_int, [C.c_void_p, U64P, U64P, U32P, U32P, C.c_uint32]),
+    "rvn_reads_residency": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), U64P]),
     "rvn_map_external": (C.c_int, [C.c_void_p, U64P, C.c_uint32, C.c_uint32, C.c_int,
                                    C.c_int, C.c_int, C.c_int]),
     "rvn_minimize": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_int]),

@@ -60,6 +60,12 @@ void SetOption(Ctx& c, const char* name, int64_t value) {
     c.keep_hits = value != 0;
   } else if (name && std::strcmp(name, "async_upload") == 0) {
     c.async_upload = value != 0;
+  } else if (name && std::strcmp(name, "host_bases") == 0) {
+    if (value < -1 || value > 1) throw InvalidArgument("host_bases: -1 (auto), 0 or 1");
+    c.host_bases = value;
+  } else if (name && std::strcmp(name, "host_bases_budget") == 0) {
+    if (value < 0) throw InvalidArgument("host_bases_budget: bytes, 0 = the free memory");
+    c.host_bases_budget = static_cast<uint64_t>(value);
   } else if (name && std::strcmp(name, "self_join") == 0) {
     c.self_join = value != 0;
   } else if (name && std::strcmp(name, "bare_count") == 0) {
@@ -189,6 +195,10 @@ RVN_API void rvn_ctx_destroy(rvn_ctx* ctx) {
     cudaEventDestroy(ctx->c.d2h_done);
   }
   for (auto e : ctx->c.up_events) cudaEventDestroy(e);
+  for (auto& h : ctx->c.bh) {
+    for (auto e : h.events) cudaEventDestroy(e);
+    if (h.used) cudaEventDestroy(h.used);
+  }
   if (ctx->c.up_fence) cudaEventDestroy(ctx->c.up_fence);
   if (ctx->c.own_stream) cudaStreamDestroy(ctx->c.stream);
   delete ctx;
@@ -216,10 +226,11 @@ RVN_API int rvn_engine_configure(rvn_ctx* ctx, uint32_t k, uint32_t w,
   });
 }
 
+// whole_set: rvn_reads_upload / rvn_reads_upload_ids, where option host_bases applies
 static void UploadReads(Ctx& c, const uint64_t* words, const uint64_t* word_off,
                         const uint32_t* lens, const uint32_t* ids,
                         uint32_t n_reads, uint32_t res_first = 0,
-                        uint32_t res_last = 0xFFFFFFFFu) {
+                        uint32_t res_last = 0xFFFFFFFFu, bool whole_set = false) {
   if (n_reads && (!word_off || !lens)) throw InvalidArgument("null read set");
   res_last = std::min(res_last, n_reads);
   if (res_first > res_last) throw InvalidArgument("resident range out of bounds");
@@ -248,8 +259,23 @@ static void UploadReads(Ctx& c, const uint64_t* words, const uint64_t* word_off,
     if (i > 0 && c.h_ids[i] < c.h_ids[i - 1]) c.ids_ascending = false;
   }
   c.n_words = c.h_woff[n_reads];
+  // (kernels and copies of earlier calls may still use the buffers of the old bases)
+  RVN_CUDA(cudaStreamSynchronize(c.stream));
+  if (c.copy_stream) RVN_CUDA(cudaStreamSynchronize(c.copy_stream));
+  c.bases_on_host = whole_set && UseHostBases(c);
+  if (c.bases_on_host) {
+    // the context's own pinned copy (the caller may change its words once this returns);
+    // the sketch kernels read it through the staging window
+    if (c.n_words && !words) throw InvalidArgument("null read set");
+    DropStagedBases(c, 0, /*release=*/false);
+    uint64_t* hw = c.h_words.reserve(c.n_words + 2);
+    if (c.n_words) std::memcpy(hw, words, c.n_words * sizeof(uint64_t));
+    c.d_words.release();
+  } else {
+    DropStagedBases(c, 0, /*release=*/true);
+  }
   // one spare slot everywhere: an external query read rides at index n_reads
-  uint64_t* dw = c.d_words.reserve(c.n_words + 2);
+  uint64_t* dw = c.bases_on_host ? nullptr : c.d_words.reserve(c.n_words + 2);
   uint64_t* dwo = c.d_woff.reserve(n_reads + 2ULL);
   uint32_t* dl = c.d_len.reserve(n_reads + 2ULL);
   uint32_t* di = c.d_ids.reserve(n_reads + 2ULL);
@@ -271,6 +297,7 @@ static void UploadReads(Ctx& c, const uint64_t* words, const uint64_t* word_off,
   const uint64_t w0 = c.h_woff[res_first], w1 = c.h_woff[res_last];
   c.up_pending = false;
   c.p_off_uploaded = false;
+  if (c.bases_on_host) return;  // (async_upload has nothing left to do)
   if (w1 > w0 && c.async_upload && res_last - res_first >= 1024) {
     // everything small the next call would send host-to-device goes first: behind the
     // bases it would wait for the copy engine (tile tables, pile offsets of stage 1)
@@ -325,7 +352,7 @@ RVN_API int rvn_reads_upload(rvn_ctx* ctx, const uint64_t* words,
                              const uint64_t* word_off, const uint32_t* lens,
                              uint32_t n_reads) {
   return Guard(ctx, [&](Ctx& c) {
-    UploadReads(c, words, word_off, lens, nullptr, n_reads);
+    UploadReads(c, words, word_off, lens, nullptr, n_reads, 0, 0xFFFFFFFFu, /*whole_set=*/true);
   }, /*sketches_first=*/true);
 }
 
@@ -341,7 +368,7 @@ RVN_API int rvn_reads_upload_ids(rvn_ctx* ctx, const uint64_t* words,
                                  const uint64_t* word_off, const uint32_t* lens,
                                  const uint32_t* ids, uint32_t n_reads) {
   return Guard(ctx, [&](Ctx& c) {
-    UploadReads(c, words, word_off, lens, ids, n_reads);
+    UploadReads(c, words, word_off, lens, ids, n_reads, 0, 0xFFFFFFFFu, /*whole_set=*/true);
   }, /*sketches_first=*/true);
 }
 
@@ -356,10 +383,12 @@ RVN_API int rvn_map_external(rvn_ctx* ctx, const uint64_t* words, uint32_t len,
     const uint32_t n = c.n_reads;
     const uint64_t nw = (static_cast<uint64_t>(len) + 31) >> 5;
     if (nw && !words) throw InvalidArgument("null read");
-    uint64_t* dw = c.d_words.reserve_keep(c.n_words + nw + 2, c.n_words, c.stream);
-    if (nw) {
-      RVN_CUDA(cudaMemcpyAsync(dw + c.n_words, words, nw * 8,
-                               cudaMemcpyHostToDevice, c.stream));
+    if (!c.bases_on_host) {
+      uint64_t* dw = c.d_words.reserve_keep(c.n_words + nw + 2, c.n_words, c.stream);
+      if (nw) {
+        RVN_CUDA(cudaMemcpyAsync(dw + c.n_words, words, nw * 8,
+                                 cudaMemcpyHostToDevice, c.stream));
+      }
     }
     EnsureTiles(c);
     // extend the host/device tables by the spare slot
@@ -385,11 +414,13 @@ RVN_API int rvn_map_external(rvn_ctx* ctx, const uint64_t* words, uint32_t len,
     c.n_reads = n + 1;
     c.s_valid = c.q_valid = c.qt_valid = false;
     // the rider's bases are resident for the duration of the call (EnsureSketch
-    // refuses reads outside [res_first, res_last))
+    // refuses reads outside [res_first, res_last)); bases on the host: the rider takes a
+    // half of the staging window
     const uint32_t res_first0 = c.res_first, res_last0 = c.res_last;
     c.res_first = n;
     c.res_last = n + 1;
     auto restore = [&]() {
+      if (c.bases_on_host) DropStagedBases(c, n, /*release=*/false);
       c.res_first = res_first0;
       c.res_last = res_last0;
       c.n_reads = n;
@@ -398,6 +429,7 @@ RVN_API int rvn_map_external(rvn_ctx* ctx, const uint64_t* words, uint32_t len,
       c.s_valid = c.q_valid = c.qt_valid = false;
     };
     try {
+      if (c.bases_on_host) StageExternalBases(c, n, words);
       // an id below an indexed id breaks the "kept postings are a suffix" shortcut
       // only through avoid_symmetric, which compares ids, not indices: fine
       MapRange(c, n, n + 1, avoid_equal != 0, avoid_symmetric != 0, minhash != 0,
@@ -530,6 +562,7 @@ RVN_API int rvn_polish_windows(rvn_ctx* ctx, uint64_t n_alignments, const uint32
                          (bp_off[n_alignments] && !breaking_points))) {
       throw InvalidArgument("null argument");
     }
+    EnsureDeviceBases(c);
     TimerReset(c);
     PolishArgs a{n_alignments, q_read, q_begin, q_len, strand, t_read, bp_off, breaking_points,
                  n_targets, window, block_quality, bq_off, reverse_complement, q, m, n, g,
@@ -549,6 +582,7 @@ RVN_API int rvn_kmer_complexity(rvn_ctx* ctx, const uint32_t* read_index,
     for (uint64_t i = 0; i < n; ++i) {
       if (read_index[i] >= c.n_reads) throw InvalidArgument("read index out of bounds");
     }
+    EnsureDeviceBases(c);
     KmerComplexity(c, read_index, positions, n, kmer_len, keep);
   });
 }
@@ -569,6 +603,7 @@ RVN_API int rvn_find_overlaps_and_repetitive_regions(rvn_ctx* ctx, double freque
                                                      const uint32_t* region_begin,
                                                      const uint32_t* region_end) {
   return Guard(ctx, [&](Ctx& c) {
+    EnsureDeviceBases(c);
     Stage2(c, frequency, identity, n_valid, region_begin, region_end);
     TimerCollect(c);
   }, /*sketches_first=*/true);
@@ -714,6 +749,7 @@ RVN_API int rvn_edit_distance_batch(rvn_ctx* ctx, uint64_t n_pairs, const uint32
                     !strand || !distance)) {
       throw InvalidArgument("null argument");
     }
+    EnsureDeviceBases(c);
     EditDistanceBatch(c, n_pairs, lhs_read, lhs_begin, lhs_len, rhs_read, rhs_begin, rhs_len,
                       strand, limit, distance);
     TimerCollect(c);
@@ -742,6 +778,7 @@ RVN_API int rvn_align_breaking_points(rvn_ctx* ctx, uint64_t n_pairs, const uint
                     !distance || (bp_off[n_pairs] && !breaking_points))) {
       throw InvalidArgument("null argument");
     }
+    EnsureDeviceBases(c);
     AlignBreakingPoints(c, n_pairs, q_read, q_begin, q_len, strand, t_read, t_begin, t_len, window,
                         bp_off, distance, breaking_points);
     TimerCollect(c);
@@ -875,6 +912,16 @@ RVN_API int rvn_debug_exclusive_scan(rvn_ctx* ctx, const uint32_t* in, uint64_t 
     }
     RVN_CUDA(cudaStreamSynchronize(c.stream));
   });
+}
+
+RVN_API int rvn_reads_residency(rvn_ctx* ctx, int* on_host, uint64_t* device_word_bytes) {
+  return Guard(ctx, [&](Ctx& c) {
+    if (on_host) *on_host = c.bases_on_host ? 1 : 0;
+    if (device_word_bytes) {
+      *device_word_bytes =
+          c.bases_on_host ? StagedBaseBytes(c) : c.d_words.cap * sizeof(uint64_t);
+    }
+  }, /*sketches_first=*/true);
 }
 
 RVN_API int rvn_get_stats(rvn_ctx* ctx, rvn_stats* out) {

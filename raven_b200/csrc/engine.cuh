@@ -61,6 +61,35 @@ struct PhaseTimer {
   std::vector<cudaEvent_t> pool;
 };
 
+// One half of the staging window of packed bases (host_bases mode, sketch.cu): the words of
+// the read range [first, last), word w of the set at words[w - woff[first]]. The copy runs
+// on the context's copy stream in pieces: reads [.., read_end[i]) have arrived once
+// events[i] has completed. `used` is recorded on the context's stream behind the last kernel
+// that read the half; a new copy into it waits for that.
+struct BaseHalf {
+  DevBuf<uint64_t> words;
+  uint32_t first = 0, last = 0;
+  bool valid = false;
+  std::vector<cudaEvent_t> events;
+  std::vector<uint32_t> read_end;
+  uint32_t pieces = 0;
+  cudaEvent_t used = nullptr;
+  bool used_recorded = false;
+};
+
+// Where the sketch kernels of a read range find their bases: word w of the set at
+// words[w - base]. pieces > 0: copies still in flight, reads [.., read_end[i]) complete once
+// events[i] has (the async_upload chunks, or a staged range's pieces). half: the staging
+// window's half that holds them, -1 = the device copy of the set (d_words).
+struct BaseView {
+  const uint64_t* words = nullptr;
+  uint64_t base = 0;
+  const cudaEvent_t* events = nullptr;
+  const uint32_t* read_end = nullptr;
+  uint32_t pieces = 0;
+  int half = -1;
+};
+
 struct Ctx {
   // device bytes held by this context's buffers (first member: it outlives them)
   uint64_t held_bytes = 0;
@@ -95,6 +124,20 @@ struct Ctx {
   std::vector<uint64_t> h_pile_off{0};
   bool ids_identity = true;  // id == index (needed by the device-side gather)
   uint32_t res_first = 0, res_last = 0;  // reads whose bases are in HBM
+  // option "host_bases": where rvn_reads_upload / rvn_reads_upload_ids keep the packed bases:
+  // 0 in d_words, 1 in the pinned host copy h_words (the sketch kernels read them from the
+  // staging window bh[]), -1 (default) on the host only when a stage-1 pass at the
+  // reference's batch sizes would fit the device with them there and not without
+  // ("host_bases_budget" replaces the usable device memory when it is not 0)
+  int64_t host_bases = -1;
+  uint64_t host_bases_budget = 0;
+  bool bases_on_host = false;  // the current upload's bases are in h_words only
+  PinBuf<uint64_t> h_words;
+  BaseHalf bh[2];
+  int bh_cur = 0;  // the half of the range a sketch asked for last
+  // reads whose bases the next sketch launch should be followed by a copy of (the range the
+  // driver sketches after it; empty: none)
+  uint32_t bases_next_first = 0, bases_next_last = 0;
   // sketch tiles: tile_off[r] = first tile of read r (depends on k)
   std::vector<uint64_t> h_tile_off;
   DevBuf<uint64_t> d_tile_off;
@@ -376,6 +419,21 @@ void EnsureSketch(Ctx& c, uint32_t first, uint32_t last);
 // micromizers of reads [first,last) into c.q_* (needs the sketch of a range
 // that contains [first,last))
 void WaitUpload(Ctx& c);  // the context's stream waits for an asynchronous upload
+// The bases of reads [first, last) for a sketch launch: the device copy of the set, or
+// (host_bases) a half of the staging window that holds them, copied there now unless a half
+// already does. The caller waits for the view's pieces, launches, then calls BasesLaunched.
+BaseView SketchBases(Ctx& c, uint32_t first, uint32_t last);
+// after the launches that read v: the half may be overwritten behind them, and the range
+// BasesNext named is copied into the other half now, beside the kernels that follow
+void BasesLaunched(Ctx& c, const BaseView& v);
+// the read range the caller sketches next: staged right after the next sketch launch
+// (no-op with the bases on the device)
+void BasesNext(Ctx& c, uint32_t first, uint32_t last);
+// rvn_map_external's rider, read n, whose words are on the caller's host memory
+void StageExternalBases(Ctx& c, uint32_t n, const uint64_t* words);
+// the halves holding reads >= `from` forget them; release: every half frees its memory
+void DropStagedBases(Ctx& c, uint32_t from, bool release);
+uint64_t StagedBaseBytes(const Ctx& c);  // device bytes of the staging window
 void EnsureMicromizers(Ctx& c, uint32_t first, uint32_t last);
 void EnsureThresholds(Ctx& c, uint32_t first, uint32_t last);
 // The sketch records of reads [first, last) straight into the two tiers of an index build
@@ -574,6 +632,13 @@ void Stage2(Ctx& c, double freq, double identity, uint32_t n, const uint32_t* h_
 void MapFlushes(Ctx& c, uint32_t first, uint32_t last, bool avoid_equal, bool avoid_symmetric,
                 bool minhash, bool want_filtered,
                 const std::function<void(uint32_t, uint32_t)>& each = nullptr);
+// option "host_bases" at an upload of the whole set (h_woff, h_len, h_pile_off are the new
+// set's): whether its bases stay on the host
+bool UseHostBases(const Ctx& c);
+// the calls that read bases at random positions: a set whose bases are on the host goes to
+// d_words whole first (the context is then in device mode until the next upload);
+// RVN_ERR_LIMIT when it does not fit the usable memory ("host_bases_budget" when not 0)
+void EnsureDeviceBases(Ctx& c);
 // rvn_minimize and rvn_filter (returns the occurrence threshold)
 void Minimize(Ctx& c, uint32_t first, uint32_t last, bool minhash);
 uint32_t Filter(Ctx& c, double freq);

@@ -890,12 +890,24 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
                            uint64_t tmax, bool tiers) {
   c.i_valid = false;
   c.occurrence = 0xFFFFFFFFu;
-  if (last > first && (first < c.res_first || last > c.res_last)) {
+  if (last > first && !c.bases_on_host && (first < c.res_first || last > c.res_last)) {
     throw StateError("the bases of these reads were not uploaded (rvn_reads_upload_range)");
   }
   // (an asynchronous upload: every chunk's bases are there before the first sketch)
   WaitUpload(c);
   const std::vector<uint32_t> cuts = ChunkCuts(c, first, last, chunk);
+  // staged bases: each sketch is followed by the copy of the range sketched next - the next
+  // chunk, after sweep 1 the first chunk again, after the last the range the caller named
+  const uint32_t after_first = c.bases_next_first, after_last = c.bases_next_last;
+  auto stage_next = [&](size_t i, bool sweep1) {
+    if (i + 2 < cuts.size()) {
+      BasesNext(c, cuts[i + 1], cuts[i + 2]);
+    } else if (sweep1) {
+      BasesNext(c, cuts[0], cuts[1]);
+    } else {
+      BasesNext(c, after_first, after_last);
+    }
+  };
   const uint32_t nr = last - first;
   const bool k32 = 2 * c.prm.k <= 30;
   const int key_bits = static_cast<int>(2 * c.prm.k);
@@ -914,6 +926,7 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
     uint64_t* q_org = c.i_org_alt.reserve(cap + 1);
     uint64_t n = 0;
     for (size_t i = 0; i + 1 < cuts.size(); ++i) {
+      stage_next(i, false);
       EnsureMicromizers(c, cuts[i], cuts[i + 1]);  // (sketches the chunk)
       TimerBegin(c, "sketch_tiers");
       if (c.q_n) {
@@ -944,6 +957,7 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
   c.h_jt_off.assign(1, 0);
   for (size_t i = 0; i + 1 < cuts.size(); ++i) {
     const uint32_t r0 = cuts[i], r1 = cuts[i + 1];
+    stage_next(i, true);
     EnsureSketch(c, r0, r1);  // (exactly the chunk: c.s_n and c.s_val are its records)
     EnsureThresholds(c, r0, r1);
     n += c.s_n;
@@ -1012,6 +1026,7 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
   uint64_t n_a = 0, n_b = 0;
   for (size_t i = 0; i + 1 < cuts.size(); ++i) {
     const uint32_t r0 = cuts[i], r1 = cuts[i + 1];
+    stage_next(i, false);
     if (fused) {
       TimerBegin(c, "sketch_tiers");
       uint64_t m_a = 0, m_b = 0;

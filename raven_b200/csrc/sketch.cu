@@ -123,9 +123,11 @@ constexpr uint64_t kStMask = 3ULL << 62;
 // and obtains its output offset from the running prefix of the tiles before it
 // (decoupled look-back on a status array), so records land in (read,
 // position) order without a counting pass. HashT = u32 when 2k <= 30.
+// Both sketch kernels read word w of the set at words[w - word_base]: 0 for the device copy
+// of the whole set, the first word of the staged range for a half of the staging window.
 template <typename HashT>
 __global__ void __launch_bounds__(kSketchThreads)
-SketchKernel(const uint64_t* __restrict__ words,
+SketchKernel(const uint64_t* __restrict__ words, uint64_t word_base,
              const uint64_t* __restrict__ woff,
              const uint32_t* __restrict__ lens,
              const uint32_t* __restrict__ ids,
@@ -183,7 +185,7 @@ SketchKernel(const uint64_t* __restrict__ words,
   const uint32_t he = min(q1 + halo, L);
 
   // ---- stage the packed words this tile touches ----
-  const uint64_t* rw = words + woff[r];
+  const uint64_t* rw = words + (woff[r] - word_base);
   const uint32_t nwords = static_cast<uint32_t>(woff[r + 1] - woff[r]);
   const uint32_t w_lo = hs >> 5;
   const uint32_t w_hi = ((he - 1 + k - 1) >> 5) + 2;  // one spare for the funnel
@@ -417,7 +419,8 @@ enum SketchOut { kSketchPerTile = 0, kSketchTiers = 1, kSketchAppend = 2 };
 
 template <int W, int kOut>
 __global__ void __launch_bounds__(kSketchThreads, 4)
-SketchFastKernel(const uint64_t* __restrict__ words, const uint64_t* __restrict__ woff,
+SketchFastKernel(const uint64_t* __restrict__ words, uint64_t word_base,
+                 const uint64_t* __restrict__ woff,
                  const uint32_t* __restrict__ lens, const uint32_t* __restrict__ ids,
                  const uint64_t* __restrict__ tile_off,
                  const uint32_t* __restrict__ tile_read, uint32_t first_read,
@@ -479,7 +482,7 @@ SketchFastKernel(const uint64_t* __restrict__ words, const uint64_t* __restrict_
       sh_wlo[threadIdx.x] = w_lo;
       sh_wn[threadIdx.x] = w_hi - w_lo;
       sh_wvalid[threadIdx.x] = nwords > w_lo ? nwords - w_lo : 0;
-      sh_wsrc[threadIdx.x] = words + wb + w_lo;
+      sh_wsrc[threadIdx.x] = words + (wb - word_base) + w_lo;
     }
     if (threadIdx.x == 0) sh_group = grp;
   }
@@ -905,7 +908,177 @@ size_t SketchSmemBytes(uint32_t w, size_t hash_bytes) {
   return max_words * 8 + span * hash_bytes + 4 + 34 * 4 + span + 16;
 }
 
+// ---- the staging window (option host_bases) ----
+// A staged range of 1024 reads or more is copied in this many pieces of about equal words,
+// cut at read boundaries: the sketch of the reads of a piece starts when it has arrived.
+constexpr uint32_t kStagePieces = 8;
+
+void EnsureCopyStream(Ctx& c) {
+  if (c.copy_stream) return;
+  RVN_CUDA(cudaStreamCreateWithFlags(&c.copy_stream, cudaStreamNonBlocking));
+  RVN_CUDA(cudaEventCreateWithFlags(&c.up_fence, cudaEventDisableTiming));
+}
+
+// the half that holds every read of [first, last), -1 = none
+int HalfWith(const Ctx& c, uint32_t first, uint32_t last) {
+  for (int i = 0; i < 2; ++i) {
+    const BaseHalf& h = c.bh[i];
+    if (h.valid && h.first <= first && last <= h.last) return i;
+  }
+  return -1;
+}
+
+// Copy of the words of reads [first, last) (src: their words on the host, from the first
+// read's first word) into half i, on the copy stream behind every kernel that read the half.
+void StageRange(Ctx& c, int i, uint32_t first, uint32_t last, const uint64_t* src) {
+  BaseHalf& h = c.bh[i];
+  const uint64_t w0 = c.h_woff[first], w1 = c.h_woff[last];
+  h.valid = false;
+  EnsureCopyStream(c);
+  if (!h.used) RVN_CUDA(cudaEventCreateWithFlags(&h.used, cudaEventDisableTiming));
+  if (w1 - w0 + 2 > h.words.cap) {  // (growth frees the buffer: its readers must be done)
+    if (h.used_recorded) RVN_CUDA(cudaEventSynchronize(h.used));
+    RVN_CUDA(cudaStreamSynchronize(c.copy_stream));
+    h.words.reserve(w1 - w0 + 2);
+  }
+  if (h.used_recorded) RVN_CUDA(cudaStreamWaitEvent(c.copy_stream, h.used, 0));
+  const uint32_t pieces = last - first >= 1024 ? kStagePieces : 1;
+  while (h.events.size() < pieces) {
+    cudaEvent_t ev;
+    RVN_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    h.events.push_back(ev);
+  }
+  h.read_end.clear();
+  uint32_t r_prev = first;
+  for (uint32_t p = 1; p <= pieces && r_prev < last; ++p) {
+    const uint64_t target = w0 + (w1 - w0) * p / pieces;
+    uint32_t r = static_cast<uint32_t>(
+        std::lower_bound(c.h_woff.begin() + r_prev + 1, c.h_woff.begin() + last + 1, target) -
+        c.h_woff.begin());
+    if (p == pieces) r = last;
+    const uint64_t a = c.h_woff[r_prev], b = c.h_woff[r];
+    if (b > a) {
+      RVN_CUDA(cudaMemcpyAsync(h.words.get() + (a - w0), src + (a - w0), (b - a) * 8,
+                               cudaMemcpyHostToDevice, c.copy_stream));
+    }
+    RVN_CUDA(cudaEventRecord(h.events[h.read_end.size()], c.copy_stream));
+    h.read_end.push_back(r);
+    r_prev = r;
+  }
+  h.pieces = static_cast<uint32_t>(h.read_end.size());
+  h.first = first;
+  h.last = last;
+  h.valid = true;
+}
+
+// the context's stream waits for piece p of v; with staged bases, phase "stage_bases" is
+// that wait: the copy time no kernel hid
+void WaitPiece(Ctx& c, const BaseView& v, uint32_t p) {
+  if (v.half >= 0) TimerBegin(c, "stage_bases");
+  RVN_CUDA(cudaStreamWaitEvent(c.stream, v.events[p], 0));
+  if (v.half >= 0) TimerEnd(c);
+}
+
+void WaitAllPieces(Ctx& c, const BaseView& v) {
+  if (v.pieces) WaitPiece(c, v, v.pieces - 1);
+}
+
+// The n_groups groups of a SketchFastKernel launch over reads [first, last), in pieces: the
+// groups of the reads a piece of v completes behind that piece's event (groups take tickets,
+// and the look-back chain runs on across launches). launch(grid) launches one piece.
+template <typename F>
+void LaunchFastPieces(Ctx& c, const BaseView& v, uint32_t first, uint32_t last,
+                      uint64_t n_groups, F&& launch) {
+  uint64_t launched = 0;
+  const uint32_t pieces = v.pieces ? v.pieces : 1;
+  for (uint32_t p = 0; p < pieces; ++p) {
+    uint64_t upto = n_groups;
+    if (v.pieces) {
+      WaitPiece(c, v, p);
+      if (p + 1 < pieces) {
+        const uint32_t r = std::min(std::max(v.read_end[p], first), last);
+        upto = (c.h_tile_off[r] - c.h_tile_off[first]) / kFastGroup;
+      }
+    }
+    if (upto <= launched) continue;
+    launch(static_cast<unsigned>(upto - launched));
+    RVN_LAUNCH_CHECK();
+    launched = upto;
+    ++c.launches;
+  }
+}
+
 }  // namespace
+
+BaseView SketchBases(Ctx& c, uint32_t first, uint32_t last) {
+  BaseView v;
+  if (!c.bases_on_host) {
+    if (first < last && (first < c.res_first || last > c.res_last)) {
+      throw StateError("the bases of these reads were not uploaded (rvn_reads_upload_range)");
+    }
+    v.words = c.d_words.get();
+    if (c.up_pending) {  // (an asynchronous upload in flight: its chunks are the pieces)
+      v.events = c.up_events.data();
+      v.read_end = c.up_read_end.data();
+      v.pieces = c.up_chunks;
+      c.up_pending = false;
+    }
+    return v;
+  }
+  int i = HalfWith(c, first, last);
+  if (i < 0) {
+    i = 1 - c.bh_cur;
+    StageRange(c, i, first, last, c.h_words.get() + c.h_woff[first]);
+  }
+  c.bh_cur = i;
+  const BaseHalf& h = c.bh[i];
+  v.words = h.words.get();
+  v.base = c.h_woff[h.first];
+  v.events = h.events.data();
+  v.read_end = h.read_end.data();
+  v.pieces = h.pieces;
+  v.half = i;
+  return v;
+}
+
+void BasesLaunched(Ctx& c, const BaseView& v) {
+  if (v.half < 0) return;
+  BaseHalf& h = c.bh[v.half];
+  RVN_CUDA(cudaEventRecord(h.used, c.stream));
+  h.used_recorded = true;
+  const uint32_t a = c.bases_next_first, b = c.bases_next_last;
+  c.bases_next_first = c.bases_next_last = 0;
+  if (a < b && b <= c.n_reads && HalfWith(c, a, b) < 0) {
+    StageRange(c, 1 - v.half, a, b, c.h_words.get() + c.h_woff[a]);
+  }
+}
+
+void BasesNext(Ctx& c, uint32_t first, uint32_t last) {
+  if (!c.bases_on_host) return;
+  c.bases_next_first = first;
+  c.bases_next_last = last;
+}
+
+void StageExternalBases(Ctx& c, uint32_t n, const uint64_t* words) {
+  StageRange(c, 1 - c.bh_cur, n, n + 1, words);
+}
+
+void DropStagedBases(Ctx& c, uint32_t from, bool release) {
+  for (BaseHalf& h : c.bh) {
+    if (h.valid && h.last > from) h.valid = false;
+    if (release && h.words.cap) {
+      if (h.used_recorded) RVN_CUDA(cudaEventSynchronize(h.used));
+      if (c.copy_stream) RVN_CUDA(cudaStreamSynchronize(c.copy_stream));
+      h.words.release();
+      h.valid = false;
+    }
+  }
+  c.bases_next_first = c.bases_next_last = 0;
+}
+
+uint64_t StagedBaseBytes(const Ctx& c) {
+  return (c.bh[0].words.cap + c.bh[1].words.cap) * sizeof(uint64_t);
+}
 
 void WaitUpload(Ctx& c) {
   if (!c.up_pending) return;
@@ -952,7 +1125,7 @@ void EnsureTiles(Ctx& c) {
 
 void EnsureSketch(Ctx& c, uint32_t first, uint32_t last) {
   if (c.s_valid && c.s_first == first && c.s_last == last) return;
-  if (first < last && (first < c.res_first || last > c.res_last)) {
+  if (first < last && !c.bases_on_host && (first < c.res_first || last > c.res_last)) {
     throw StateError("the bases of these reads were not uploaded (rvn_reads_upload_range)");
   }
   EnsureTiles(c);
@@ -984,54 +1157,41 @@ void EnsureSketch(Ctx& c, uint32_t first, uint32_t last) {
     uint64_t* tout = c.tile_out.reserve(n_tiles + 1);
     uint64_t* status = c.tile_status.reserve(n_tiles + 2);
     unsigned int* ticket = reinterpret_cast<unsigned int*>(status + n_tiles);
+    // (an asynchronous upload or a staged range still in flight: the fast kernel starts on
+    // the pieces that have arrived, the others wait for all of them)
+    const BaseView v = SketchBases(c, first, last);
     for (int attempt = 0; attempt < 2; ++attempt) {
       uint64_t* val = c.s_val.reserve(k32 ? cap / 2 + 1 : cap);
       uint64_t* org = c.s_org.reserve(cap);
       RVN_CUDA(cudaMemsetAsync(status, 0, (n_tiles + 2) * sizeof(uint64_t), c.stream));
-      if (!(k32 && c.prm.w == 5)) WaitUpload(c);
       if (k32 && c.prm.w == 5) {  // raven's default window: the fast kernel
         // (status words of this kernel: one per group of kFastGroup tiles)
         const uint64_t n_groups = (n_tiles + kFastGroup - 1) / kFastGroup;
-        // An asynchronous upload still in flight: the groups of the reads a chunk
-        // completes are launched behind that chunk's event (groups take tickets, and
-        // the look-back chain runs on across launches)
-        uint64_t launched = 0;
-        const uint32_t pieces = c.up_pending ? c.up_chunks : 1;
-        for (uint32_t p = 0; p < pieces; ++p) {
-          uint64_t upto = n_groups;
-          if (c.up_pending) {
-            RVN_CUDA(cudaStreamWaitEvent(c.stream, c.up_events[p], 0));
-            if (p + 1 < pieces) {
-              const uint32_t r = std::min(std::max(c.up_read_end[p], first), last);
-              upto = (c.h_tile_off[r] - c.h_tile_off[first]) / kFastGroup;
-            }
-          }
-          if (upto <= launched) continue;
-          SketchFastKernel<5, kSketchPerTile><<<static_cast<unsigned>(upto - launched), kSketchThreads, 0,
-                                       c.stream>>>(
-              c.d_words.get(), c.d_woff.get(), c.d_len.get(), c.d_ids.get(),
+        LaunchFastPieces(c, v, first, last, n_groups, [&](unsigned grid) {
+          SketchFastKernel<5, kSketchPerTile><<<grid, kSketchThreads, 0, c.stream>>>(
+              v.words, v.base, c.d_woff.get(), c.d_len.get(), c.d_ids.get(),
               c.d_tile_off.get(), c.d_tile_read.get(), first, last, c.prm.k, ticket, status, tout,
               n_tiles, cap, reinterpret_cast<uint32_t*>(val), org, 0u, nullptr, 0, nullptr, 0);
-          launched = upto;
-          ++c.launches;
-        }
+        });
         --c.launches;  // (counted once more below)
-        c.up_pending = false;
       } else if (k32) {
+        WaitAllPieces(c, v);
         SketchKernel<uint32_t><<<static_cast<unsigned>(n_tiles), kSketchThreads, smem,
                                  c.stream>>>(
-            c.d_words.get(), c.d_woff.get(), c.d_len.get(), c.d_ids.get(),
+            v.words, v.base, c.d_woff.get(), c.d_len.get(), c.d_ids.get(),
             c.d_tile_off.get(), first, last, c.prm.k, c.prm.w, ticket, status, tout,
             n_tiles, cap, reinterpret_cast<uint32_t*>(val), org);
       } else {
+        WaitAllPieces(c, v);
         SketchKernel<uint64_t><<<static_cast<unsigned>(n_tiles), kSketchThreads, smem,
                                  c.stream>>>(
-            c.d_words.get(), c.d_woff.get(), c.d_len.get(), c.d_ids.get(),
+            v.words, v.base, c.d_woff.get(), c.d_len.get(), c.d_ids.get(),
             c.d_tile_off.get(), first, last, c.prm.k, c.prm.w, ticket, status, tout,
             n_tiles, cap, val, org);
       }
       RVN_LAUNCH_CHECK();
       ++c.launches;
+      BasesLaunched(c, v);
       total = ReadU64(c, tout + n_tiles);
       if (total <= cap) break;
       cap = total;  // denser than expected: once more with the exact size
@@ -1062,7 +1222,7 @@ bool SketchTiersFused(const Ctx& c) { return 2 * c.prm.k <= 30 && c.prm.w == 5; 
 void SketchTiers(Ctx& c, uint32_t first, uint32_t last, uint32_t limit, uint32_t* a_val,
                  uint64_t* a_org, uint64_t cap_a, uint32_t* b_val, uint64_t cap_b,
                  uint64_t* n_a, uint64_t* n_b) {
-  if (first < last && (first < c.res_first || last > c.res_last)) {
+  if (first < last && !c.bases_on_host && (first < c.res_first || last > c.res_last)) {
     throw StateError("the bases of these reads were not uploaded (rvn_reads_upload_range)");
   }
   EnsureTiles(c);
@@ -1070,6 +1230,7 @@ void SketchTiers(Ctx& c, uint32_t first, uint32_t last, uint32_t limit, uint32_t
   *n_a = *n_b = 0;
   const uint64_t n_tiles = c.h_tile_off[last] - c.h_tile_off[first];
   if (n_tiles == 0) return;
+  const BaseView v = SketchBases(c, first, last);
   if (n_tiles >= (1ULL << 31)) throw LimitError("too many sketch tiles");
   const uint64_t n_groups = (n_tiles + kFastGroup - 1) / kFastGroup;
   uint64_t* tout = c.tile_out.reserve(4);
@@ -1078,12 +1239,13 @@ void SketchTiers(Ctx& c, uint32_t first, uint32_t last, uint32_t limit, uint32_t
   uint64_t* status_b = status + n_groups + 1;
   unsigned int* ticket = reinterpret_cast<unsigned int*>(status_b + n_groups + 1);
   RVN_CUDA(cudaMemsetAsync(status, 0, (2 * (n_groups + 1) + 2) * sizeof(uint64_t), c.stream));
-  SketchFastKernel<5, kSketchTiers><<<static_cast<unsigned>(n_groups), kSketchThreads, 0, c.stream>>>(
-      c.d_words.get(), c.d_woff.get(), c.d_len.get(), c.d_ids.get(), c.d_tile_off.get(),
-      c.d_tile_read.get(), first, last, c.prm.k, ticket, status, tout, n_tiles, cap_a, a_val,
-      a_org, limit, status_b, cap_b, b_val, 0);
-  RVN_LAUNCH_CHECK();
-  ++c.launches;
+  LaunchFastPieces(c, v, first, last, n_groups, [&](unsigned grid) {
+    SketchFastKernel<5, kSketchTiers><<<grid, kSketchThreads, 0, c.stream>>>(
+        v.words, v.base, c.d_woff.get(), c.d_len.get(), c.d_ids.get(), c.d_tile_off.get(),
+        c.d_tile_read.get(), first, last, c.prm.k, ticket, status, tout, n_tiles, cap_a, a_val,
+        a_org, limit, status_b, cap_b, b_val, 0);
+  });
+  BasesLaunched(c, v);
   uint64_t* h = c.pin64.reserve(8);
   RVN_CUDA(cudaMemcpyAsync(h, tout, 2 * sizeof(uint64_t), cudaMemcpyDeviceToHost, c.stream));
   RVN_CUDA(cudaStreamSynchronize(c.stream));
@@ -1093,7 +1255,7 @@ void SketchTiers(Ctx& c, uint32_t first, uint32_t last, uint32_t limit, uint32_t
 
 void SketchAppend(Ctx& c, uint32_t first, uint32_t last, uint32_t* out_val, uint64_t* out_org,
                   uint64_t base, uint64_t cap) {
-  if (first < last && (first < c.res_first || last > c.res_last)) {
+  if (first < last && !c.bases_on_host && (first < c.res_first || last > c.res_last)) {
     throw StateError("the bases of these reads were not uploaded (rvn_reads_upload_range)");
   }
   EnsureTiles(c);
@@ -1110,13 +1272,14 @@ void SketchAppend(Ctx& c, uint32_t first, uint32_t last, uint32_t* out_val, uint
   uint64_t* status = c.tile_status.reserve(n_groups + 2);
   unsigned int* ticket = reinterpret_cast<unsigned int*>(status + n_groups + 1);
   RVN_CUDA(cudaMemsetAsync(status, 0, (n_groups + 2) * sizeof(uint64_t), c.stream));
-  SketchFastKernel<5, kSketchAppend><<<static_cast<unsigned>(n_groups), kSketchThreads, 0,
-                                       c.stream>>>(
-      c.d_words.get(), c.d_woff.get(), c.d_len.get(), c.d_ids.get(), c.d_tile_off.get(),
-      c.d_tile_read.get(), first, last, c.prm.k, ticket, status, tout, n_tiles, cap, out_val,
-      out_org, 0u, nullptr, 0, nullptr, base);
-  RVN_LAUNCH_CHECK();
-  ++c.launches;
+  const BaseView v = SketchBases(c, first, last);
+  LaunchFastPieces(c, v, first, last, n_groups, [&](unsigned grid) {
+    SketchFastKernel<5, kSketchAppend><<<grid, kSketchThreads, 0, c.stream>>>(
+        v.words, v.base, c.d_woff.get(), c.d_len.get(), c.d_ids.get(), c.d_tile_off.get(),
+        c.d_tile_read.get(), first, last, c.prm.k, ticket, status, tout, n_tiles, cap, out_val,
+        out_org, 0u, nullptr, 0, nullptr, base);
+  });
+  BasesLaunched(c, v);
 }
 
 uint64_t SketchAppendTotal(Ctx& c) { return ReadU64(c, c.tile_out.get()); }

@@ -81,6 +81,30 @@ double IndexFootprint(const Ctx& c, const std::vector<Batch>& batches, uint64_t 
                                 kFlushBytesPerBase * static_cast<double>(flush_bases));
 }
 
+// Words of the largest read range a pass sketches: an index batch, or one chunk of it
+// (chunk > 0), or a query flush.
+uint64_t LargestSketchWords(const Ctx& c, const std::vector<Batch>& batches, uint64_t chunk) {
+  uint64_t words = 0;
+  auto range = [&](uint32_t a, uint32_t b) { words = std::max(words, c.h_woff[b] - c.h_woff[a]); };
+  for (const Batch& b : batches) {
+    if (chunk) {
+      const std::vector<uint32_t> cuts = ChunkCuts(c, b.j, b.end, chunk);
+      for (size_t i = 0; i + 1 < cuts.size(); ++i) range(cuts[i], cuts[i + 1]);
+    } else {
+      range(b.j, b.end);
+    }
+    for (const auto& f : b.flushes) range(f.first, f.second);
+  }
+  return words;
+}
+
+// Device bytes of the packed bases during a pass: the whole set, or with the bases on the
+// host the two halves of the staging window, each as large as the largest range sketched.
+double BasesBytes(const Ctx& c, const std::vector<Batch>& batches, uint64_t chunk, bool host) {
+  if (!host) return 8.0 * c.n_words;
+  return 2.0 * 8.0 * static_cast<double>(LargestSketchWords(c, batches, chunk));
+}
+
 // Estimated memory of a stage-1 pass over the uploaded reads, in bytes.
 struct Footprint {
   double resident = 0;         // device, resident pass
@@ -98,9 +122,10 @@ struct Footprint {
 // - windowed, on the device: the same per slot of the largest window, with kmax
 //   (at least 1) records per list row; on the host: the rows, counts and piles of
 //   all reads.
-// chunk: the index build's chunk size (0: one-shot), see IndexFootprint
+// chunk: the index build's chunk size (0: one-shot), see IndexFootprint; host: the bases
+// are on the host (BasesBytes)
 Footprint Stage1Footprint(const Ctx& c, const std::vector<Batch>& batches, uint64_t kmax,
-                          uint64_t chunk) {
+                          uint64_t chunk, bool host) {
   const uint32_t n = c.n_reads;
   const std::vector<uint64_t>& off = c.h_pile_off;
   const double bins = static_cast<double>(off[n]);
@@ -115,7 +140,8 @@ Footprint Stage1Footprint(const Ctx& c, const std::vector<Batch>& batches, uint6
       window = std::max(window, 6.0 * wbins + 4.0 * slots + slots * stride * list_bytes);
     }
   }
-  const double reads = 8.0 * c.n_words + 32.0 * n + IndexFootprint(c, batches, chunk);
+  const double reads =
+      BasesBytes(c, batches, chunk, host) + 32.0 * n + IndexFootprint(c, batches, chunk);
   const double kept = std::min(static_cast<double>(kmax), n > 0 ? n - 1.0 : 0.0);
   Footprint f;
   f.resident = reads + 6.0 * bins + 4.0 * n + n * kept * list_bytes;
@@ -144,7 +170,7 @@ uint64_t IndexChunk(const Ctx& c, double one_shot) {
 
 // a stage-1 pass with one-shot builds: resident, or windowed (max_overlaps permitting)
 double Stage1OneShot(const Ctx& c, const std::vector<Batch>& batches, uint64_t kmax) {
-  const Footprint f = Stage1Footprint(c, batches, kmax, 0);
+  const Footprint f = Stage1Footprint(c, batches, kmax, 0, c.bases_on_host);
   return kmax <= kWindowMaxOverlaps ? std::min(f.resident, f.windowed_device) : f.resident;
 }
 
@@ -158,8 +184,9 @@ constexpr double kUntieredIndexBytesPerBase = 8.9;
 double MinimizeFootprint(const Ctx& c, uint32_t first, uint32_t last, uint64_t chunk) {
   const double bb = static_cast<double>(ReadBases(c, first, last));
   const double sketched = chunk ? std::min(bb, static_cast<double>(chunk)) : bb;
-  return 8.0 * c.n_words + 32.0 * c.n_reads + kUntieredIndexBytesPerBase * bb +
-         kChunkSketchBytesPerBase * sketched;
+  const std::vector<Batch> batch{Batch{first, last, {}}};
+  return BasesBytes(c, batch, chunk, c.bases_on_host) + 32.0 * c.n_reads +
+         kUntieredIndexBytesPerBase * bb + kChunkSketchBytesPerBase * sketched;
 }
 
 // rvn_map works its query range in flushes, as the reference cuts its queries
@@ -177,7 +204,8 @@ uint64_t MapFlushBases(const Ctx& c, uint64_t range_bases, bool join) {
   // a flush can grow into the free memory and into every buffer of the context but the
   // reads and the index
   auto bytes = [](const auto& b) { return static_cast<double>(b.cap * sizeof(*b.p)); };
-  const double fixed = bytes(c.d_words) + bytes(c.i_val) + bytes(c.i_org) + bytes(c.i_val_alt) +
+  const double fixed = bytes(c.d_words) + static_cast<double>(StagedBaseBytes(c)) +
+                       bytes(c.i_val) + bytes(c.i_org) + bytes(c.i_val_alt) +
                        bytes(c.i_org_alt) + bytes(c.i_bucket) + bytes(c.j_packed);
   const double room = UsableMemory(c, 0) - fixed;
   const double flush = room / (join ? kJoinFlushBytesPerBase : kFlushBytesPerBase);
@@ -193,7 +221,7 @@ uint64_t MapFlushBases(const Ctx& c, uint64_t range_bases, bool join) {
 bool UseWindow(Ctx& c, const std::vector<Batch>& batches, uint64_t kmax, uint64_t chunk) {
   if (c.stage1_window >= 0) return c.stage1_window != 0;
   if (kmax > kWindowMaxOverlaps) return false;
-  const Footprint f = Stage1Footprint(c, batches, kmax, chunk);
+  const Footprint f = Stage1Footprint(c, batches, kmax, chunk, c.bases_on_host);
   const double budget = UsableMemory(c, c.stage1_window_budget);
   if (f.resident <= budget) return false;
   const double host_free = static_cast<double>(sysconf(_SC_AVPHYS_PAGES)) *
@@ -477,8 +505,13 @@ void MapFlushes(Ctx& c, uint32_t first, uint32_t last, bool avoid_equal, bool av
                     first >= c.i_first && last <= c.i_last;
   const std::vector<uint32_t> cuts =
       ChunkCuts(c, first, last, MapFlushBases(c, ReadBases(c, first, last), join));
+  // staged bases: each probe-path flush's sketch is followed by the copy of the next flush's
+  auto stage_next = [&](size_t i) {
+    if (!join && i + 2 < cuts.size()) BasesNext(c, cuts[i + 1], cuts[i + 2]);
+  };
   if (each) {
     for (size_t i = 0; i + 1 < cuts.size(); ++i) {
+      stage_next(i);
       MapRange(c, cuts[i], cuts[i + 1], avoid_equal, avoid_symmetric, minhash, want_filtered,
                /*fetch=*/false);
       each(cuts[i], cuts[i + 1] - cuts[i]);
@@ -496,6 +529,7 @@ void MapFlushes(Ctx& c, uint32_t first, uint32_t last, bool avoid_equal, bool av
   uint64_t total = 0, f_total = 0;
   for (size_t i = 0; i + 1 < cuts.size(); ++i) {
     const uint32_t r0 = cuts[i], m = cuts[i + 1] - cuts[i];
+    stage_next(i);
     MapRange(c, r0, r0 + m, avoid_equal, avoid_symmetric, minhash, want_filtered,
              /*fetch=*/false);
     TimerBegin(c, "map_flush");
@@ -672,8 +706,35 @@ void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
   const std::vector<uint32_t> final_reads = FinalReads(batches, n);
   size_t flush = 0;  // index of the flush in the schedule
 
+  // Staged bases: the range sketched after each sketch, copied beside the kernels that read
+  // no bases - the batch's first range (itself, or its first chunk), then the flushes that
+  // probe (those that are not inside the batch, or all of them with minhash), then the
+  // next batch's first range. next_sketch[i]: the first such range from batch i's flushes on.
+  auto probes = [&](const Batch& b, const std::pair<uint32_t, uint32_t>& f) {
+    return !(c.self_join && !minhash && f.first >= b.j && f.second <= b.end);
+  };
+  auto first_range = [&](const Batch& b) {
+    const std::vector<uint32_t> cuts = ChunkCuts(c, b.j, b.end, chunk ? chunk : ~0ULL);
+    return std::make_pair(cuts[0], cuts[1]);
+  };
+  auto stage_after = [&](size_t bi, size_t fi) {  // the range after flush fi - 1 of batch bi
+    if (!c.bases_on_host) return;
+    for (size_t i = fi; i < batches[bi].flushes.size(); ++i) {
+      if (probes(batches[bi], batches[bi].flushes[i])) {
+        BasesNext(c, batches[bi].flushes[i].first, batches[bi].flushes[i].second);
+        return;
+      }
+    }
+    if (bi + 1 < batches.size()) {
+      const auto r = first_range(batches[bi + 1]);
+      BasesNext(c, r.first, r.second);
+    }
+  };
+
   uint64_t tmax = 0;  // largest micromizer value of the reads sketched so far
-  for (const Batch& b : batches) {
+  for (size_t bi = 0; bi < batches.size(); ++bi) {
+    const Batch& b = batches[bi];
+    stage_after(bi, 0);
     // Queries are micromizers only (construct.cc:62): no record above the largest
     // micromizer value of any read so far can be hit - those are counted for the
     // occurrence threshold but stay out of the index (index.cu, tiers)
@@ -692,7 +753,9 @@ void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
     }
     if (win) win->BeginBatch(b);
 
-    for (const auto& f : b.flushes) {
+    for (size_t fi = 0; fi < b.flushes.size(); ++fi) {
+      const auto& f = b.flushes[fi];
+      stage_after(bi, fi + 1);
       MapRange(c, f.first, f.second, true, true, true, false, /*fetch=*/false);
       const uint32_t final = final_reads[flush++];
       if (win) {
@@ -740,11 +803,43 @@ void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
   c.st_piles_on_device = !windowed;
 }
 
+bool UseHostBases(const Ctx& c) {
+  if (c.host_bases >= 0) return c.host_bases != 0;
+  if (c.n_reads == 0) return false;
+  // the windowed, chunked pass of the reference's schedule at its default max_overlaps
+  const std::vector<Batch> batches = Schedule(c, 0, 0);
+  const double usable = UsableMemory(c, c.host_bases_budget);
+  if (Stage1Footprint(c, batches, 32, kAutoIndexChunk, false).windowed_device <= usable) {
+    return false;
+  }
+  return Stage1Footprint(c, batches, 32, kAutoIndexChunk, true).windowed_device <= usable;
+}
+
+void EnsureDeviceBases(Ctx& c) {
+  if (!c.bases_on_host) return;
+  const uint64_t bytes = (c.n_words + 2) * sizeof(uint64_t);
+  const double usable = UsableMemory(c, c.host_bases_budget);
+  if (static_cast<double>(bytes) > usable) {
+    throw LimitError("the packed bases of the whole read set (" + std::to_string(bytes) +
+                     " bytes) do not fit the device (" +
+                     std::to_string(static_cast<uint64_t>(usable)) + " bytes usable)");
+  }
+  RVN_CUDA(cudaStreamSynchronize(c.stream));
+  DropStagedBases(c, 0, /*release=*/true);
+  uint64_t* dw = c.d_words.reserve(c.n_words + 2);
+  RVN_CUDA(cudaMemcpyAsync(dw, c.h_words.get(), c.n_words * sizeof(uint64_t),
+                           cudaMemcpyHostToDevice, c.stream));
+  RVN_CUDA(cudaStreamSynchronize(c.stream));
+  c.bases_on_host = false;
+  c.res_first = 0;
+  c.res_last = c.n_reads;
+}
+
 void Stage1Footprints(const Ctx& c, uint64_t kmax, uint64_t ib, uint64_t qb,
                       uint64_t* resident, uint64_t* windowed_device, uint64_t* windowed_host) {
   const std::vector<Batch> batches = Schedule(c, ib, qb);
-  const Footprint f =
-      Stage1Footprint(c, batches, kmax, IndexChunk(c, Stage1OneShot(c, batches, kmax)));
+  const Footprint f = Stage1Footprint(
+      c, batches, kmax, IndexChunk(c, Stage1OneShot(c, batches, kmax)), c.bases_on_host);
   if (resident) *resident = static_cast<uint64_t>(f.resident);
   if (windowed_device) *windowed_device = static_cast<uint64_t>(f.windowed_device);
   if (windowed_host) *windowed_host = static_cast<uint64_t>(f.windowed_host);

@@ -433,6 +433,22 @@ class Engine:
         self.set_option("stage1_window", mode)
         self.set_option("stage1_window_budget", budget)
 
+    def set_host_bases(self, mode=-1, budget=0):
+        """Where the next upload (without ``resident``) keeps the packed bases: 0 on the
+        device, 1 in a pinned host copy of the context's own (each sketch copies its read
+        range to a device staging window), -1 auto (on the host only when a stage-1 pass at
+        the reference's batch sizes fits the device that way and not otherwise; ``budget``
+        bytes replace the usable device memory when not 0). Same results."""
+        self.set_option("host_bases", mode)
+        self.set_option("host_bases_budget", budget)
+
+    def reads_residency(self):
+        """Where the bases of the current upload live: on_host, and device_word_bytes, the
+        device bytes of packed words held for them (the whole set, or the staging window)."""
+        on, b = C.c_int(0), C.c_uint64(0)
+        self._check(self.lib.rvn_reads_residency(self.h, C.byref(on), C.byref(b)))
+        return dict(on_host=bool(on.value), device_word_bytes=b.value)
+
     def stage1_footprint(self, max_overlaps=32, index_batch_bases=0, query_batch_bases=0):
         """The auto mode's estimates for a stage-1 call over the uploaded reads, in bytes:
         resident (device), windowed_device and windowed_host (pinned)."""
