@@ -8,24 +8,31 @@
 // parity oracle, in oracle/spoa_graph.cpp + oracle/racon_window.cpp.
 //
 // One warp per window, many windows in flight (the graph surgery between two
-// layers is sequential pointer work; occupancy hides its latency):
+// layers is sequential pointer work; occupancy hides its latency). Three kernels
+// share one definition of the graph and of everything but the DP:
 //   * lane 0 keeps the partial order graph (nodes, in/out edge lists in
-//     insertion order, aligned-node sets, per-node sequence counts) in a
-//     per-window scratch slab, extracts the sub-graph a partial layer aligns
-//     to, and sorts it topologically exactly like spoa's DFS;
-//   * all 32 lanes fill the DP rows: coalesced int16 rows, the diagonal
-//     neighbour through a shuffle, and the horizontal gap recurrence
-//     H[i][j] = max(M[j], H[i][j-1] + g) solved as a warp max-scan of
-//     M[j] - j*g (exact in integers);
-//   * lane 0 walks the traceback with spoa's preference (diagonal over
-//     predecessors in in-edge order, then vertical, then horizontal), merges
-//     the layer into the graph, and finally runs the heaviest-bundle consensus
-//     with branch completion and the coverage-based TGS trimming.
+//     insertion order, aligned-node sets, per-node sequence counts) as packed
+//     records in a per-window scratch slab, with one flag byte per node, extracts
+//     the sub-graph a partial layer aligns to, and sorts it topologically exactly
+//     like spoa's DFS;
+//   * all 32 lanes fill the DP rows, and lane 0 walks the traceback with spoa's
+//     preference (diagonal over predecessors in in-edge order, then vertical, then
+//     horizontal). These two steps are each kernel's own: PoaKernelFast
+//     (poa_fast.cuh) keeps rows in registers, for layers of at most 575 bases;
+//     PoaKernel fills coalesced rows, the diagonal neighbour through a shuffle and
+//     the horizontal gap recurrence H[i][j] = max(M[j], H[i][j-1] + g) as a warp
+//     max-scan of M[j] - j*g (exact in integers), with 16-bit (PoaNarrow) or
+//     32-bit (PoaWide) ids;
+//   * lane 0 merges the layer into the graph, and finally runs the heaviest-bundle
+//     consensus with branch completion and the coverage-based TGS trimming.
 // A node's Coverage() (distinct sequence labels on its incident edges) equals
 // the number of sequences (of >= 2 bases) whose path visits it, so a per-node
 // counter replaces spoa's per-edge label lists.
 // No tensor-core work exists here (no dense contraction).
 #include <algorithm>
+#include <cstddef>
+#include <cstring>
+#include <type_traits>
 
 #include "engine.cuh"
 
@@ -33,12 +40,16 @@ namespace rvn {
 
 namespace {
 
-constexpr uint16_t kNone = 0xFFFF;
 constexpr int kPoaStatusOk = 1;        // polished
 constexpr int kPoaStatusChimeric = 2;  // trimming skipped (racon's warning)
 constexpr int kPoaStatusCapacity = 64; // scratch too small: host retries bigger
 constexpr int kPoaStatusInvalid = 128; // bad layer coordinates / letters
 constexpr uint32_t kPoaMaxLayers = 4095;  // kept layers of one window (16-bit order slots)
+
+// the register-row kernel's DP (poa_fast.cuh): kS contiguous columns per lane
+constexpr int kS = 18;
+constexpr uint32_t kFastCols = 32 * kS;  // 576 = longest layer + 1
+constexpr uint32_t kDirStride = 32 * 20; // bytes per direction row (20 per lane)
 
 struct PoaShape {
   uint32_t ncap;   // node capacity
@@ -48,11 +59,12 @@ struct PoaShape {
   uint32_t width;  // DP row stride (lmax + 1 rounded up to 32)
 };
 
-// The two widths of the generic kernel: one definition of PoaKernel and its helpers,
-// instantiated for each.
+// The two widths of the graph and the consensus: one definition of each, instantiated
+// for both.
 //   PoaNarrow: 16-bit node, edge and order ids and coverage, int16 layer positions and
 //     DP cells - every window of the default contract (65000 window bases, 32000 layer
-//     bases, 4095 layers, 65000 nodes or edges, the int16 score guard).
+//     bases, 4095 layers, 65000 nodes or edges, the int16 score guard). Both the
+//     register-row kernel and PoaKernel<PoaNarrow> use it.
 //   PoaWide: 32-bit ids, positions and coverage, int32 cells - the windows past those
 //     limits (option "poa_wide"); its order slots are sized per launch.
 struct PoaNarrow {
@@ -85,49 +97,92 @@ struct PoaWide {
   __host__ __device__ static uint32_t Layers(const Shape& s) { return s.layers; }
 };
 
-// byte offsets of the arrays inside one window's scratch slab
+// Nodes and edges as packed records, so one load reads what the surgery needs of a node
+// or an edge: 8 bytes each for 16-bit ids, 16 bytes for 32-bit ids.
+template <class Id>
+struct alignas(4 * sizeof(Id)) PoaNodeA {  // in-edge list, out-edge list, letter
+  Id in_head, in_tail, out_head;
+  uint8_t code, n_aligned;
+};
+template <class Id>
+struct alignas(4 * sizeof(Id)) PoaNodeB {  // aligned nodes (one per other letter), coverage
+  Id aligned[3];
+  Id cov;
+};
+template <class Id>
+struct alignas(4 * sizeof(Id)) PoaEdge {  // adjacency lists in insertion order
+  Id tail, head, next_in, next_out;
+};
+static_assert(sizeof(PoaNodeA<uint16_t>) == 8 && offsetof(PoaNodeA<uint16_t>, code) == 6 &&
+              sizeof(PoaNodeB<uint16_t>) == 8 && sizeof(PoaEdge<uint16_t>) == 8,
+              "16-bit records are 8 bytes");
+static_assert(sizeof(PoaNodeA<uint32_t>) == 16 && sizeof(PoaNodeB<uint32_t>) == 16 &&
+              sizeof(PoaEdge<uint32_t>) == 16, "32-bit records are 16 bytes");
+
+// one vector load / store for a whole record
+template <class T>
+using PoaVec = typename std::conditional<sizeof(T) == 8, uint2, uint4>::type;
+template <class T>
+__device__ __forceinline__ T Ld(const T* p) {
+  const PoaVec<T> v = *reinterpret_cast<const PoaVec<T>*>(p);
+  T t;
+  memcpy(&t, &v, sizeof t);
+  return t;
+}
+template <class T>
+__device__ __forceinline__ void St(T* p, const T& t) {
+  PoaVec<T> v;
+  memcpy(&v, &t, sizeof v);
+  *reinterpret_cast<PoaVec<T>*>(p) = v;
+}
+template <class Id>
+__device__ __forceinline__ uint32_t AlignedAt(const PoaNodeB<Id>& b, uint32_t i) {
+  return i == 0 ? b.aligned[0] : i == 1 ? b.aligned[1] : b.aligned[2];
+}
+
+// node flags: topological mark (0 new, 1 on the stack, 2 done), ignored by the sort,
+// inside the (sub)graph of the layer, sink of that (sub)graph
+constexpr uint8_t kMarks = 3, kIgnored = 4, kInSub = 8, kSink = 16;
+
+// Byte offsets of the arrays inside one window's scratch slab: the graph's, then the
+// kernel's own. PoaKernelFast keeps flags, r2n and n2r in shared memory and has its DP
+// matrix at kFastCols columns with one direction byte per cell; PoaKernel keeps them
+// here and has its matrix at shape.width columns.
 struct PoaLayout {
-  size_t code, n_aligned, marks, ignored, in_sub, sink;
-  size_t in_head, in_tail, out_head, aligned, cov, r2n, n2r, stack, order;
-  size_t e_tail, e_head, e_next_in, e_next_out, e_weight;
-  size_t aln_node, aln_pos, pred, score, H, bytes;
+  size_t node_a, node_b, edge, edge_w, stack, order, aln_node, aln_pos, pred, score;
+  size_t flags, r2n, n2r, H, DIR, bytes;
 };
 
 template <class W>
-__host__ __device__ inline PoaLayout MakePoaLayout(const typename W::Shape& s) {
-  constexpr size_t id = sizeof(typename W::Id), pos = sizeof(typename W::Pos);
-  PoaLayout L;
+__host__ __device__ inline PoaLayout MakePoaLayout(const typename W::Shape& s, bool fast) {
+  using Id = typename W::Id;
+  constexpr size_t id = sizeof(Id), pos = sizeof(typename W::Pos);
+  PoaLayout L{};
   size_t o = 0;
   auto take = [&](size_t bytes) {
     size_t at = o;
     o += (bytes + 15) & ~size_t(15);
     return at;
   };
-  L.code = take(s.ncap);
-  L.n_aligned = take(s.ncap);
-  L.marks = take(s.ncap);
-  L.ignored = take(s.ncap);
-  L.in_sub = take(s.ncap);
-  L.sink = take(s.ncap);
-  L.in_head = take(id * s.ncap);
-  L.in_tail = take(id * s.ncap);
-  L.out_head = take(id * s.ncap);
-  L.aligned = take(id * 3 * s.ncap);
-  L.cov = take(id * s.ncap);
-  L.r2n = take(id * s.ncap);
-  L.n2r = take(id * s.ncap);
+  L.node_a = take(sizeof(PoaNodeA<Id>) * s.ncap);
+  L.node_b = take(sizeof(PoaNodeB<Id>) * s.ncap);
+  L.edge = take(sizeof(PoaEdge<Id>) * s.ecap);
+  L.edge_w = take(4ULL * s.ecap);
   L.stack = take(id * 4 * s.ncap);
   L.order = take(id * (W::Layers(s) + 1));
-  L.e_tail = take(id * s.ecap);
-  L.e_head = take(id * s.ecap);
-  L.e_next_in = take(id * s.ecap);
-  L.e_next_out = take(id * s.ecap);
-  L.e_weight = take(4ULL * s.ecap);
   L.aln_node = take(pos * (s.ncap + s.lmax + 2));
   L.aln_pos = take(pos * (s.ncap + s.lmax + 2));
   L.pred = take(4ULL * s.ncap);
   L.score = take(8ULL * s.ncap);
-  L.H = take(sizeof(typename W::Cell) * s.rows * s.width);
+  if (fast) {
+    L.H = take(sizeof(typename W::Cell) * s.rows * kFastCols);
+    L.DIR = take(1ULL * s.rows * kDirStride);
+  } else {
+    L.flags = take(s.ncap);
+    L.r2n = take(id * s.ncap);
+    L.n2r = take(id * s.ncap);
+    L.H = take(sizeof(typename W::Cell) * s.rows * s.width);
+  }
   L.bytes = o;
   return L;
 }
@@ -135,15 +190,20 @@ __host__ __device__ inline PoaLayout MakePoaLayout(const typename W::Shape& s) {
 template <class W>
 struct PoaGraph {
   using Id = typename W::Id;
-  uint8_t *code, *n_aligned, *marks, *ignored, *in_sub, *sink;
-  Id *in_head, *in_tail, *out_head, *aligned, *cov, *r2n, *n2r, *stack, *order;
-  Id *e_tail, *e_head, *e_next_in, *e_next_out;
-  int32_t* e_weight;
+  PoaNodeA<Id>* node_a;
+  PoaNodeB<Id>* node_b;
+  PoaEdge<Id>* edge;
+  int32_t* edge_w;
+  Id *stack, *order;
   typename W::Pos *aln_node, *aln_pos;
   int32_t* pred;
   long long* score;
+  uint8_t* flags;
+  Id *r2n, *n2r;  // rank -> node and node -> rank of the last TopoSort
   typename W::Cell* H;
+  uint8_t* DIR;  // PoaKernelFast only
   uint32_t n_nodes, n_edges, ncap, ecap, stack_cap;
+  uint32_t rows;  // of the layer's (sub)graph
   bool overflow;
 };
 
@@ -189,7 +249,7 @@ template <class Order>
 __device__ uint32_t OrderLayers(Order* order, const uint64_t* seq_off,
                                 const uint32_t* seq_begin, const uint32_t* seq_end,
                                 uint32_t s0, uint32_t s1, uint32_t L0, uint32_t lmax,
-                                uint32_t max_layers = kPoaMaxLayers) {
+                                uint32_t max_layers) {
   uint32_t n = 0;
   for (uint32_t s = s0 + 1; s < s1; ++s) {
     if (!LayerKept(seq_off, seq_begin, seq_end, s)) continue;
@@ -207,52 +267,65 @@ __device__ uint32_t OrderLayers(Order* order, const uint64_t* seq_off,
 }
 
 template <class W>
-__device__ typename W::Id AddNode(PoaGraph<W>& g, uint32_t code) {
+__device__ uint32_t AddNode(PoaGraph<W>& g, uint32_t code) {
   if (g.n_nodes >= g.ncap) {
     g.overflow = true;
     return 0;
   }
   const uint32_t v = g.n_nodes++;
-  g.code[v] = static_cast<uint8_t>(code);
-  g.n_aligned[v] = 0;
-  g.in_head[v] = g.in_tail[v] = g.out_head[v] = W::kNone;
-  g.cov[v] = 0;
-  return static_cast<typename W::Id>(v);
+  St(g.node_a + v, PoaNodeA<typename W::Id>{W::kNone, W::kNone, W::kNone,
+                                            static_cast<uint8_t>(code), 0});
+  St(g.node_b + v, PoaNodeB<typename W::Id>{});
+  return v;
 }
 
 // spoa Graph::AddEdge: bump the weight of an existing edge or append a new
 // one at the END of both adjacency lists (insertion order is observable)
 template <class W>
-__device__ void AddEdge(PoaGraph<W>& g, typename W::Id tail, typename W::Id head, int32_t w) {
+__device__ void AddEdge(PoaGraph<W>& g, uint32_t tail, uint32_t head, int32_t w) {
   using Id = typename W::Id;
-  Id last_out = W::kNone;
-  for (Id e = g.out_head[tail]; e != W::kNone; e = g.e_next_out[e]) {
-    if (g.e_head[e] == head) {
-      g.e_weight[e] += w;
+  uint32_t last_out = W::kNone;
+  for (uint32_t e = Ld(g.node_a + tail).out_head; e != W::kNone;) {
+    const PoaEdge<Id> ea = Ld(g.edge + e);
+    if (ea.head == head) {
+      g.edge_w[e] += w;
       return;
     }
     last_out = e;
+    e = ea.next_out;
   }
   if (g.n_edges >= g.ecap) {
     g.overflow = true;
     return;
   }
-  const Id e = static_cast<Id>(g.n_edges++);
-  g.e_tail[e] = tail;
-  g.e_head[e] = head;
-  g.e_weight[e] = w;
-  g.e_next_in[e] = g.e_next_out[e] = W::kNone;
+  const uint32_t e = g.n_edges++;
+  St(g.edge + e, PoaEdge<Id>{static_cast<Id>(tail), static_cast<Id>(head), W::kNone, W::kNone});
+  g.edge_w[e] = w;
   if (last_out == W::kNone) {
-    g.out_head[tail] = e;
+    g.node_a[tail].out_head = static_cast<Id>(e);
   } else {
-    g.e_next_out[last_out] = e;
+    g.edge[last_out].next_out = static_cast<Id>(e);
   }
-  if (g.in_head[head] == W::kNone) {
-    g.in_head[head] = e;
+  const PoaNodeA<Id> h = Ld(g.node_a + head);
+  if (h.in_head == W::kNone) {
+    g.node_a[head].in_head = static_cast<Id>(e);
   } else {
-    g.e_next_in[g.in_tail[head]] = e;
+    g.edge[h.in_tail].next_in = static_cast<Id>(e);
   }
-  g.in_tail[head] = e;
+  g.node_a[head].in_tail = static_cast<Id>(e);
+}
+
+// coverage = the sequences (of >= 2 bases) whose path visits the node
+template <class W>
+__device__ __forceinline__ void AddCov(PoaGraph<W>& g, uint32_t v) {
+  g.node_b[v].cov += 1;
+}
+
+// append b to a's aligned nodes
+template <class W>
+__device__ void LinkAligned(PoaGraph<W>& g, uint32_t a, uint32_t b) {
+  const uint32_t k = g.node_a[a].n_aligned++;
+  g.node_b[a].aligned[k] = static_cast<typename W::Id>(b);
 }
 
 struct SeqView {
@@ -267,13 +340,11 @@ struct SeqView {
 
 // a chain of fresh nodes for s[begin, end); returns its first node or W::kNone
 template <class W>
-__device__ typename W::Id AddChain(PoaGraph<W>& g, const SeqView& s, uint32_t begin,
-                                   uint32_t end) {
-  using Id = typename W::Id;
+__device__ uint32_t AddChain(PoaGraph<W>& g, const SeqView& s, uint32_t begin, uint32_t end) {
   if (begin == end) return W::kNone;
-  Id first = W::kNone, prev = W::kNone;
+  uint32_t first = W::kNone, prev = W::kNone;
   for (uint32_t i = begin; i < end && !g.overflow; ++i) {
-    const Id cur = AddNode(g, CodeOf(s.bases[i]));
+    const uint32_t cur = AddNode(g, CodeOf(s.bases[i]));
     if (prev != W::kNone) AddEdge(g, prev, cur, s.weight(i - 1) + s.weight(i));
     if (first == W::kNone) first = cur;
     prev = cur;
@@ -281,65 +352,69 @@ __device__ typename W::Id AddChain(PoaGraph<W>& g, const SeqView& s, uint32_t be
   return first;
 }
 
-// spoa Graph::TopologicalSort restricted to the nodes with in_sub != 0
-// (Graph::Subgraph keeps relative ids and adjacency order, so the restricted
-// DFS over the full graph yields exactly the sub-graph's order)
+// spoa Graph::TopologicalSort restricted to the nodes flagged kInSub, whose marks and
+// ignored bits are clear (Graph::Subgraph keeps relative ids and adjacency order, so
+// the restricted DFS over the full graph yields exactly the sub-graph's order)
 template <class W>
 __device__ uint32_t TopoSort(PoaGraph<W>& g) {
   using Id = typename W::Id;
   const uint32_t n = g.n_nodes;
-  for (uint32_t v = 0; v < n; ++v) {
-    g.marks[v] = 0;
-    g.ignored[v] = 0;
-  }
   uint32_t rank = 0, sp = 0;
   for (uint32_t root = 0; root < n; ++root) {
-    if (!g.in_sub[root] || g.marks[root] != 0) continue;
+    if (!(g.flags[root] & kInSub) || (g.flags[root] & kMarks)) continue;
     g.stack[sp++] = static_cast<Id>(root);
     while (sp > 0) {
-      const Id cur = g.stack[sp - 1];
+      const uint32_t cur = g.stack[sp - 1];
       bool valid = true;
-      if (g.marks[cur] != 2) {
-        for (Id e = g.in_head[cur]; e != W::kNone; e = g.e_next_in[e]) {
-          const Id t = g.e_tail[e];
-          if (g.in_sub[t] && g.marks[t] != 2) {
+      if ((g.flags[cur] & kMarks) != 2) {
+        const PoaNodeA<Id> a = Ld(g.node_a + cur);
+        for (uint32_t e = a.in_head; e != W::kNone;) {
+          const PoaEdge<Id> ea = Ld(g.edge + e);
+          const uint32_t t = ea.tail;
+          const uint8_t ft = g.flags[t];
+          if ((ft & kInSub) && (ft & kMarks) != 2) {
             if (sp >= g.stack_cap) {
               g.overflow = true;
               return 0;
             }
-            g.stack[sp++] = t;
+            g.stack[sp++] = static_cast<Id>(t);
             valid = false;
           }
+          e = ea.next_in;
         }
-        if (!g.ignored[cur]) {
-          for (uint32_t a = 0; a < g.n_aligned[cur]; ++a) {
-            const Id t = g.aligned[3 * cur + a];
-            if (g.in_sub[t] && g.marks[t] != 2) {
+        const uint32_t na = a.n_aligned;
+        PoaNodeB<Id> b{};
+        if (na) b = Ld(g.node_b + cur);
+        if (!(g.flags[cur] & kIgnored)) {
+          for (uint32_t i = 0; i < na; ++i) {
+            const uint32_t t = AlignedAt(b, i);
+            const uint8_t ft = g.flags[t];
+            if ((ft & kInSub) && (ft & kMarks) != 2) {
               if (sp >= g.stack_cap) {
                 g.overflow = true;
                 return 0;
               }
-              g.stack[sp++] = t;
-              g.ignored[t] = 1;
+              g.stack[sp++] = static_cast<Id>(t);
+              g.flags[t] = ft | kIgnored;
               valid = false;
             }
           }
         }
         if (valid) {
-          g.marks[cur] = 2;
-          if (!g.ignored[cur]) {
+          g.flags[cur] = (g.flags[cur] & ~kMarks) | 2;
+          if (!(g.flags[cur] & kIgnored)) {
             g.n2r[cur] = static_cast<Id>(rank);
-            g.r2n[rank++] = cur;
-            for (uint32_t a = 0; a < g.n_aligned[cur]; ++a) {
-              const Id t = g.aligned[3 * cur + a];
-              if (g.in_sub[t]) {
+            g.r2n[rank++] = static_cast<Id>(cur);
+            for (uint32_t i = 0; i < na; ++i) {
+              const uint32_t t = AlignedAt(b, i);
+              if (g.flags[t] & kInSub) {
                 g.n2r[t] = static_cast<Id>(rank);
-                g.r2n[rank++] = t;
+                g.r2n[rank++] = static_cast<Id>(t);
               }
             }
           }
         } else {
-          g.marks[cur] = 1;
+          g.flags[cur] = (g.flags[cur] & ~kMarks) | 1;
         }
       }
       if (valid) --sp;
@@ -348,32 +423,38 @@ __device__ uint32_t TopoSort(PoaGraph<W>& g) {
   return rank;
 }
 
-// spoa Graph::ExtractSubgraph(nodes[end], nodes[begin]): backward reachability
-// from `from` through in-edges and aligned nodes, keeping ids >= min_id
+// spoa Graph::ExtractSubgraph(nodes[end], nodes[begin]): backward reachability from
+// `from` through in-edges and aligned nodes, keeping ids >= min_id, into clear flags
 template <class W>
 __device__ void MarkSubgraph(PoaGraph<W>& g, uint32_t from, uint32_t min_id) {
   using Id = typename W::Id;
-  for (uint32_t v = 0; v < g.n_nodes; ++v) g.in_sub[v] = 0;
   uint32_t sp = 0;
   g.stack[sp++] = static_cast<Id>(from);
   while (sp > 0) {
-    const Id cur = g.stack[--sp];
-    if (g.in_sub[cur] || cur < min_id) continue;
-    for (Id e = g.in_head[cur]; e != W::kNone; e = g.e_next_in[e]) {
+    const uint32_t cur = g.stack[--sp];
+    if ((g.flags[cur] & kInSub) || cur < min_id) continue;
+    const PoaNodeA<Id> a = Ld(g.node_a + cur);
+    for (uint32_t e = a.in_head; e != W::kNone;) {
+      const PoaEdge<Id> ea = Ld(g.edge + e);
       if (sp >= g.stack_cap) {
         g.overflow = true;
         return;
       }
-      g.stack[sp++] = g.e_tail[e];
+      g.stack[sp++] = ea.tail;
+      e = ea.next_in;
     }
-    for (uint32_t a = 0; a < g.n_aligned[cur]; ++a) {
-      if (sp >= g.stack_cap) {
-        g.overflow = true;
-        return;
+    const uint32_t na = a.n_aligned;
+    if (na) {
+      const PoaNodeB<Id> b = Ld(g.node_b + cur);
+      for (uint32_t i = 0; i < na; ++i) {
+        if (sp >= g.stack_cap) {
+          g.overflow = true;
+          return;
+        }
+        g.stack[sp++] = static_cast<Id>(AlignedAt(b, i));
       }
-      g.stack[sp++] = g.aligned[3 * cur + a];
     }
-    g.in_sub[cur] = 1;
+    g.flags[cur] |= kInSub;
   }
 }
 
@@ -390,29 +471,32 @@ __device__ void AddAlignment(PoaGraph<W>& g, const SeqView& s, uint32_t aln_len)
     }
   }
   const uint32_t before = g.n_nodes;
-  Id begin = AddChain(g, s, 0, first_pos);
-  Id prev = before == g.n_nodes ? W::kNone : static_cast<Id>(g.n_nodes - 1);
-  const Id last = AddChain(g, s, last_pos + 1, s.len);
-  // count this sequence on the chains (coverage = sequences through a node)
+  uint32_t begin = AddChain(g, s, 0, first_pos);
+  uint32_t prev = before == g.n_nodes ? W::kNone : g.n_nodes - 1;
+  const uint32_t last = AddChain(g, s, last_pos + 1, s.len);
+  // count this sequence on the chains
   const bool counts = s.len >= 2;
   if (counts) {
-    for (uint32_t v = before; v < g.n_nodes; ++v) g.cov[v] += 1;
+    for (uint32_t v = before; v < g.n_nodes; ++v) AddCov(g, v);
   }
   for (uint32_t i = 0; i < aln_len && !g.overflow; ++i) {
     const int32_t pos = g.aln_pos[i];
     if (pos == -1) continue;
     const uint32_t code = CodeOf(s.bases[pos]);
-    Id cur = W::kNone;
+    uint32_t cur = W::kNone;
     if (g.aln_node[i] == -1) {
       cur = AddNode(g, code);
     } else {
-      const Id jt = static_cast<Id>(g.aln_node[i]);
-      if (g.code[jt] == code) {
+      const uint32_t jt = static_cast<Id>(g.aln_node[i]);
+      const PoaNodeA<Id> ja = Ld(g.node_a + jt);
+      if (ja.code == code) {
         cur = jt;
       } else {
-        for (uint32_t a = 0; a < g.n_aligned[jt]; ++a) {
-          const Id kt = g.aligned[3 * jt + a];
-          if (g.code[kt] == code) {
+        const uint32_t na = ja.n_aligned;
+        const PoaNodeB<Id> jb = Ld(g.node_b + jt);
+        for (uint32_t a = 0; a < na; ++a) {
+          const uint32_t kt = AlignedAt(jb, a);
+          if (Ld(g.node_a + kt).code == code) {
             cur = kt;
             break;
           }
@@ -420,19 +504,18 @@ __device__ void AddAlignment(PoaGraph<W>& g, const SeqView& s, uint32_t aln_len)
         if (cur == W::kNone) {  // a new letter for this column
           cur = AddNode(g, code);
           if (g.overflow) break;
-          const uint32_t na = g.n_aligned[jt];
           for (uint32_t a = 0; a < na; ++a) {
-            const Id kt = g.aligned[3 * jt + a];
-            g.aligned[3 * kt + g.n_aligned[kt]++] = cur;
-            g.aligned[3 * cur + g.n_aligned[cur]++] = kt;
+            const uint32_t kt = AlignedAt(jb, a);
+            LinkAligned(g, kt, cur);
+            LinkAligned(g, cur, kt);
           }
-          g.aligned[3 * jt + g.n_aligned[jt]++] = cur;
-          g.aligned[3 * cur + g.n_aligned[cur]++] = jt;
+          LinkAligned(g, jt, cur);
+          LinkAligned(g, cur, jt);
         }
       }
     }
     if (g.overflow) break;
-    if (counts) g.cov[cur] += 1;
+    if (counts) AddCov(g, cur);
     if (begin == W::kNone) begin = cur;
     if (prev != W::kNone) AddEdge(g, prev, cur, s.weight(pos - 1) + s.weight(pos));
     prev = cur;
@@ -442,6 +525,273 @@ __device__ void AddAlignment(PoaGraph<W>& g, const SeqView& s, uint32_t aln_len)
   }
 }
 
+// (all lanes) racon's window prologue, over the window's `nseq` kept sequences. Returns
+// true when it is done here: fewer than 3 give the backbone, "unpolished"; a letter
+// other than ACGT fails it (racon feeds 2-bit reads).
+__device__ __forceinline__ bool WindowDone(uint32_t nseq, uint32_t s0, uint32_t s1, uint32_t L0,
+                                           const uint64_t* seq_off, const uint8_t* bases,
+                                           uint8_t* out, uint32_t* cov_dst, uint32_t* cons_len,
+                                           uint8_t* status, uint32_t lane) {
+  if (nseq < 3) {
+    for (uint32_t i = lane; i < L0; i += 32) {
+      out[i] = bases[seq_off[s0] + i];
+      if (cov_dst) cov_dst[i] = 0;
+    }
+    if (lane == 0) {
+      *cons_len = L0;
+      *status = 0;
+    }
+    return true;
+  }
+  bool bad_letter = false;
+  for (uint64_t i = seq_off[s0] + lane; i < seq_off[s1]; i += 32) {
+    if (CodeOf(bases[i]) < 0) bad_letter = true;
+  }
+  if (__any_sync(0xffffffffu, bad_letter)) {
+    if (lane == 0) {
+      *cons_len = 0;
+      *status = kPoaStatusInvalid;
+    }
+    return true;
+  }
+  return false;
+}
+
+// (lane 0) the graph's arrays in the window's scratch slab (the kernel sets flags, r2n
+// and n2r), the layers' order, and the backbone chain (spoa AddAlignment with an empty
+// alignment: its edges weigh by its own qualities when the batch has qualities, and 0
+// when it has none). Returns 0 or the status that ends the window.
+template <class W>
+__device__ uint32_t SetupGraph(PoaGraph<W>& g, uint8_t* base, const PoaLayout& L,
+                               const typename W::Shape& shape, const uint64_t* seq_off,
+                               const uint8_t* bases, const uint8_t* quals,
+                               const uint32_t* seq_begin, const uint32_t* seq_end,
+                               uint32_t s0, uint32_t s1, uint32_t L0) {
+  using Id = typename W::Id;
+  g.node_a = reinterpret_cast<PoaNodeA<Id>*>(base + L.node_a);
+  g.node_b = reinterpret_cast<PoaNodeB<Id>*>(base + L.node_b);
+  g.edge = reinterpret_cast<PoaEdge<Id>*>(base + L.edge);
+  g.edge_w = reinterpret_cast<int32_t*>(base + L.edge_w);
+  g.stack = reinterpret_cast<Id*>(base + L.stack);
+  g.order = reinterpret_cast<Id*>(base + L.order);
+  g.aln_node = reinterpret_cast<typename W::Pos*>(base + L.aln_node);
+  g.aln_pos = reinterpret_cast<typename W::Pos*>(base + L.aln_pos);
+  g.pred = reinterpret_cast<int32_t*>(base + L.pred);
+  g.score = reinterpret_cast<long long*>(base + L.score);
+  g.H = reinterpret_cast<typename W::Cell*>(base + L.H);
+  g.DIR = base + L.DIR;
+  g.n_nodes = g.n_edges = 0;
+  g.ncap = shape.ncap;
+  g.ecap = shape.ecap;
+  g.stack_cap = 4 * shape.ncap;
+  g.overflow = false;
+  // layer coordinates are validated up front
+  const uint32_t fail = OrderLayers(g.order, seq_off, seq_begin, seq_end, s0, s1, L0,
+                                    shape.lmax, W::Layers(shape));
+  if (!fail) {
+    const SeqView bb{bases + seq_off[s0], quals ? quals + seq_off[s0] : nullptr, L0, 0};
+    AddChain(g, bb, 0, L0);
+    if (L0 >= 2) {
+      for (uint32_t v = 0; v < g.n_nodes; ++v) AddCov(g, v);
+    }
+  }
+  return fail;
+}
+
+// (all lanes) the graph a layer aligns to, in topological order: the whole graph, or
+// the sub-graph between the layer's begin and end nodes; the cell guard; the sinks
+// (no out-edge inside the (sub)graph). Returns the rows; on overflow the window stops.
+template <class W>
+__device__ __forceinline__ uint32_t LayerGraph(PoaGraph<W>& g, bool full, uint32_t lb,
+                                               uint32_t le, uint32_t len, int m, int n,
+                                               int gap, uint32_t lane) {
+  const uint32_t nn = g.n_nodes;
+  for (uint32_t v = lane; v < nn; v += 32) g.flags[v] = full ? kInSub : 0;
+  __syncwarp();
+  if (lane == 0) {
+    if (!full) MarkSubgraph(g, le, lb);
+    const uint32_t rows = g.overflow ? 0 : TopoSort(g);
+    // the cells' range: |score| <= max|m,n,g| * (rows + columns)
+    const int amax = max(max(abs(m), abs(n)), abs(gap));
+    if (static_cast<long long>(amax) * (rows + len + 2) > W::kCellLimit) g.overflow = true;
+    g.rows = rows;
+  }
+  __syncwarp();
+  const uint32_t rows = g.rows;
+  if (g.overflow) return rows;
+  for (uint32_t r = lane; r < rows; r += 32) {
+    const uint32_t v = g.r2n[r];
+    bool sink = true;
+    for (uint32_t e = Ld(g.node_a + v).out_head; e != W::kNone;) {
+      const PoaEdge<typename W::Id> ea = Ld(g.edge + e);
+      if (g.flags[ea.head] & kInSub) {
+        sink = false;
+        break;
+      }
+      e = ea.next_out;
+    }
+    if (sink) g.flags[v] |= kSink;
+  }
+  __syncwarp();
+  return rows;
+}
+
+// (lane 0) the traceback of `alen` steps, written from its end, into emission order,
+// and the layer into the graph
+template <class W>
+__device__ void MergeLayer(PoaGraph<W>& g, const SeqView& sv, uint32_t alen) {
+  for (uint32_t a = 0; a < alen / 2; ++a) {
+    const typename W::Pos tn = g.aln_node[a], tp = g.aln_pos[a];
+    g.aln_node[a] = g.aln_node[alen - 1 - a];
+    g.aln_pos[a] = g.aln_pos[alen - 1 - a];
+    g.aln_node[alen - 1 - a] = tn;
+    g.aln_pos[alen - 1 - a] = tp;
+  }
+  if (g.overflow) return;
+  if (alen == 0) {
+    // spoa: an empty alignment appends the sequence as a separate chain
+    const uint32_t before = g.n_nodes;
+    AddChain(g, sv, 0, sv.len);
+    if (sv.len >= 2) {
+      for (uint32_t v = before; v < g.n_nodes; ++v) AddCov(g, v);
+    }
+  } else {
+    AddAlignment(g, sv, alen);
+  }
+}
+
+// (all lanes) the window's result: spoa's heaviest bundle with branch completion,
+// racon's coverage-based TGS trimming, the consensus and its coverage, the status, and
+// the window's DP cells
+template <class W>
+__device__ __forceinline__ void Consensus(PoaGraph<W>& g, uint32_t fail, uint32_t nseq,
+                                          int trim, int tgs, unsigned long long my_cells,
+                                          uint8_t* out, uint32_t* cov_dst, uint32_t* cons_len,
+                                          uint8_t* status, unsigned long long* cells,
+                                          uint32_t lane) {
+  using Id = typename W::Id;
+  const uint32_t nn = g.n_nodes;
+  for (uint32_t v = lane; v < nn; v += 32) g.flags[v] = kInSub;
+  __syncwarp();
+  if (lane != 0) return;
+  uint32_t st = 0, clen = 0;
+  if (fail) {
+    st = fail;
+  } else if (g.overflow) {
+    st = kPoaStatusCapacity;
+  } else {
+    const uint32_t rows = TopoSort(g);
+    if (g.overflow) {
+      st = kPoaStatusCapacity;
+    } else {
+      for (uint32_t v = 0; v < g.n_nodes; ++v) {
+        g.pred[v] = -1;
+        g.score[v] = -1;
+      }
+      int32_t mx = -1;
+      for (uint32_t r = 0; r < rows; ++r) {
+        const uint32_t v = g.r2n[r];
+        for (uint32_t e = Ld(g.node_a + v).in_head; e != W::kNone;) {
+          const PoaEdge<Id> ea = Ld(g.edge + e);
+          const uint32_t t = ea.tail;
+          const long long wgt = g.edge_w[e];
+          if (g.score[v] < wgt || (g.score[v] == wgt && g.score[g.pred[v]] <= g.score[t])) {
+            g.score[v] = wgt;
+            g.pred[v] = static_cast<int32_t>(t);
+          }
+          e = ea.next_in;
+        }
+        if (g.pred[v] != -1) g.score[v] += g.score[g.pred[v]];
+        if (mx < 0 || g.score[mx] < g.score[v]) mx = static_cast<int32_t>(v);
+      }
+      while (Ld(g.node_a + mx).out_head != W::kNone) {  // branch completion
+        const uint32_t rank = g.n2r[mx];
+        for (uint32_t e = Ld(g.node_a + mx).out_head; e != W::kNone;) {
+          const PoaEdge<Id> ea = Ld(g.edge + e);
+          for (uint32_t f = Ld(g.node_a + ea.head).in_head; f != W::kNone;) {
+            const PoaEdge<Id> fa = Ld(g.edge + f);
+            if (fa.tail != static_cast<uint32_t>(mx)) g.score[fa.tail] = -1;
+            f = fa.next_in;
+          }
+          e = ea.next_out;
+        }
+        int32_t nmx = -1;
+        for (uint32_t r = rank + 1; r < rows; ++r) {
+          const uint32_t v = g.r2n[r];
+          g.score[v] = -1;
+          g.pred[v] = -1;
+          for (uint32_t e = Ld(g.node_a + v).in_head; e != W::kNone;) {
+            const PoaEdge<Id> ea = Ld(g.edge + e);
+            const uint32_t t = ea.tail;
+            const long long wgt = g.edge_w[e];
+            e = ea.next_in;
+            if (g.score[t] == -1) continue;
+            if (g.score[v] < wgt || (g.score[v] == wgt && g.score[g.pred[v]] <= g.score[t])) {
+              g.score[v] = wgt;
+              g.pred[v] = static_cast<int32_t>(t);
+            }
+          }
+          if (g.pred[v] != -1) g.score[v] += g.score[g.pred[v]];
+          if (nmx < 0 || g.score[nmx] < g.score[v]) nmx = static_cast<int32_t>(v);
+        }
+        mx = nmx;
+      }
+      // walk back; r2n is free now and holds the reversed path
+      uint32_t plen = 0;
+      int32_t v = mx;
+      while (g.pred[v] != -1) {
+        g.r2n[plen++] = static_cast<Id>(v);
+        v = g.pred[v];
+      }
+      g.r2n[plen++] = static_cast<Id>(v);
+      // coverage of a consensus base = its node + the aligned nodes
+      auto coverage = [&](uint32_t idx) -> uint32_t {
+        const uint32_t nd = g.r2n[plen - 1 - idx];
+        uint32_t cvg = g.node_b[nd].cov;
+        const uint32_t na = Ld(g.node_a + nd).n_aligned;
+        if (na) {
+          const PoaNodeB<Id> b = Ld(g.node_b + nd);
+          for (uint32_t a = 0; a < na; ++a) cvg += g.node_b[AlignedAt(b, a)].cov;
+        }
+        return cvg;
+      };
+      uint32_t cb = 0, ce = plen;  // [cb, ce)
+      st = kPoaStatusOk;
+      if (tgs && trim) {
+        const uint32_t avg = (nseq - 1) / 2;
+        int32_t b = 0, e2 = static_cast<int32_t>(plen) - 1;
+        for (; b < static_cast<int32_t>(plen); ++b) {
+          if (coverage(b) >= avg) break;
+        }
+        for (; e2 >= 0; --e2) {
+          if (coverage(e2) >= avg) break;
+        }
+        if (b >= e2) {
+          st |= kPoaStatusChimeric;
+        } else {
+          cb = b;
+          ce = e2 + 1;
+        }
+      }
+      clen = ce - cb;
+      for (uint32_t i = 0; i < clen; ++i) {
+        const uint32_t nd = g.r2n[plen - 1 - (cb + i)];
+        out[i] = "ACGT"[Ld(g.node_a + nd).code];
+        if (cov_dst) cov_dst[i] = coverage(cb + i);
+      }
+    }
+  }
+  *cons_len = clen;
+  *status = static_cast<uint8_t>(st);
+  // DP cells of this window (lanes hold the same count); an attempt that ran out
+  // of capacity is run again and counted then
+  if (cells && st != kPoaStatusCapacity) atomicAdd(cells, my_cells);
+}
+
+// The generic DP: all lanes fill a row 32 columns at a time, the diagonal neighbour
+// from the row above, the horizontal gap recurrence H[i][j] = max(M[j], H[i][j-1] + g)
+// as a warp max-scan of M[j] - j*g (exact in integers); lane 0's traceback re-derives
+// each step from H with spoa's preference.
 template <class W>
 __global__ void __launch_bounds__(32)
 PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
@@ -460,85 +810,24 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
   const uint32_t lane = threadIdx.x;
   const uint32_t w = win_list ? win_list[blockIdx.x] : blockIdx.x;
   const uint32_t s0 = win_first[w], s1 = win_first[w + 1];
-  const uint32_t nseq = KeptSequences(seq_off, seq_begin, seq_end, s0, s1, lane);
   const uint32_t L0 = static_cast<uint32_t>(seq_off[s0 + 1] - seq_off[s0]);
   uint8_t* out = cons + cons_off[w];
   uint32_t* cov_dst = cov_out ? cov_out + cons_off[w] : nullptr;
-
-  if (nseq < 3) {  // fewer than 3 sequences: the backbone, "unpolished"
-    for (uint32_t i = lane; i < L0; i += 32) {
-      out[i] = bases[seq_off[s0] + i];
-      if (cov_dst) cov_dst[i] = 0;
-    }
-    if (lane == 0) {
-      cons_len[w] = L0;
-      status[w] = 0;
-    }
+  const uint32_t nseq = KeptSequences(seq_off, seq_begin, seq_end, s0, s1, lane);
+  if (WindowDone(nseq, s0, s1, L0, seq_off, bases, out, cov_dst, cons_len + w, status + w, lane)) {
     return;
   }
 
-  // only ACGT letters are valid (racon feeds 2-bit reads)
-  {
-    bool bad_letter = false;
-    for (uint64_t i = seq_off[s0] + lane; i < seq_off[s1]; i += 32) {
-      if (CodeOf(bases[i]) < 0) bad_letter = true;
-    }
-    if (__any_sync(0xffffffffu, bad_letter)) {
-      if (lane == 0) {
-        cons_len[w] = 0;
-        status[w] = kPoaStatusInvalid;
-      }
-      return;
-    }
-  }
-
   uint8_t* base = scratch + scratch_stride * blockIdx.x;
-  const PoaLayout L = MakePoaLayout<W>(shape);
+  const PoaLayout L = MakePoaLayout<W>(shape, false);
   __shared__ PoaGraph<W> g;
-  __shared__ uint32_t sh_rows, sh_fail;
+  __shared__ uint32_t sh_fail;
   if (lane == 0) {
-    g.code = base + L.code;
-    g.n_aligned = base + L.n_aligned;
-    g.marks = base + L.marks;
-    g.ignored = base + L.ignored;
-    g.in_sub = base + L.in_sub;
-    g.sink = base + L.sink;
-    g.in_head = reinterpret_cast<Id*>(base + L.in_head);
-    g.in_tail = reinterpret_cast<Id*>(base + L.in_tail);
-    g.out_head = reinterpret_cast<Id*>(base + L.out_head);
-    g.aligned = reinterpret_cast<Id*>(base + L.aligned);
-    g.cov = reinterpret_cast<Id*>(base + L.cov);
+    g.flags = base + L.flags;
     g.r2n = reinterpret_cast<Id*>(base + L.r2n);
     g.n2r = reinterpret_cast<Id*>(base + L.n2r);
-    g.stack = reinterpret_cast<Id*>(base + L.stack);
-    g.order = reinterpret_cast<Id*>(base + L.order);
-    g.e_tail = reinterpret_cast<Id*>(base + L.e_tail);
-    g.e_head = reinterpret_cast<Id*>(base + L.e_head);
-    g.e_next_in = reinterpret_cast<Id*>(base + L.e_next_in);
-    g.e_next_out = reinterpret_cast<Id*>(base + L.e_next_out);
-    g.e_weight = reinterpret_cast<int32_t*>(base + L.e_weight);
-    g.aln_node = reinterpret_cast<Pos*>(base + L.aln_node);
-    g.aln_pos = reinterpret_cast<Pos*>(base + L.aln_pos);
-    g.pred = reinterpret_cast<int32_t*>(base + L.pred);
-    g.score = reinterpret_cast<long long*>(base + L.score);
-    g.H = reinterpret_cast<Cell*>(base + L.H);
-    g.n_nodes = g.n_edges = 0;
-    g.ncap = shape.ncap;
-    g.ecap = shape.ecap;
-    g.stack_cap = 4 * shape.ncap;
-    g.overflow = false;
-    // layer coordinates are validated up front
-    sh_fail = OrderLayers(g.order, seq_off, seq_begin, seq_end, s0, s1, L0, shape.lmax,
-                          W::Layers(shape));
-    if (!sh_fail) {
-      // backbone chain (spoa AddAlignment with an empty alignment): its edges weigh
-      // by its own qualities when the batch has qualities, and 0 when it has none
-      SeqView bb{bases + seq_off[s0], quals ? quals + seq_off[s0] : nullptr, L0, 0};
-      AddChain(g, bb, 0, L0);
-      if (L0 >= 2) {
-        for (uint32_t v = 0; v < g.n_nodes; ++v) g.cov[v] += 1;
-      }
-    }
+    sh_fail = SetupGraph(g, base, L, shape, seq_off, bases, quals, seq_begin, seq_end, s0, s1,
+                         L0);
   }
   __syncwarp();
 
@@ -552,35 +841,8 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
     const SeqView sv{bases + seq_off[s], quals ? quals + seq_off[s] : nullptr,
                      static_cast<uint32_t>(seq_off[s + 1] - seq_off[s]), 1};
     const uint32_t len = sv.len;
-
-    // ---- (lane 0) the graph this layer aligns to, in topological order ----
-    if (lane == 0) {
-      const uint32_t lb = seq_begin[s], le = seq_end[s];
-      if (lb < offset && le > L0 - offset) {
-        for (uint32_t v = 0; v < g.n_nodes; ++v) g.in_sub[v] = 1;
-      } else {
-        MarkSubgraph(g, le, lb);
-      }
-      uint32_t rows = g.overflow ? 0 : TopoSort(g);
-      // a node is a sink if it has no out-edge inside the (sub)graph
-      for (uint32_t r = 0; r < rows; ++r) {
-        const Id v = g.r2n[r];
-        uint8_t sink = 1;
-        for (Id e = g.out_head[v]; e != W::kNone; e = g.e_next_out[e]) {
-          if (g.in_sub[g.e_head[e]]) {
-            sink = 0;
-            break;
-          }
-        }
-        g.sink[v] = sink;
-      }
-      // the cells' range: |score| <= max|m,n,g| * (rows + columns)
-      const int amax = max(max(abs(m), abs(n)), abs(gap));
-      if (static_cast<long long>(amax) * (rows + len + 2) > W::kCellLimit) g.overflow = true;
-      sh_rows = rows;
-    }
-    __syncwarp();
-    const uint32_t rows = sh_rows;
+    const uint32_t lb = seq_begin[s], le = seq_end[s];
+    const uint32_t rows = LayerGraph(g, lb < offset && le > L0 - offset, lb, le, len, m, n, gap, lane);
     if (g.overflow) break;
     my_cells += static_cast<unsigned long long>(rows + 1) * (len + 1);
 
@@ -590,19 +852,20 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
     __syncwarp();
     int best_score = -2147483647, best_row = -1;
     for (uint32_t r = 0; r < rows; ++r) {
-      const Id v = g.r2n[r];
-      const uint32_t vcode = g.code[v];
+      const uint32_t v = g.r2n[r];
+      const PoaNodeA<Id> va = Ld(g.node_a + v);
       Cell* row = H + static_cast<size_t>(r + 1) * width;
       // column 0
       int col0 = 0;
       {
         bool any = false;
         int pen = -2147483647;
-        for (Id e = g.in_head[v]; e != W::kNone; e = g.e_next_in[e]) {
-          const Id t = g.e_tail[e];
-          if (!g.in_sub[t]) continue;
+        for (uint32_t e = va.in_head; e != W::kNone;) {
+          const PoaEdge<Id> ea = Ld(g.edge + e);
+          e = ea.next_in;
+          if (!(g.flags[ea.tail] & kInSub)) continue;
           any = true;
-          pen = max(pen, static_cast<int>(H[static_cast<size_t>(g.n2r[t] + 1) * width]));
+          pen = max(pen, static_cast<int>(H[static_cast<size_t>(g.n2r[ea.tail] + 1) * width]));
         }
         col0 = (any ? pen : 0) + gap;
       }
@@ -611,13 +874,14 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
         const uint32_t j = c0 + lane;
         int M = W::kNoCell;
         if (j <= len) {
-          const int match = (static_cast<uint32_t>(CodeOf(sv.bases[j - 1])) == vcode) ? m : n;
+          const int match = (static_cast<uint32_t>(CodeOf(sv.bases[j - 1])) == va.code) ? m : n;
           bool any = false;
-          for (Id e = g.in_head[v]; e != W::kNone; e = g.e_next_in[e]) {
-            const Id t = g.e_tail[e];
-            if (!g.in_sub[t]) continue;
+          for (uint32_t e = va.in_head; e != W::kNone;) {
+            const PoaEdge<Id> ea = Ld(g.edge + e);
+            e = ea.next_in;
+            if (!(g.flags[ea.tail] & kInSub)) continue;
             any = true;
-            const Cell* pr = H + static_cast<size_t>(g.n2r[t] + 1) * width;
+            const Cell* pr = H + static_cast<size_t>(g.n2r[ea.tail] + 1) * width;
             M = max(M, max(static_cast<int>(pr[j - 1]) + match,
                            static_cast<int>(pr[j]) + gap));
           }
@@ -638,7 +902,7 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
       }
       if (lane == 0) row[0] = static_cast<Cell>(col0);
       __syncwarp();
-      if (g.sink[v]) {
+      if (g.flags[v] & kSink) {
         const int sc = row[len];
         if (best_score < sc) {
           best_score = sc;
@@ -647,7 +911,8 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
       }
     }
 
-    // ---- (lane 0) traceback + merge ----
+    // ---- (lane 0) traceback: diagonal over predecessors in in-edge order, then
+    // vertical, then horizontal ----
     if (lane == 0) {
       uint32_t alen = 0;
       uint32_t i = best_row < 0 ? 0 : static_cast<uint32_t>(best_row), j = len;
@@ -658,15 +923,15 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
         uint32_t pi = 0, pj = 0;
         bool found = false;
         if (i != 0 && j != 0) {
-          const Id v = g.r2n[i - 1];
-          const int match =
-              (static_cast<uint32_t>(CodeOf(sv.bases[j - 1])) == g.code[v]) ? m : n;
+          const PoaNodeA<Id> va = Ld(g.node_a + g.r2n[i - 1]);
+          const int match = (static_cast<uint32_t>(CodeOf(sv.bases[j - 1])) == va.code) ? m : n;
           bool any = false;
-          for (Id e = g.in_head[v]; e != W::kNone && !found; e = g.e_next_in[e]) {
-            const Id t = g.e_tail[e];
-            if (!g.in_sub[t]) continue;
+          for (uint32_t e = va.in_head; e != W::kNone && !found;) {
+            const PoaEdge<Id> ea = Ld(g.edge + e);
+            e = ea.next_in;
+            if (!(g.flags[ea.tail] & kInSub)) continue;
             any = true;
-            const uint32_t p = g.n2r[t] + 1;
+            const uint32_t p = g.n2r[ea.tail] + 1;
             if (h == H[static_cast<size_t>(p) * width + (j - 1)] + match) {
               pi = p;
               pj = j - 1;
@@ -680,13 +945,13 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
           }
         }
         if (!found && i != 0) {
-          const Id v = g.r2n[i - 1];
           bool any = false;
-          for (Id e = g.in_head[v]; e != W::kNone && !found; e = g.e_next_in[e]) {
-            const Id t = g.e_tail[e];
-            if (!g.in_sub[t]) continue;
+          for (uint32_t e = Ld(g.node_a + g.r2n[i - 1]).in_head; e != W::kNone && !found;) {
+            const PoaEdge<Id> ea = Ld(g.edge + e);
+            e = ea.next_in;
+            if (!(g.flags[ea.tail] & kInSub)) continue;
             any = true;
-            const uint32_t p = g.n2r[t] + 1;
+            const uint32_t p = g.n2r[ea.tail] + 1;
             if (h == H[static_cast<size_t>(p) * width + j] + gap) {
               pi = p;
               pj = j;
@@ -714,141 +979,12 @@ PoaKernel(uint32_t n_windows, const uint32_t* __restrict__ win_list,
         i = pi;
         j = pj;
       }
-      // reverse into emission order
-      for (uint32_t a = 0; a < alen / 2; ++a) {
-        const Pos tn = g.aln_node[a], tp = g.aln_pos[a];
-        g.aln_node[a] = g.aln_node[alen - 1 - a];
-        g.aln_pos[a] = g.aln_pos[alen - 1 - a];
-        g.aln_node[alen - 1 - a] = tn;
-        g.aln_pos[alen - 1 - a] = tp;
-      }
-      if (!g.overflow) {
-        if (alen == 0) {
-          // spoa: an empty alignment appends the sequence as a separate chain
-          const uint32_t before = g.n_nodes;
-          AddChain(g, sv, 0, sv.len);
-          if (sv.len >= 2) {
-            for (uint32_t v = before; v < g.n_nodes; ++v) g.cov[v] += 1;
-          }
-        } else {
-          AddAlignment(g, sv, alen);
-        }
-      }
+      MergeLayer(g, sv, alen);
     }
     __syncwarp();
   }
-
-  // ---- (lane 0) consensus: heaviest bundle + branch completion + trimming ----
-  if (lane == 0) {
-    uint32_t st = 0;
-    uint32_t clen = 0;
-    if (sh_fail) {
-      st = sh_fail;
-    } else if (g.overflow) {
-      st = kPoaStatusCapacity;
-    } else {
-      for (uint32_t v = 0; v < g.n_nodes; ++v) g.in_sub[v] = 1;
-      const uint32_t rows = TopoSort(g);
-      if (g.overflow) {
-        st = kPoaStatusCapacity;
-      } else {
-        for (uint32_t v = 0; v < g.n_nodes; ++v) {
-          g.pred[v] = -1;
-          g.score[v] = -1;
-        }
-        auto relax = [&](Id v) {
-          for (Id e = g.in_head[v]; e != W::kNone; e = g.e_next_in[e]) {
-            const Id t = g.e_tail[e];
-            const long long wgt = g.e_weight[e];
-            if (g.score[v] < wgt ||
-                (g.score[v] == wgt && g.score[g.pred[v]] <= g.score[t])) {
-              g.score[v] = wgt;
-              g.pred[v] = t;
-            }
-          }
-          if (g.pred[v] != -1) g.score[v] += g.score[g.pred[v]];
-        };
-        int32_t mx = -1;
-        for (uint32_t r = 0; r < rows; ++r) {
-          const Id v = g.r2n[r];
-          relax(v);
-          if (mx < 0 || g.score[mx] < g.score[v]) mx = v;
-        }
-        while (g.out_head[mx] != W::kNone) {  // branch completion
-          const uint32_t rank = g.n2r[mx];
-          for (Id e = g.out_head[mx]; e != W::kNone; e = g.e_next_out[e]) {
-            const Id hd = g.e_head[e];
-            for (Id f = g.in_head[hd]; f != W::kNone; f = g.e_next_in[f]) {
-              if (g.e_tail[f] != mx) g.score[g.e_tail[f]] = -1;
-            }
-          }
-          int32_t nmx = -1;
-          for (uint32_t r = rank + 1; r < rows; ++r) {
-            const Id v = g.r2n[r];
-            g.score[v] = -1;
-            g.pred[v] = -1;
-            for (Id e = g.in_head[v]; e != W::kNone; e = g.e_next_in[e]) {
-              const Id t = g.e_tail[e];
-              if (g.score[t] == -1) continue;
-              const long long wgt = g.e_weight[e];
-              if (g.score[v] < wgt ||
-                  (g.score[v] == wgt && g.score[g.pred[v]] <= g.score[t])) {
-                g.score[v] = wgt;
-                g.pred[v] = t;
-              }
-            }
-            if (g.pred[v] != -1) g.score[v] += g.score[g.pred[v]];
-            if (nmx < 0 || g.score[nmx] < g.score[v]) nmx = v;
-          }
-          mx = nmx;
-        }
-        // walk back; r2n is free now and holds the reversed path
-        uint32_t plen = 0;
-        int32_t v = mx;
-        while (g.pred[v] != -1) {
-          g.r2n[plen++] = static_cast<Id>(v);
-          v = g.pred[v];
-        }
-        g.r2n[plen++] = static_cast<Id>(v);
-        // coverage of a consensus base = its node + the aligned nodes
-        auto coverage = [&](uint32_t idx) -> uint32_t {
-          const Id nd = g.r2n[plen - 1 - idx];
-          uint32_t cvg = g.cov[nd];
-          for (uint32_t a = 0; a < g.n_aligned[nd]; ++a) cvg += g.cov[g.aligned[3 * nd + a]];
-          return cvg;
-        };
-        uint32_t cb = 0, ce = plen;  // [cb, ce)
-        st = kPoaStatusOk;
-        if (tgs && trim) {
-          const uint32_t avg = (nseq - 1) / 2;
-          int32_t b = 0, e2 = static_cast<int32_t>(plen) - 1;
-          for (; b < static_cast<int32_t>(plen); ++b) {
-            if (coverage(b) >= avg) break;
-          }
-          for (; e2 >= 0; --e2) {
-            if (coverage(e2) >= avg) break;
-          }
-          if (b >= e2) {
-            st |= kPoaStatusChimeric;
-          } else {
-            cb = b;
-            ce = e2 + 1;
-          }
-        }
-        clen = ce - cb;
-        for (uint32_t i = 0; i < clen; ++i) {
-          const Id nd = g.r2n[plen - 1 - (cb + i)];
-          out[i] = "ACGT"[g.code[nd]];
-          if (cov_dst) cov_dst[i] = coverage(cb + i);
-        }
-      }
-    }
-    cons_len[w] = clen;
-    status[w] = static_cast<uint8_t>(st);
-    // DP cells of this window (lanes hold the same count); an attempt that ran out
-    // of capacity is run again and counted then
-    if (cells && st != kPoaStatusCapacity) atomicAdd(cells, my_cells);
-  }
+  Consensus(g, sh_fail, nseq, trim, tgs, my_cells, out, cov_dst, cons_len + w, status + w,
+            cells, lane);
 }
 
 }  // namespace
@@ -913,7 +1049,7 @@ void PoaWideRun(Ctx& c, std::vector<uint32_t> todo, const PoaWindowDims& d,
     return a;
   };
   const auto stride_of = [](const PoaWideShape& s) {
-    return (MakePoaLayout<PoaWide>(s).bytes + 255) & ~size_t(255);
+    return (MakePoaLayout<PoaWide>(s, false).bytes + 255) & ~size_t(255);
   };
   while (!todo.empty()) {
     std::vector<size_t> need(n_windows, 0);
@@ -1070,9 +1206,7 @@ void PoaRun(Ctx& c, uint32_t n_windows, const uint32_t* h_win_first, const uint6
       shape.width = (lmax + 1 + 31) & ~31u;
       const size_t fast_smem = ((shape.ncap + 15) & ~15u) + 4ULL * shape.ncap + 16;
       const bool fast = group == 0 && fast_smem <= 220 * 1024;  // the register-row kernel
-      const size_t stride = ((fast ? MakeFastLayout(shape).bytes
-                                   : MakePoaLayout<PoaNarrow>(shape).bytes) +
-                             255) & ~size_t(255);
+      const size_t stride = (MakePoaLayout<PoaNarrow>(shape, fast).bytes + 255) & ~size_t(255);
       if (fast) {
         RVN_CUDA(cudaFuncSetAttribute(PoaKernelFast,
                                       cudaFuncAttributeMaxDynamicSharedMemorySize,
