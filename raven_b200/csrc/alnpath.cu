@@ -547,9 +547,8 @@ void AlignBreakingPoints(Ctx& c, uint64_t n, const uint32_t* q_read, const uint3
   for (uint64_t i = 0; i < n; ++i) {
     const uint32_t a = q_read[i], b = t_read[i];
     if (a >= c.n_reads || b >= c.n_reads) throw InvalidArgument("read index out of bounds");
-    if (a < c.res_first || a >= c.res_last || b < c.res_first || b >= c.res_last) {
-      throw StateError("the bases of these reads were not uploaded (rvn_reads_upload_range)");
-    }
+    CheckResident(c, a, a + 1);
+    CheckResident(c, b, b + 1);
     if (static_cast<uint64_t>(q_begin[i]) + q_len[i] > c.h_len[a] ||
         static_cast<uint64_t>(t_begin[i]) + t_len[i] > c.h_len[b]) {
       throw InvalidArgument("substring beyond the end of its read");

@@ -59,13 +59,13 @@ void SetOption(Ctx& c, const char* name, int64_t value) {
   if (name && std::strcmp(name, "keep_hits") == 0) {
     c.keep_hits = value != 0;
   } else if (name && std::strcmp(name, "async_upload") == 0) {
-    c.async_upload = value != 0;
+    c.bases.async_upload = value != 0;
   } else if (name && std::strcmp(name, "host_bases") == 0) {
     if (value < -1 || value > 1) throw InvalidArgument("host_bases: -1 (auto), 0 or 1");
-    c.host_bases = value;
+    c.bases.host_bases = value;
   } else if (name && std::strcmp(name, "host_bases_budget") == 0) {
     if (value < 0) throw InvalidArgument("host_bases_budget: bytes, 0 = the free memory");
-    c.host_bases_budget = static_cast<uint64_t>(value);
+    c.bases.host_bases_budget = static_cast<uint64_t>(value);
   } else if (name && std::strcmp(name, "self_join") == 0) {
     c.self_join = value != 0;
   } else if (name && std::strcmp(name, "bare_count") == 0) {
@@ -184,22 +184,13 @@ RVN_API void rvn_ctx_destroy(rvn_ctx* ctx) {
   }
   for (auto e : ctx->c.timer.pool) cudaEventDestroy(e);
   ArenaRelease(ctx->c);
-  if (ctx->c.copy_stream) {
-    cudaStreamSynchronize(ctx->c.copy_stream);
-    cudaStreamDestroy(ctx->c.copy_stream);
-  }
+  ReleaseBases(ctx->c);
   if (ctx->c.d2h_stream) {
     cudaStreamSynchronize(ctx->c.d2h_stream);
     cudaStreamDestroy(ctx->c.d2h_stream);
     cudaEventDestroy(ctx->c.d2h_ready);
     cudaEventDestroy(ctx->c.d2h_done);
   }
-  for (auto e : ctx->c.up_events) cudaEventDestroy(e);
-  for (auto& h : ctx->c.bh) {
-    for (auto e : h.events) cudaEventDestroy(e);
-    if (h.used) cudaEventDestroy(h.used);
-  }
-  if (ctx->c.up_fence) cudaEventDestroy(ctx->c.up_fence);
   if (ctx->c.own_stream) cudaStreamDestroy(ctx->c.stream);
   delete ctx;
 }
@@ -224,128 +215,6 @@ RVN_API int rvn_engine_configure(rvn_ctx* ctx, uint32_t k, uint32_t w,
     c.tiles_k = 0;  // the tile table depends on (k, w)
     c.occurrence = 0xFFFFFFFFu;
   });
-}
-
-// whole_set: rvn_reads_upload / rvn_reads_upload_ids, where option host_bases applies
-static void UploadReads(Ctx& c, const uint64_t* words, const uint64_t* word_off,
-                        const uint32_t* lens, const uint32_t* ids,
-                        uint32_t n_reads, uint32_t res_first = 0,
-                        uint32_t res_last = 0xFFFFFFFFu, bool whole_set = false) {
-  if (n_reads && (!word_off || !lens)) throw InvalidArgument("null read set");
-  res_last = std::min(res_last, n_reads);
-  if (res_first > res_last) throw InvalidArgument("resident range out of bounds");
-  if (n_reads == 0xFFFFFFFFu) throw LimitError("too many reads");
-  c.s_valid = c.q_valid = c.qt_valid = c.i_valid = c.r_valid = c.st_valid = false;
-  c.st_piles_on_device = false;
-  c.tiles_k = 0;
-  c.n_reads = n_reads;
-  c.h_woff.assign(1, 0);
-  if (n_reads) c.h_woff.assign(word_off, word_off + n_reads + 1);
-  c.h_len.assign(lens, lens + n_reads);
-  // piles: len >> 4 bins each (pile.cc:19-31)
-  c.h_pile_off.assign(n_reads + 1ULL, 0);
-  for (uint32_t i = 0; i < n_reads; ++i) c.h_pile_off[i + 1] = c.h_pile_off[i] + (lens[i] >> 4);
-  c.h_ids.resize(n_reads);
-  c.ids_identity = true;
-  c.ids_ascending = true;
-  for (uint32_t i = 0; i < n_reads; ++i) {
-    const uint64_t have = c.h_woff[i + 1] - c.h_woff[i];
-    if (have < ((static_cast<uint64_t>(lens[i]) + 31) >> 5)) {
-      throw InvalidArgument("read shorter than its declared length");
-    }
-    if (lens[i] >= (1u << 31)) throw LimitError("read of 2^31 or more bases");
-    c.h_ids[i] = ids ? ids[i] : i;
-    if (c.h_ids[i] != i) c.ids_identity = false;
-    if (i > 0 && c.h_ids[i] < c.h_ids[i - 1]) c.ids_ascending = false;
-  }
-  c.n_words = c.h_woff[n_reads];
-  // (kernels and copies of earlier calls may still use the buffers of the old bases)
-  RVN_CUDA(cudaStreamSynchronize(c.stream));
-  if (c.copy_stream) RVN_CUDA(cudaStreamSynchronize(c.copy_stream));
-  c.bases_on_host = whole_set && UseHostBases(c);
-  if (c.bases_on_host) {
-    // the context's own pinned copy (the caller may change its words once this returns);
-    // the sketch kernels read it through the staging window
-    if (c.n_words && !words) throw InvalidArgument("null read set");
-    DropStagedBases(c, 0, /*release=*/false);
-    uint64_t* hw = c.h_words.reserve(c.n_words + 2);
-    if (c.n_words) std::memcpy(hw, words, c.n_words * sizeof(uint64_t));
-    c.d_words.release();
-  } else {
-    DropStagedBases(c, 0, /*release=*/true);
-  }
-  // one spare slot everywhere: an external query read rides at index n_reads
-  uint64_t* dw = c.bases_on_host ? nullptr : c.d_words.reserve(c.n_words + 2);
-  uint64_t* dwo = c.d_woff.reserve(n_reads + 2ULL);
-  uint32_t* dl = c.d_len.reserve(n_reads + 2ULL);
-  uint32_t* di = c.d_ids.reserve(n_reads + 2ULL);
-  // bases of the resident reads only (a rank of a partitioned run sketches its
-  // own range; lengths and ids of all reads are always resident)
-  c.res_first = res_first;
-  c.res_last = res_last;
-  // offsets, lengths, ids first (small, from pageable memory: behind the bases they
-  // would wait for the copy engine)
-  RVN_CUDA(cudaMemcpyAsync(dwo, c.h_woff.data(), (n_reads + 1ULL) * 8,
-                           cudaMemcpyHostToDevice, c.stream));
-  if (n_reads) {
-    RVN_CUDA(cudaMemcpyAsync(dl, c.h_len.data(), n_reads * 4ULL,
-                             cudaMemcpyHostToDevice, c.stream));
-    RVN_CUDA(cudaMemcpyAsync(di, c.h_ids.data(), n_reads * 4ULL,
-                             cudaMemcpyHostToDevice, c.stream));
-  }
-  RVN_CUDA(cudaStreamSynchronize(c.stream));
-  const uint64_t w0 = c.h_woff[res_first], w1 = c.h_woff[res_last];
-  c.up_pending = false;
-  c.p_off_uploaded = false;
-  if (c.bases_on_host) return;  // (async_upload has nothing left to do)
-  if (w1 > w0 && c.async_upload && res_last - res_first >= 1024) {
-    // everything small the next call would send host-to-device goes first: behind the
-    // bases it would wait for the copy engine (tile tables, pile offsets of stage 1)
-    EnsureTiles(c);
-    uint64_t* d_poff = c.p_off.reserve(n_reads + 1ULL);
-    RVN_CUDA(cudaMemcpyAsync(d_poff, c.h_pile_off.data(), (n_reads + 1ULL) * 8,
-                             cudaMemcpyHostToDevice, c.stream));
-    RVN_CUDA(cudaStreamSynchronize(c.stream));
-    c.p_off_uploaded = true;
-    // chunks that end at read boundaries, on the copy stream; the caller keeps
-    // `words` alive until the next call on this context has returned
-    constexpr uint32_t kChunks = 8;
-    if (!c.copy_stream) {
-      RVN_CUDA(cudaStreamCreateWithFlags(&c.copy_stream, cudaStreamNonBlocking));
-      RVN_CUDA(cudaEventCreateWithFlags(&c.up_fence, cudaEventDisableTiming));
-    }
-    while (c.up_events.size() < kChunks) {
-      cudaEvent_t ev;
-      RVN_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-      c.up_events.push_back(ev);
-    }
-    // (kernels of earlier calls may still read the old bases)
-    RVN_CUDA(cudaEventRecord(c.up_fence, c.stream));
-    RVN_CUDA(cudaStreamWaitEvent(c.copy_stream, c.up_fence, 0));
-    c.up_read_end.clear();
-    uint32_t r_prev = res_first;
-    for (uint32_t i = 1; i <= kChunks && r_prev < res_last; ++i) {
-      const uint64_t target = w0 + (w1 - w0) * i / kChunks;
-      uint32_t r = static_cast<uint32_t>(
-          std::lower_bound(c.h_woff.begin() + r_prev + 1, c.h_woff.begin() + res_last + 1, target) -
-          c.h_woff.begin());
-      if (i == kChunks || r > res_last) r = res_last;
-      const uint64_t a = c.h_woff[r_prev], b = c.h_woff[r];
-      if (b > a) {
-        RVN_CUDA(cudaMemcpyAsync(dw + a, words + a, (b - a) * 8, cudaMemcpyHostToDevice,
-                                 c.copy_stream));
-      }
-      RVN_CUDA(cudaEventRecord(c.up_events[c.up_read_end.size()], c.copy_stream));
-      c.up_read_end.push_back(r);
-      r_prev = r;
-    }
-    c.up_chunks = static_cast<uint32_t>(c.up_read_end.size());
-    c.up_pending = c.up_chunks > 0;
-  } else if (w1 > w0) {
-    RVN_CUDA(cudaMemcpyAsync(dw + w0, words + w0, (w1 - w0) * 8, cudaMemcpyHostToDevice,
-                             c.stream));
-    RVN_CUDA(cudaStreamSynchronize(c.stream));
-  }
 }
 
 RVN_API int rvn_reads_upload(rvn_ctx* ctx, const uint64_t* words,
@@ -380,65 +249,13 @@ RVN_API int rvn_map_external(rvn_ctx* ctx, const uint64_t* words, uint32_t len,
   return Guard(ctx, [&](Ctx& c) {
     if (!c.i_valid) throw StateError("Map before Minimize");
     if (len >= (1u << 31)) throw LimitError("read of 2^31 or more bases");
+    if (len && !words) throw InvalidArgument("null read");
     const uint32_t n = c.n_reads;
-    const uint64_t nw = (static_cast<uint64_t>(len) + 31) >> 5;
-    if (nw && !words) throw InvalidArgument("null read");
-    if (!c.bases_on_host) {
-      uint64_t* dw = c.d_words.reserve_keep(c.n_words + nw + 2, c.n_words, c.stream);
-      if (nw) {
-        RVN_CUDA(cudaMemcpyAsync(dw + c.n_words, words, nw * 8,
-                                 cudaMemcpyHostToDevice, c.stream));
-      }
-    }
-    EnsureTiles(c);
-    // extend the host/device tables by the spare slot
-    const uint64_t woff_tail[2] = {c.n_words, c.n_words + nw};
-    uint64_t tiles = 0;
-    if (len >= c.prm.k && len - c.prm.k + 1 >= c.prm.w) {
-      tiles = (len - c.prm.k + 1 + kSketchTile - 1) / kSketchTile;
-    }
-    const uint64_t tile_tail[2] = {c.h_tile_off[n], c.h_tile_off[n] + tiles};
-    RVN_CUDA(cudaMemcpyAsync(c.d_woff.get() + n, woff_tail, 16,
-                             cudaMemcpyHostToDevice, c.stream));
-    RVN_CUDA(cudaMemcpyAsync(c.d_tile_off.get() + n, tile_tail, 16,
-                             cudaMemcpyHostToDevice, c.stream));
-    RVN_CUDA(cudaMemcpyAsync(c.d_len.get() + n, &len, 4, cudaMemcpyHostToDevice,
-                             c.stream));
-    RVN_CUDA(cudaMemcpyAsync(c.d_ids.get() + n, &id, 4, cudaMemcpyHostToDevice,
-                             c.stream));
-    RVN_CUDA(cudaStreamSynchronize(c.stream));
-    c.h_woff.push_back(c.n_words + nw);
-    c.h_len.push_back(len);
-    c.h_ids.push_back(id);
-    c.h_tile_off.push_back(tile_tail[1]);
-    c.n_reads = n + 1;
-    c.s_valid = c.q_valid = c.qt_valid = false;
-    // the rider's bases are resident for the duration of the call (EnsureSketch
-    // refuses reads outside [res_first, res_last)); bases on the host: the rider takes a
-    // half of the staging window
-    const uint32_t res_first0 = c.res_first, res_last0 = c.res_last;
-    c.res_first = n;
-    c.res_last = n + 1;
-    auto restore = [&]() {
-      if (c.bases_on_host) DropStagedBases(c, n, /*release=*/false);
-      c.res_first = res_first0;
-      c.res_last = res_last0;
-      c.n_reads = n;
-      c.h_woff.pop_back(); c.h_len.pop_back(); c.h_ids.pop_back();
-      c.h_tile_off.pop_back();
-      c.s_valid = c.q_valid = c.qt_valid = false;
-    };
-    try {
-      if (c.bases_on_host) StageExternalBases(c, n, words);
-      // an id below an indexed id breaks the "kept postings are a suffix" shortcut
-      // only through avoid_symmetric, which compares ids, not indices: fine
-      MapRange(c, n, n + 1, avoid_equal != 0, avoid_symmetric != 0, minhash != 0,
-               want_filtered != 0);
-    } catch (...) {
-      restore();
-      throw;
-    }
-    restore();
+    RiderRead rider(c, words, len, id);
+    // an id below an indexed id breaks the "kept postings are a suffix" shortcut
+    // only through avoid_symmetric, which compares ids, not indices: fine
+    MapRange(c, n, n + 1, avoid_equal != 0, avoid_symmetric != 0, minhash != 0,
+             want_filtered != 0);
     TimerCollect(c);
   });
 }
@@ -916,10 +733,10 @@ RVN_API int rvn_debug_exclusive_scan(rvn_ctx* ctx, const uint32_t* in, uint64_t 
 
 RVN_API int rvn_reads_residency(rvn_ctx* ctx, int* on_host, uint64_t* device_word_bytes) {
   return Guard(ctx, [&](Ctx& c) {
-    if (on_host) *on_host = c.bases_on_host ? 1 : 0;
+    if (on_host) *on_host = c.bases.on_host ? 1 : 0;
     if (device_word_bytes) {
       *device_word_bytes =
-          c.bases_on_host ? StagedBaseBytes(c) : c.d_words.cap * sizeof(uint64_t);
+          c.bases.on_host ? StagedBaseBytes(c) : c.d_words.cap * sizeof(uint64_t);
     }
   }, /*sketches_first=*/true);
 }

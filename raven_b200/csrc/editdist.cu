@@ -295,9 +295,8 @@ void EditDistanceBatch(Ctx& c, uint64_t n, const uint32_t* lhs_read, const uint3
   for (uint64_t i = 0; i < n; ++i) {
     const uint32_t a = lhs_read[i], b = rhs_read[i];
     if (a >= c.n_reads || b >= c.n_reads) throw InvalidArgument("read index out of bounds");
-    if (a < c.res_first || a >= c.res_last || b < c.res_first || b >= c.res_last) {
-      throw StateError("the bases of these reads were not uploaded (rvn_reads_upload_range)");
-    }
+    CheckResident(c, a, a + 1);
+    CheckResident(c, b, b + 1);
     if (static_cast<uint64_t>(lhs_begin[i]) + lhs_len[i] > c.h_len[a] ||
         static_cast<uint64_t>(rhs_begin[i]) + rhs_len[i] > c.h_len[b]) {
       throw InvalidArgument("substring beyond the end of its read");

@@ -61,18 +61,24 @@ struct PhaseTimer {
   std::vector<cudaEvent_t> pool;
 };
 
-// One half of the staging window of packed bases (host_bases mode, sketch.cu): the words of
-// the read range [first, last), word w of the set at words[w - woff[first]]. The copy runs
-// on the context's copy stream in pieces: reads [.., read_end[i]) have arrived once
-// events[i] has completed. `used` is recorded on the context's stream behind the last kernel
-// that read the half; a new copy into it waits for that.
+// The words of a read range copied to the device on the context's copy stream in pieces cut
+// at read boundaries (bases.cu): reads [.., read_end[i]) have arrived once events[i] has
+// completed. n: the pieces of the last copy (the events are reused).
+struct CopyPieces {
+  std::vector<cudaEvent_t> events;
+  std::vector<uint32_t> read_end;
+  uint32_t n = 0;
+};
+
+// One half of the staging window of packed bases (host_bases mode): the words of the read
+// range [first, last), word w of the set at words[w - woff[first]], arriving in `copy`.
+// `used` is recorded on the context's stream behind the last kernel that read the half; a
+// new copy into it waits for that.
 struct BaseHalf {
   DevBuf<uint64_t> words;
   uint32_t first = 0, last = 0;
   bool valid = false;
-  std::vector<cudaEvent_t> events;
-  std::vector<uint32_t> read_end;
-  uint32_t pieces = 0;
+  CopyPieces copy;
   cudaEvent_t used = nullptr;
   bool used_recorded = false;
 };
@@ -90,6 +96,33 @@ struct BaseView {
   int half = -1;
 };
 
+// Where the packed bases of the uploaded reads are (bases.cu)
+struct Bases {
+  // option "host_bases": where rvn_reads_upload / rvn_reads_upload_ids keep the bases: 0 in
+  // d_words, 1 in the pinned host copy h_words (the sketch kernels read them from the staging
+  // window half[]), -1 (default) on the host only when a stage-1 pass at the reference's
+  // batch sizes would fit the device with them there and not without ("host_bases_budget"
+  // replaces the usable device memory when it is not 0)
+  int64_t host_bases = -1;
+  uint64_t host_bases_budget = 0;
+  bool on_host = false;  // the current upload's bases are in h_words only
+  PinBuf<uint64_t> h_words;
+  BaseHalf half[2];
+  int cur = 0;  // the half of the range a sketch asked for last
+  // reads whose bases the next sketch launch should be followed by a copy of (the range the
+  // driver sketches after it; empty: none)
+  uint32_t next_first = 0, next_last = 0;
+  uint32_t res_first = 0, res_last = 0;  // reads whose bases are in d_words
+  // option "async_upload": the bases travel to d_words on the copy stream in pieces, behind
+  // up_fence (recorded on the context's stream: kernels of earlier calls may still read the
+  // old bases). The next sketch launch starts on the pieces that have arrived, any other call
+  // waits for all of them (WaitUpload); upload.n = 0: none in flight.
+  int64_t async_upload = 0;
+  cudaStream_t copy_stream = nullptr;  // (the staging window's copies too)
+  cudaEvent_t up_fence = nullptr;
+  CopyPieces upload;
+};
+
 struct Ctx {
   // device bytes held by this context's buffers (first member: it outlives them)
   uint64_t held_bytes = 0;
@@ -97,15 +130,6 @@ struct Ctx {
   int sms = 132;  // multiprocessors of `device` (grid caps of the grid-stride kernels)
   cudaStream_t stream = nullptr;
   bool own_stream = false;
-  // option "async_upload": the packed bases travel on a copy stream in chunks; the
-  // sketch kernel of the next call starts on the reads that have arrived
-  int64_t async_upload = 0;
-  cudaStream_t copy_stream = nullptr;
-  cudaEvent_t up_fence = nullptr;
-  std::vector<cudaEvent_t> up_events;   // one per chunk (reused)
-  std::vector<uint32_t> up_read_end;    // reads [.., up_read_end[i]) are complete after chunk i
-  uint32_t up_chunks = 0;
-  bool up_pending = false;
   bool p_off_uploaded = false;  // stage-1 pile offsets already on the device
   std::string err;
   Params prm;
@@ -123,21 +147,7 @@ struct Ctx {
   // upload too: a context starts as an empty read set)
   std::vector<uint64_t> h_pile_off{0};
   bool ids_identity = true;  // id == index (needed by the device-side gather)
-  uint32_t res_first = 0, res_last = 0;  // reads whose bases are in HBM
-  // option "host_bases": where rvn_reads_upload / rvn_reads_upload_ids keep the packed bases:
-  // 0 in d_words, 1 in the pinned host copy h_words (the sketch kernels read them from the
-  // staging window bh[]), -1 (default) on the host only when a stage-1 pass at the
-  // reference's batch sizes would fit the device with them there and not without
-  // ("host_bases_budget" replaces the usable device memory when it is not 0)
-  int64_t host_bases = -1;
-  uint64_t host_bases_budget = 0;
-  bool bases_on_host = false;  // the current upload's bases are in h_words only
-  PinBuf<uint64_t> h_words;
-  BaseHalf bh[2];
-  int bh_cur = 0;  // the half of the range a sketch asked for last
-  // reads whose bases the next sketch launch should be followed by a copy of (the range the
-  // driver sketches after it; empty: none)
-  uint32_t bases_next_first = 0, bases_next_last = 0;
+  Bases bases;
   // sketch tiles: tile_off[r] = first tile of read r (depends on k)
   std::vector<uint64_t> h_tile_off;
   DevBuf<uint64_t> d_tile_off;
@@ -412,16 +422,20 @@ void TimerEnd(Ctx& c);
 void TimerCollect(Ctx& c);
 void TimerReset(Ctx& c);
 
-// ---- sketch.cu ----
-void EnsureTiles(Ctx& c);
-// full minimizers of reads [first,last) into c.s_* (no-op if already there)
-void EnsureSketch(Ctx& c, uint32_t first, uint32_t last);
-// micromizers of reads [first,last) into c.q_* (needs the sketch of a range
-// that contains [first,last))
+// ---- bases.cu ----
+// rvn_reads_upload*: the read tables and the bases (whole_set: rvn_reads_upload /
+// rvn_reads_upload_ids, where option host_bases applies)
+void UploadReads(Ctx& c, const uint64_t* words, const uint64_t* word_off, const uint32_t* lens,
+                 const uint32_t* ids, uint32_t n_reads, uint32_t res_first = 0,
+                 uint32_t res_last = 0xFFFFFFFFu, bool whole_set = false);
+// RVN_ERR_STATE unless the bases of reads [first, last) can be read: the range is empty, the
+// bases are on the host (a sketch stages its range), or it lies inside the resident range
+void CheckResident(const Ctx& c, uint32_t first, uint32_t last);
 void WaitUpload(Ctx& c);  // the context's stream waits for an asynchronous upload
 // The bases of reads [first, last) for a sketch launch: the device copy of the set, or
 // (host_bases) a half of the staging window that holds them, copied there now unless a half
-// already does. The caller waits for the view's pieces, launches, then calls BasesLaunched.
+// already does. The caller checks the range (CheckResident), waits for the view's pieces,
+// launches, then calls BasesLaunched.
 BaseView SketchBases(Ctx& c, uint32_t first, uint32_t last);
 // after the launches that read v: the half may be overwritten behind them, and the range
 // BasesNext named is copied into the other half now, beside the kernels that follow
@@ -429,11 +443,30 @@ void BasesLaunched(Ctx& c, const BaseView& v);
 // the read range the caller sketches next: staged right after the next sketch launch
 // (no-op with the bases on the device)
 void BasesNext(Ctx& c, uint32_t first, uint32_t last);
-// rvn_map_external's rider, read n, whose words are on the caller's host memory
-void StageExternalBases(Ctx& c, uint32_t n, const uint64_t* words);
-// the halves holding reads >= `from` forget them; release: every half frees its memory
-void DropStagedBases(Ctx& c, uint32_t from, bool release);
 uint64_t StagedBaseBytes(const Ctx& c);  // device bytes of the staging window
+// the calls that read bases at random positions: a set whose bases are on the host goes to
+// d_words whole first (the context is then in device mode until the next upload);
+// RVN_ERR_LIMIT when it does not fit the usable memory ("host_bases_budget" when not 0)
+void EnsureDeviceBases(Ctx& c);
+// rvn_map_external's rider: a read outside the uploaded set, its words in the caller's host
+// memory, rides in the spare slot n_reads while the guard lives: in the host and device
+// tables, as the resident range and, with the bases on the host, in a half of the staging
+// window. The destructor restores the set.
+struct RiderRead {
+  RiderRead(Ctx& c, const uint64_t* words, uint32_t len, uint32_t id);
+  RiderRead(const RiderRead&) = delete;
+  ~RiderRead();
+  Ctx& c;
+  const uint32_t n, res_first, res_last;  // the set's reads and resident range
+};
+void ReleaseBases(Ctx& c);  // rvn_ctx_destroy: the copy stream and the events
+
+// ---- sketch.cu ----
+void EnsureTiles(Ctx& c);
+// full minimizers of reads [first,last) into c.s_* (no-op if already there)
+void EnsureSketch(Ctx& c, uint32_t first, uint32_t last);
+// micromizers of reads [first,last) into c.q_* (needs the sketch of a range
+// that contains [first,last))
 void EnsureMicromizers(Ctx& c, uint32_t first, uint32_t last);
 void EnsureThresholds(Ctx& c, uint32_t first, uint32_t last);
 // The sketch records of reads [first, last) straight into the two tiers of an index build
@@ -635,10 +668,9 @@ void MapFlushes(Ctx& c, uint32_t first, uint32_t last, bool avoid_equal, bool av
 // option "host_bases" at an upload of the whole set (h_woff, h_len, h_pile_off are the new
 // set's): whether its bases stay on the host
 bool UseHostBases(const Ctx& c);
-// the calls that read bases at random positions: a set whose bases are on the host goes to
-// d_words whole first (the context is then in device mode until the next upload);
-// RVN_ERR_LIMIT when it does not fit the usable memory ("host_bases_budget" when not 0)
-void EnsureDeviceBases(Ctx& c);
+// device memory a pass can use: `budget`, or when that is 0 the free memory plus the
+// buffers this context already holds (a pass re-uses them)
+double UsableMemory(const Ctx& c, uint64_t budget);
 // rvn_minimize and rvn_filter (returns the occurrence threshold)
 void Minimize(Ctx& c, uint32_t first, uint32_t last, bool minhash);
 uint32_t Filter(Ctx& c, double freq);

@@ -890,15 +890,13 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
                            uint64_t tmax, bool tiers) {
   c.i_valid = false;
   c.occurrence = 0xFFFFFFFFu;
-  if (last > first && !c.bases_on_host && (first < c.res_first || last > c.res_last)) {
-    throw StateError("the bases of these reads were not uploaded (rvn_reads_upload_range)");
-  }
+  CheckResident(c, first, last);
   // (an asynchronous upload: every chunk's bases are there before the first sketch)
   WaitUpload(c);
   const std::vector<uint32_t> cuts = ChunkCuts(c, first, last, chunk);
   // staged bases: each sketch is followed by the copy of the range sketched next - the next
   // chunk, after sweep 1 the first chunk again, after the last the range the caller named
-  const uint32_t after_first = c.bases_next_first, after_last = c.bases_next_last;
+  const uint32_t after_first = c.bases.next_first, after_last = c.bases.next_last;
   auto stage_next = [&](size_t i, bool sweep1) {
     if (i + 2 < cuts.size()) {
       BasesNext(c, cuts[i + 1], cuts[i + 2]);

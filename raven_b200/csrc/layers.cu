@@ -190,14 +190,9 @@ void PolishWindows(Ctx& c, const PolishArgs& a) {
   if (c.n_reads == 0) throw StateError("no reads uploaded (rvn_reads_upload)");
   if (a.n_targets > c.n_reads) throw InvalidArgument("more targets than uploaded reads");
   const uint32_t T = a.n_targets, W = a.window;
-  auto resident = [&](uint32_t r) {
-    if (r < c.res_first || r >= c.res_last) {
-      throw StateError("the bases of these reads were not uploaded (rvn_reads_upload_range)");
-    }
-  };
   std::vector<uint64_t> first_window(T + 1ULL, 0);
   for (uint32_t t = 0; t < T; ++t) {
-    resident(t);
+    CheckResident(c, t, t + 1);
     first_window[t + 1] = first_window[t] + (c.h_len[t] + static_cast<uint64_t>(W) - 1) / W;
   }
   const uint64_t n_win64 = first_window[T];
@@ -222,7 +217,7 @@ void PolishWindows(Ctx& c, const PolishArgs& a) {
   for (uint64_t i = 0; i < A; ++i) {
     const uint32_t k = a.q_read[i], t = a.t_read[i];
     if (k >= c.n_reads || t >= T) throw InvalidArgument("read index out of bounds");
-    resident(k);
+    CheckResident(c, k, k + 1);
     const uint32_t L = c.h_len[k];
     if (static_cast<uint64_t>(a.q_begin[i]) + a.q_len[i] > L) {
       throw InvalidArgument("substring beyond the end of its read");

@@ -908,69 +908,6 @@ size_t SketchSmemBytes(uint32_t w, size_t hash_bytes) {
   return max_words * 8 + span * hash_bytes + 4 + 34 * 4 + span + 16;
 }
 
-// ---- the staging window (option host_bases) ----
-// A staged range of 1024 reads or more is copied in this many pieces of about equal words,
-// cut at read boundaries: the sketch of the reads of a piece starts when it has arrived.
-constexpr uint32_t kStagePieces = 8;
-
-void EnsureCopyStream(Ctx& c) {
-  if (c.copy_stream) return;
-  RVN_CUDA(cudaStreamCreateWithFlags(&c.copy_stream, cudaStreamNonBlocking));
-  RVN_CUDA(cudaEventCreateWithFlags(&c.up_fence, cudaEventDisableTiming));
-}
-
-// the half that holds every read of [first, last), -1 = none
-int HalfWith(const Ctx& c, uint32_t first, uint32_t last) {
-  for (int i = 0; i < 2; ++i) {
-    const BaseHalf& h = c.bh[i];
-    if (h.valid && h.first <= first && last <= h.last) return i;
-  }
-  return -1;
-}
-
-// Copy of the words of reads [first, last) (src: their words on the host, from the first
-// read's first word) into half i, on the copy stream behind every kernel that read the half.
-void StageRange(Ctx& c, int i, uint32_t first, uint32_t last, const uint64_t* src) {
-  BaseHalf& h = c.bh[i];
-  const uint64_t w0 = c.h_woff[first], w1 = c.h_woff[last];
-  h.valid = false;
-  EnsureCopyStream(c);
-  if (!h.used) RVN_CUDA(cudaEventCreateWithFlags(&h.used, cudaEventDisableTiming));
-  if (w1 - w0 + 2 > h.words.cap) {  // (growth frees the buffer: its readers must be done)
-    if (h.used_recorded) RVN_CUDA(cudaEventSynchronize(h.used));
-    RVN_CUDA(cudaStreamSynchronize(c.copy_stream));
-    h.words.reserve(w1 - w0 + 2);
-  }
-  if (h.used_recorded) RVN_CUDA(cudaStreamWaitEvent(c.copy_stream, h.used, 0));
-  const uint32_t pieces = last - first >= 1024 ? kStagePieces : 1;
-  while (h.events.size() < pieces) {
-    cudaEvent_t ev;
-    RVN_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    h.events.push_back(ev);
-  }
-  h.read_end.clear();
-  uint32_t r_prev = first;
-  for (uint32_t p = 1; p <= pieces && r_prev < last; ++p) {
-    const uint64_t target = w0 + (w1 - w0) * p / pieces;
-    uint32_t r = static_cast<uint32_t>(
-        std::lower_bound(c.h_woff.begin() + r_prev + 1, c.h_woff.begin() + last + 1, target) -
-        c.h_woff.begin());
-    if (p == pieces) r = last;
-    const uint64_t a = c.h_woff[r_prev], b = c.h_woff[r];
-    if (b > a) {
-      RVN_CUDA(cudaMemcpyAsync(h.words.get() + (a - w0), src + (a - w0), (b - a) * 8,
-                               cudaMemcpyHostToDevice, c.copy_stream));
-    }
-    RVN_CUDA(cudaEventRecord(h.events[h.read_end.size()], c.copy_stream));
-    h.read_end.push_back(r);
-    r_prev = r;
-  }
-  h.pieces = static_cast<uint32_t>(h.read_end.size());
-  h.first = first;
-  h.last = last;
-  h.valid = true;
-}
-
 // the context's stream waits for piece p of v; with staged bases, phase "stage_bases" is
 // that wait: the copy time no kernel hid
 void WaitPiece(Ctx& c, const BaseView& v, uint32_t p) {
@@ -1009,82 +946,6 @@ void LaunchFastPieces(Ctx& c, const BaseView& v, uint32_t first, uint32_t last,
 }
 
 }  // namespace
-
-BaseView SketchBases(Ctx& c, uint32_t first, uint32_t last) {
-  BaseView v;
-  if (!c.bases_on_host) {
-    if (first < last && (first < c.res_first || last > c.res_last)) {
-      throw StateError("the bases of these reads were not uploaded (rvn_reads_upload_range)");
-    }
-    v.words = c.d_words.get();
-    if (c.up_pending) {  // (an asynchronous upload in flight: its chunks are the pieces)
-      v.events = c.up_events.data();
-      v.read_end = c.up_read_end.data();
-      v.pieces = c.up_chunks;
-      c.up_pending = false;
-    }
-    return v;
-  }
-  int i = HalfWith(c, first, last);
-  if (i < 0) {
-    i = 1 - c.bh_cur;
-    StageRange(c, i, first, last, c.h_words.get() + c.h_woff[first]);
-  }
-  c.bh_cur = i;
-  const BaseHalf& h = c.bh[i];
-  v.words = h.words.get();
-  v.base = c.h_woff[h.first];
-  v.events = h.events.data();
-  v.read_end = h.read_end.data();
-  v.pieces = h.pieces;
-  v.half = i;
-  return v;
-}
-
-void BasesLaunched(Ctx& c, const BaseView& v) {
-  if (v.half < 0) return;
-  BaseHalf& h = c.bh[v.half];
-  RVN_CUDA(cudaEventRecord(h.used, c.stream));
-  h.used_recorded = true;
-  const uint32_t a = c.bases_next_first, b = c.bases_next_last;
-  c.bases_next_first = c.bases_next_last = 0;
-  if (a < b && b <= c.n_reads && HalfWith(c, a, b) < 0) {
-    StageRange(c, 1 - v.half, a, b, c.h_words.get() + c.h_woff[a]);
-  }
-}
-
-void BasesNext(Ctx& c, uint32_t first, uint32_t last) {
-  if (!c.bases_on_host) return;
-  c.bases_next_first = first;
-  c.bases_next_last = last;
-}
-
-void StageExternalBases(Ctx& c, uint32_t n, const uint64_t* words) {
-  StageRange(c, 1 - c.bh_cur, n, n + 1, words);
-}
-
-void DropStagedBases(Ctx& c, uint32_t from, bool release) {
-  for (BaseHalf& h : c.bh) {
-    if (h.valid && h.last > from) h.valid = false;
-    if (release && h.words.cap) {
-      if (h.used_recorded) RVN_CUDA(cudaEventSynchronize(h.used));
-      if (c.copy_stream) RVN_CUDA(cudaStreamSynchronize(c.copy_stream));
-      h.words.release();
-      h.valid = false;
-    }
-  }
-  c.bases_next_first = c.bases_next_last = 0;
-}
-
-uint64_t StagedBaseBytes(const Ctx& c) {
-  return (c.bh[0].words.cap + c.bh[1].words.cap) * sizeof(uint64_t);
-}
-
-void WaitUpload(Ctx& c) {
-  if (!c.up_pending) return;
-  RVN_CUDA(cudaStreamWaitEvent(c.stream, c.up_events[c.up_chunks - 1], 0));
-  c.up_pending = false;
-}
 
 void EnsureTiles(Ctx& c) {
   if (c.tiles_k == c.prm.k && c.h_tile_off.size() == c.n_reads + 1ULL) return;
@@ -1125,9 +986,7 @@ void EnsureTiles(Ctx& c) {
 
 void EnsureSketch(Ctx& c, uint32_t first, uint32_t last) {
   if (c.s_valid && c.s_first == first && c.s_last == last) return;
-  if (first < last && !c.bases_on_host && (first < c.res_first || last > c.res_last)) {
-    throw StateError("the bases of these reads were not uploaded (rvn_reads_upload_range)");
-  }
+  CheckResident(c, first, last);
   EnsureTiles(c);
   c.s_valid = false;
   c.q_valid = false;
@@ -1222,9 +1081,7 @@ bool SketchTiersFused(const Ctx& c) { return 2 * c.prm.k <= 30 && c.prm.w == 5; 
 void SketchTiers(Ctx& c, uint32_t first, uint32_t last, uint32_t limit, uint32_t* a_val,
                  uint64_t* a_org, uint64_t cap_a, uint32_t* b_val, uint64_t cap_b,
                  uint64_t* n_a, uint64_t* n_b) {
-  if (first < last && !c.bases_on_host && (first < c.res_first || last > c.res_last)) {
-    throw StateError("the bases of these reads were not uploaded (rvn_reads_upload_range)");
-  }
+  CheckResident(c, first, last);
   EnsureTiles(c);
   WaitUpload(c);
   *n_a = *n_b = 0;
@@ -1255,9 +1112,7 @@ void SketchTiers(Ctx& c, uint32_t first, uint32_t last, uint32_t limit, uint32_t
 
 void SketchAppend(Ctx& c, uint32_t first, uint32_t last, uint32_t* out_val, uint64_t* out_org,
                   uint64_t base, uint64_t cap) {
-  if (first < last && !c.bases_on_host && (first < c.res_first || last > c.res_last)) {
-    throw StateError("the bases of these reads were not uploaded (rvn_reads_upload_range)");
-  }
+  CheckResident(c, first, last);
   EnsureTiles(c);
   WaitUpload(c);
   const uint64_t n_tiles = c.h_tile_off[last] - c.h_tile_off[first];

@@ -150,15 +150,6 @@ Footprint Stage1Footprint(const Ctx& c, const std::vector<Batch>& batches, uint6
   return f;
 }
 
-// device memory a pass can use: `budget`, or when that is 0 the free memory plus the
-// buffers this context already holds (a pass re-uses them)
-double UsableMemory(const Ctx& c, uint64_t budget) {
-  if (budget) return static_cast<double>(budget);
-  size_t free_b = 0, total_b = 0;
-  RVN_CUDA(cudaMemGetInfo(&free_b, &total_b));
-  return static_cast<double>(free_b) + static_cast<double>(c.held_bytes);
-}
-
 // Option "index_chunk_bases": the chunk size of an index build, 0 = one-shot.
 // -1 (auto): chunks of kAutoIndexChunk bases only when `one_shot`, the caller's estimate
 // of its device memory with one-shot builds, exceeds the usable memory
@@ -170,7 +161,7 @@ uint64_t IndexChunk(const Ctx& c, double one_shot) {
 
 // a stage-1 pass with one-shot builds: resident, or windowed (max_overlaps permitting)
 double Stage1OneShot(const Ctx& c, const std::vector<Batch>& batches, uint64_t kmax) {
-  const Footprint f = Stage1Footprint(c, batches, kmax, 0, c.bases_on_host);
+  const Footprint f = Stage1Footprint(c, batches, kmax, 0, c.bases.on_host);
   return kmax <= kWindowMaxOverlaps ? std::min(f.resident, f.windowed_device) : f.resident;
 }
 
@@ -185,7 +176,7 @@ double MinimizeFootprint(const Ctx& c, uint32_t first, uint32_t last, uint64_t c
   const double bb = static_cast<double>(ReadBases(c, first, last));
   const double sketched = chunk ? std::min(bb, static_cast<double>(chunk)) : bb;
   const std::vector<Batch> batch{Batch{first, last, {}}};
-  return BasesBytes(c, batch, chunk, c.bases_on_host) + 32.0 * c.n_reads +
+  return BasesBytes(c, batch, chunk, c.bases.on_host) + 32.0 * c.n_reads +
          kUntieredIndexBytesPerBase * bb + kChunkSketchBytesPerBase * sketched;
 }
 
@@ -221,7 +212,7 @@ uint64_t MapFlushBases(const Ctx& c, uint64_t range_bases, bool join) {
 bool UseWindow(Ctx& c, const std::vector<Batch>& batches, uint64_t kmax, uint64_t chunk) {
   if (c.stage1_window >= 0) return c.stage1_window != 0;
   if (kmax > kWindowMaxOverlaps) return false;
-  const Footprint f = Stage1Footprint(c, batches, kmax, chunk, c.bases_on_host);
+  const Footprint f = Stage1Footprint(c, batches, kmax, chunk, c.bases.on_host);
   const double budget = UsableMemory(c, c.stage1_window_budget);
   if (f.resident <= budget) return false;
   const double host_free = static_cast<double>(sysconf(_SC_AVPHYS_PAGES)) *
@@ -576,9 +567,7 @@ void Stage2(Ctx& c, double freq, double identity, uint32_t n, const uint32_t* h_
             const uint32_t* h_rend) {
   if (n > c.n_reads) throw InvalidArgument("more valid reads than uploaded reads");
   if (n && (!h_rbeg || !h_rend)) throw InvalidArgument("null regions");
-  if (n && (c.res_first > 0 || c.res_last < n)) {
-    throw StateError("the bases of the valid reads were not uploaded");
-  }
+  CheckResident(c, 0, n);
   c.s2_valid = false;
   uint32_t max_id = 0;
   for (uint32_t i = 0; i < n; ++i) {
@@ -718,7 +707,7 @@ void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
     return std::make_pair(cuts[0], cuts[1]);
   };
   auto stage_after = [&](size_t bi, size_t fi) {  // the range after flush fi - 1 of batch bi
-    if (!c.bases_on_host) return;
+    if (!c.bases.on_host) return;
     for (size_t i = fi; i < batches[bi].flushes.size(); ++i) {
       if (probes(batches[bi], batches[bi].flushes[i])) {
         BasesNext(c, batches[bi].flushes[i].first, batches[bi].flushes[i].second);
@@ -804,42 +793,29 @@ void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
 }
 
 bool UseHostBases(const Ctx& c) {
-  if (c.host_bases >= 0) return c.host_bases != 0;
+  if (c.bases.host_bases >= 0) return c.bases.host_bases != 0;
   if (c.n_reads == 0) return false;
   // the windowed, chunked pass of the reference's schedule at its default max_overlaps
   const std::vector<Batch> batches = Schedule(c, 0, 0);
-  const double usable = UsableMemory(c, c.host_bases_budget);
+  const double usable = UsableMemory(c, c.bases.host_bases_budget);
   if (Stage1Footprint(c, batches, 32, kAutoIndexChunk, false).windowed_device <= usable) {
     return false;
   }
   return Stage1Footprint(c, batches, 32, kAutoIndexChunk, true).windowed_device <= usable;
 }
 
-void EnsureDeviceBases(Ctx& c) {
-  if (!c.bases_on_host) return;
-  const uint64_t bytes = (c.n_words + 2) * sizeof(uint64_t);
-  const double usable = UsableMemory(c, c.host_bases_budget);
-  if (static_cast<double>(bytes) > usable) {
-    throw LimitError("the packed bases of the whole read set (" + std::to_string(bytes) +
-                     " bytes) do not fit the device (" +
-                     std::to_string(static_cast<uint64_t>(usable)) + " bytes usable)");
-  }
-  RVN_CUDA(cudaStreamSynchronize(c.stream));
-  DropStagedBases(c, 0, /*release=*/true);
-  uint64_t* dw = c.d_words.reserve(c.n_words + 2);
-  RVN_CUDA(cudaMemcpyAsync(dw, c.h_words.get(), c.n_words * sizeof(uint64_t),
-                           cudaMemcpyHostToDevice, c.stream));
-  RVN_CUDA(cudaStreamSynchronize(c.stream));
-  c.bases_on_host = false;
-  c.res_first = 0;
-  c.res_last = c.n_reads;
+double UsableMemory(const Ctx& c, uint64_t budget) {
+  if (budget) return static_cast<double>(budget);
+  size_t free_b = 0, total_b = 0;
+  RVN_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  return static_cast<double>(free_b) + static_cast<double>(c.held_bytes);
 }
 
 void Stage1Footprints(const Ctx& c, uint64_t kmax, uint64_t ib, uint64_t qb,
                       uint64_t* resident, uint64_t* windowed_device, uint64_t* windowed_host) {
   const std::vector<Batch> batches = Schedule(c, ib, qb);
   const Footprint f = Stage1Footprint(
-      c, batches, kmax, IndexChunk(c, Stage1OneShot(c, batches, kmax)), c.bases_on_host);
+      c, batches, kmax, IndexChunk(c, Stage1OneShot(c, batches, kmax)), c.bases.on_host);
   if (resident) *resident = static_cast<uint64_t>(f.resident);
   if (windowed_device) *windowed_device = static_cast<uint64_t>(f.windowed_device);
   if (windowed_host) *windowed_host = static_cast<uint64_t>(f.windowed_host);
