@@ -130,6 +130,30 @@ int rvn_reads_upload_ids(rvn_ctx* ctx, const uint64_t* words,
                          const uint64_t* word_off, const uint32_t* lens,
                          const uint32_t* ids, uint32_t n_reads);
 
+/* raven's input loop (RavenExe/src/main.cc:258-299: raven::CreateParser, RavenLib/src/io.cc:7-41,
+ * then Parse(-1) per file, files concatenated in order, empty files skipped) with the records
+ * parsed and packed on the device; the result is the context's read set (ids 0..n-1), as after
+ * rvn_reads_upload. sizes (may be NULL): reads, words, block qualities, name bytes.
+ * Plain and gzip files (multi-member included) are read with zlib's gzread on a thread of the
+ * library's own, in chunks of option "fastx_chunk_bytes" (results do not depend on it).
+ * Option "host_bases" applies to the parsed set. Errors: RVN_ERR_INVALID with the message
+ * the reference's loop prints for the first failing record in file order (an unsupported
+ * suffix, a file that cannot be opened, "invalid file format" wherever the drop-in FASTA or
+ * FASTQ parser throws, "not a nucleotide"); RVN_ERR_LIMIT for a read of 2^31 bases or more,
+ * or words that do not fit the device while the set is parsed (naming the bytes). After a
+ * failed call the context holds no read set (the calls on reads are RVN_ERR_STATE until the
+ * next upload). Phases in rvn_get_timings: "fastx_read" (host read or inflate that nothing
+ * hid), "fastx_copy" and "fastx_parse" (per chunk). */
+int rvn_reads_upload_files(rvn_ctx* ctx, const char* const* paths, uint32_t n_paths,
+                           uint64_t sizes[4]);
+
+/* Host copies of the parsed set; any pointer may be NULL. bq_off as rvn_polish_windows takes it
+ * (an empty range for a FASTA read); names are cut at the first white space, as raven's parser
+ * does, name i = names[name_off[i] .. name_off[i+1]). RVN_ERR_STATE if the current set was not
+ * made by rvn_reads_upload_files. */
+int rvn_reads_parsed(rvn_ctx* ctx, uint64_t* words, uint64_t* word_off, uint32_t* lens,
+                     uint8_t* block_quality, uint64_t* bq_off, char* names, uint64_t* name_off);
+
 /* Where the packed bases of the current upload live (option "host_bases"): *on_host = 1
  * when they stay in the context's pinned host copy and the sketch kernels read them from a
  * staging window, 0 when the device holds the whole set; *device_word_bytes = the device
@@ -504,7 +528,8 @@ int rvn_get_stats(rvn_ctx* ctx, rvn_stats* out);
  * upload); "index_chunk_budget" (bytes: replaces the free device memory in that auto
  * decision, 0 = the free memory); "map_flush_bases" (rvn_map cuts its range into flushes of
  * >= N query bases; 0 = the default, from the device memory; for tests of the flush
- * path, results do not depend on it); "stage2_batch_bases" (rvn_find_overlaps_and_repetitive_
+ * path, results do not depend on it); "fastx_chunk_bytes" (text bytes rvn_reads_upload_files
+ * parses per chunk; 0 = the default, 256 MiB; results do not depend on it); "stage2_batch_bases" (rvn_find_overlaps_and_repetitive_
  * regions cuts its index batches at >= N bases instead of the reference's 1U << 30; 0 = the
  * reference's cut; for tests of the multi-batch path: it changes what the reference's
  * schedule would compute at that cut); "poa_wide" and "poa_scratch_budget" (rvn_poa_batch and

@@ -26,6 +26,7 @@
 #include "raven/graph/overlap_utils.h"
 #include "raven/pile.h"
 #include "raven_b200.h"
+#include "raven_b200/load_sequences.hpp"  // raven_b200::LoadSequences
 #include "raven_b200/overlap_clip.hpp"
 #include "thread_pool/thread_pool.hpp"
 

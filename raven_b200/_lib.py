@@ -41,6 +41,9 @@ SIGNATURES = {
     "rvn_reads_upload_range": (C.c_int, [C.c_void_p, U64P, U64P, U32P, C.c_uint32,
                                          C.c_uint32, C.c_uint32]),
     "rvn_reads_upload_ids": (C.c_int, [C.c_void_p, U64P, U64P, U32P, U32P, C.c_uint32]),
+    "rvn_reads_upload_files": (C.c_int, [C.c_void_p, C.POINTER(C.c_char_p), C.c_uint32, U64P]),
+    "rvn_reads_parsed": (C.c_int, [C.c_void_p, U64P, U64P, U32P, C.POINTER(C.c_uint8), U64P,
+                                   C.c_void_p, U64P]),
     "rvn_reads_residency": (C.c_int, [C.c_void_p, C.POINTER(C.c_int), U64P]),
     "rvn_map_external": (C.c_int, [C.c_void_p, U64P, C.c_uint32, C.c_uint32, C.c_int,
                                    C.c_int, C.c_int, C.c_int]),

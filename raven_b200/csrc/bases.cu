@@ -116,18 +116,15 @@ void RestoreSet(const RiderRead& r) {
   c.s_valid = c.q_valid = c.qt_valid = false;
 }
 
-}  // namespace
-
-void UploadReads(Ctx& c, const uint64_t* words, const uint64_t* word_off, const uint32_t* lens,
-                 const uint32_t* ids, uint32_t n_reads, uint32_t res_first, uint32_t res_last,
-                 bool whole_set) {
-  Bases& b = c.bases;
+// The host read tables of a new set (offsets, lengths, pile offsets, ids); the device
+// buffers of the old set are idle when this returns.
+void SetReadTables(Ctx& c, const uint64_t* word_off, const uint32_t* lens, const uint32_t* ids,
+                   uint32_t n_reads) {
   if (n_reads && (!word_off || !lens)) throw InvalidArgument("null read set");
-  res_last = std::min(res_last, n_reads);
-  if (res_first > res_last) throw InvalidArgument("resident range out of bounds");
   if (n_reads == 0xFFFFFFFFu) throw LimitError("too many reads");
   c.s_valid = c.q_valid = c.qt_valid = c.i_valid = c.r_valid = c.st_valid = false;
   c.st_piles_on_device = false;
+  c.reads_unset = c.fx_valid = false;
   c.tiles_k = 0;
   c.n_reads = n_reads;
   c.h_woff.assign(1, 0);
@@ -152,7 +149,37 @@ void UploadReads(Ctx& c, const uint64_t* words, const uint64_t* word_off, const 
   c.n_words = c.h_woff[n_reads];
   // (kernels and copies of earlier calls may still use the buffers of the old bases)
   RVN_CUDA(cudaStreamSynchronize(c.stream));
-  if (b.copy_stream) RVN_CUDA(cudaStreamSynchronize(b.copy_stream));
+  if (c.bases.copy_stream) RVN_CUDA(cudaStreamSynchronize(c.bases.copy_stream));
+}
+
+// offsets, lengths, ids to the device (small, from pageable memory: behind the bases they
+// would wait for the copy engine); one spare slot everywhere: an external query read rides
+// at index n_reads
+void UploadReadTables(Ctx& c) {
+  const uint32_t n_reads = c.n_reads;
+  uint64_t* dwo = c.d_woff.reserve(n_reads + 2ULL);
+  uint32_t* dl = c.d_len.reserve(n_reads + 2ULL);
+  uint32_t* di = c.d_ids.reserve(n_reads + 2ULL);
+  RVN_CUDA(cudaMemcpyAsync(dwo, c.h_woff.data(), (n_reads + 1ULL) * 8,
+                           cudaMemcpyHostToDevice, c.stream));
+  if (n_reads) {
+    RVN_CUDA(cudaMemcpyAsync(dl, c.h_len.data(), n_reads * 4ULL,
+                             cudaMemcpyHostToDevice, c.stream));
+    RVN_CUDA(cudaMemcpyAsync(di, c.h_ids.data(), n_reads * 4ULL,
+                             cudaMemcpyHostToDevice, c.stream));
+  }
+  RVN_CUDA(cudaStreamSynchronize(c.stream));
+}
+
+}  // namespace
+
+void UploadReads(Ctx& c, const uint64_t* words, const uint64_t* word_off, const uint32_t* lens,
+                 const uint32_t* ids, uint32_t n_reads, uint32_t res_first, uint32_t res_last,
+                 bool whole_set) {
+  Bases& b = c.bases;
+  res_last = std::min(res_last, n_reads);
+  if (res_first > res_last) throw InvalidArgument("resident range out of bounds");
+  SetReadTables(c, word_off, lens, ids, n_reads);
   b.on_host = whole_set && UseHostBases(c);
   if (b.on_host) {
     // the context's own pinned copy (the caller may change its words once this returns);
@@ -165,26 +192,12 @@ void UploadReads(Ctx& c, const uint64_t* words, const uint64_t* word_off, const 
   } else {
     DropStagedBases(c, 0, /*release=*/true);
   }
-  // one spare slot everywhere: an external query read rides at index n_reads
   uint64_t* dw = b.on_host ? nullptr : c.d_words.reserve(c.n_words + 2);
-  uint64_t* dwo = c.d_woff.reserve(n_reads + 2ULL);
-  uint32_t* dl = c.d_len.reserve(n_reads + 2ULL);
-  uint32_t* di = c.d_ids.reserve(n_reads + 2ULL);
   // bases of the resident reads only (a rank of a partitioned run sketches its
   // own range; lengths and ids of all reads are always resident)
   b.res_first = res_first;
   b.res_last = res_last;
-  // offsets, lengths, ids first (small, from pageable memory: behind the bases they
-  // would wait for the copy engine)
-  RVN_CUDA(cudaMemcpyAsync(dwo, c.h_woff.data(), (n_reads + 1ULL) * 8,
-                           cudaMemcpyHostToDevice, c.stream));
-  if (n_reads) {
-    RVN_CUDA(cudaMemcpyAsync(dl, c.h_len.data(), n_reads * 4ULL,
-                             cudaMemcpyHostToDevice, c.stream));
-    RVN_CUDA(cudaMemcpyAsync(di, c.h_ids.data(), n_reads * 4ULL,
-                             cudaMemcpyHostToDevice, c.stream));
-  }
-  RVN_CUDA(cudaStreamSynchronize(c.stream));
+  UploadReadTables(c);
   const uint64_t w0 = c.h_woff[res_first], w1 = c.h_woff[res_last];
   b.upload.n = 0;
   c.p_off_uploaded = false;
@@ -210,6 +223,29 @@ void UploadReads(Ctx& c, const uint64_t* words, const uint64_t* word_off, const 
                              c.stream));
     RVN_CUDA(cudaStreamSynchronize(c.stream));
   }
+}
+
+void AdoptParsedReads(Ctx& c, const uint64_t* word_off, const uint32_t* lens, uint32_t n_reads) {
+  Bases& b = c.bases;
+  SetReadTables(c, word_off, lens, nullptr, n_reads);
+  b.on_host = UseHostBases(c);
+  if (b.on_host) {
+    DropStagedBases(c, 0, /*release=*/false);
+    uint64_t* hw = b.h_words.reserve(c.n_words + 2);
+    if (c.n_words) {
+      RVN_CUDA(cudaMemcpyAsync(hw, c.d_words.get(), c.n_words * sizeof(uint64_t),
+                               cudaMemcpyDeviceToHost, c.stream));
+      RVN_CUDA(cudaStreamSynchronize(c.stream));
+    }
+    c.d_words.release();
+  } else {
+    DropStagedBases(c, 0, /*release=*/true);
+  }
+  b.res_first = 0;
+  b.res_last = n_reads;
+  UploadReadTables(c);
+  b.upload.n = 0;
+  c.p_off_uploaded = false;
 }
 
 void CheckResident(const Ctx& c, uint32_t first, uint32_t last) {

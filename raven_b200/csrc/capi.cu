@@ -49,7 +49,13 @@ int Guard(rvn_ctx* ctx, F&& f, bool sketches_first = false) {
   }
 }
 
+// the calls that work on the uploaded reads
+void CheckReadSet(const Ctx& c) {
+  if (c.reads_unset) throw StateError("no read set: the last rvn_reads_upload_files failed");
+}
+
 void CheckRange(const Ctx& c, uint32_t first, uint32_t last) {
+  CheckReadSet(c);
   if (first > last || last > c.n_reads) {
     throw InvalidArgument("read range out of bounds");
   }
@@ -93,6 +99,9 @@ void SetOption(Ctx& c, const char* name, int64_t value) {
   } else if (name && std::strcmp(name, "map_flush_bases") == 0) {
     if (value < 0) throw InvalidArgument("map_flush_bases: bases, 0 = from the device memory");
     c.map_flush_bases = static_cast<uint64_t>(value);
+  } else if (name && std::strcmp(name, "fastx_chunk_bytes") == 0) {
+    if (value < 0) throw InvalidArgument("fastx_chunk_bytes: bytes, 0 = 256 MiB");
+    c.fastx_chunk_bytes = static_cast<uint64_t>(value);
   } else if (name && std::strcmp(name, "stage2_batch_bases") == 0) {
     if (value < 0) throw InvalidArgument("stage2_batch_bases: bases, 0 = the reference's 2^30");
     c.stage2_batch_bases = static_cast<uint64_t>(value);
@@ -241,12 +250,36 @@ RVN_API int rvn_reads_upload_ids(rvn_ctx* ctx, const uint64_t* words,
   }, /*sketches_first=*/true);
 }
 
+RVN_API int rvn_reads_upload_files(rvn_ctx* ctx, const char* const* paths, uint32_t n_paths,
+                                   uint64_t sizes[4]) {
+  return Guard(ctx, [&](Ctx& c) {
+    if (n_paths && !paths) throw InvalidArgument("null paths");
+    UploadFiles(c, paths, n_paths);
+    TimerCollect(c);
+    if (sizes) {
+      sizes[0] = c.n_reads;
+      sizes[1] = c.n_words;
+      sizes[2] = c.fx_bq.size();
+      sizes[3] = c.fx_names.size();
+    }
+  });
+}
+
+RVN_API int rvn_reads_parsed(rvn_ctx* ctx, uint64_t* words, uint64_t* word_off, uint32_t* lens,
+                             uint8_t* block_quality, uint64_t* bq_off, char* names,
+                             uint64_t* name_off) {
+  return Guard(ctx, [&](Ctx& c) {
+    ParsedReads(c, words, word_off, lens, block_quality, bq_off, names, name_off);
+  });
+}
+
 // Map one read that is not part of the uploaded set (it rides in the spare
 // slot behind the set for the duration of the call)
 RVN_API int rvn_map_external(rvn_ctx* ctx, const uint64_t* words, uint32_t len,
                              uint32_t id, int avoid_equal, int avoid_symmetric,
                              int minhash, int want_filtered) {
   return Guard(ctx, [&](Ctx& c) {
+    CheckReadSet(c);
     if (!c.i_valid) throw StateError("Map before Minimize");
     if (len >= (1u << 31)) throw LimitError("read of 2^31 or more bases");
     if (len && !words) throw InvalidArgument("null read");
@@ -410,6 +443,7 @@ RVN_API int rvn_find_overlaps_and_create_piles(rvn_ctx* ctx, double frequency,
                                                uint64_t index_batch_bases,
                                                uint64_t query_batch_bases) {
   return Guard(ctx, [&](Ctx& c) {
+    CheckReadSet(c);
     Stage1(c, frequency, max_overlaps, minhash != 0, index_batch_bases,
            query_batch_bases);
   }, /*sketches_first=*/true);
@@ -420,6 +454,7 @@ RVN_API int rvn_find_overlaps_and_repetitive_regions(rvn_ctx* ctx, double freque
                                                      const uint32_t* region_begin,
                                                      const uint32_t* region_end) {
   return Guard(ctx, [&](Ctx& c) {
+    CheckReadSet(c);
     EnsureDeviceBases(c);
     Stage2(c, frequency, identity, n_valid, region_begin, region_end);
     TimerCollect(c);

@@ -148,6 +148,16 @@ struct Ctx {
   std::vector<uint64_t> h_pile_off{0};
   bool ids_identity = true;  // id == index (needed by the device-side gather)
   Bases bases;
+  // ---- rvn_reads_upload_files (fastx.cu) ----
+  // option "fastx_chunk_bytes": text bytes parsed per chunk (0: 256 MiB)
+  uint64_t fastx_chunk_bytes = 0;
+  bool reads_unset = false;  // a failed rvn_reads_upload_files left no read set
+  // the current set was made by rvn_reads_upload_files: its block qualities (bq_off as
+  // rvn_polish_windows takes it) and names (name i = fx_names[fx_name_off[i], [i + 1]))
+  bool fx_valid = false;
+  std::vector<uint8_t> fx_bq;
+  std::vector<uint64_t> fx_bq_off, fx_name_off;
+  std::string fx_names;
   // sketch tiles: tile_off[r] = first tile of read r (depends on k)
   std::vector<uint64_t> h_tile_off;
   DevBuf<uint64_t> d_tile_off;
@@ -428,6 +438,9 @@ void TimerReset(Ctx& c);
 void UploadReads(Ctx& c, const uint64_t* words, const uint64_t* word_off, const uint32_t* lens,
                  const uint32_t* ids, uint32_t n_reads, uint32_t res_first = 0,
                  uint32_t res_last = 0xFFFFFFFFu, bool whole_set = false);
+// rvn_reads_upload_files: the set whose words the parse left in d_words (word_off, lens:
+// its tables) becomes the context's read set as after UploadReads of the same words
+void AdoptParsedReads(Ctx& c, const uint64_t* word_off, const uint32_t* lens, uint32_t n_reads);
 // RVN_ERR_STATE unless the bases of reads [first, last) can be read: the range is empty, the
 // bases are on the host (a sketch stages its range), or it lies inside the resident range
 void CheckResident(const Ctx& c, uint32_t first, uint32_t last);
@@ -460,6 +473,12 @@ struct RiderRead {
   const uint32_t n, res_first, res_last;  // the set's reads and resident range
 };
 void ReleaseBases(Ctx& c);  // rvn_ctx_destroy: the copy stream and the events
+
+// ---- fastx.cu ----
+// rvn_reads_upload_files and rvn_reads_parsed (include/raven_b200.h)
+void UploadFiles(Ctx& c, const char* const* paths, uint32_t n_paths);
+void ParsedReads(Ctx& c, uint64_t* words, uint64_t* word_off, uint32_t* lens,
+                 uint8_t* block_quality, uint64_t* bq_off, char* names, uint64_t* name_off);
 
 // ---- sketch.cu ----
 void EnsureTiles(Ctx& c);

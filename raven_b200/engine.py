@@ -16,10 +16,11 @@ Errors: the reference throws ``std::invalid_argument`` for a frequency outside
 from __future__ import annotations
 
 import ctypes as C
+import os
 
 import numpy as np
 
-from . import _lib
+from . import _lib, seqio
 from ._lib import OVLP, U16P, U32P, U64P, Overlap, Stats
 
 _ERR = {-1: ValueError, -2: RuntimeError, -3: RuntimeError, -4: OverflowError}
@@ -109,6 +110,38 @@ class Engine:
                 self.h, words.ctypes.data_as(U64P), woff.ctypes.data_as(U64P),
                 lens.ctypes.data_as(U32P), rs.n, resident[0], resident[1]))
         self.n_reads = rs.n
+
+    def upload_files(self, paths, words=False):
+        """raven's input loop over FASTA / FASTQ(.gz) files (RavenExe/src/main.cc:258-299)
+        with the records parsed and packed on the device, as the read set (ids 0..n-1): a
+        seqio.ReadSet with lengths, word offsets, block qualities (an empty range for a FASTA
+        read) and names, and the words when ``words`` is true. A malformed file raises
+        ValueError with the reference's message."""
+        enc = [os.fsencode(p) for p in paths]
+        arr = (C.c_char_p * max(1, len(enc)))(*enc)
+        sizes = (C.c_uint64 * 4)()
+        self._keep = None
+        self.n_reads = 0
+        self._check(self.lib.rvn_reads_upload_files(self.h, arr, len(enc), sizes))
+        n, nw, nbq, nnames = (int(x) for x in sizes)
+        w = np.zeros(nw, np.uint64) if words else None
+        woff = np.zeros(n + 1, np.uint64)
+        lens = np.zeros(n, np.uint32)
+        bq = np.zeros(nbq, np.uint8)
+        bq_off = np.zeros(n + 1, np.uint64)
+        names = np.zeros(nnames, np.uint8)
+        name_off = np.zeros(n + 1, np.uint64)
+        self._check(self.lib.rvn_reads_parsed(
+            self.h, None if w is None else w.ctypes.data_as(U64P), woff.ctypes.data_as(U64P),
+            lens.ctypes.data_as(U32P), bq.ctypes.data_as(C.POINTER(C.c_uint8)),
+            bq_off.ctypes.data_as(U64P), names.ctypes.data, name_off.ctypes.data_as(U64P)))
+        raw = names.tobytes()
+        rs = seqio.ReadSet(w, woff, lens, bq, bq_off,
+                           [raw[int(name_off[i]):int(name_off[i + 1])].decode(
+                               errors="surrogateescape") for i in range(n)])
+        self._keep = (w, woff, lens)
+        self.n_reads = n
+        return rs
 
     def minimize(self, first, last, minhash=False):
         self._check(self.lib.rvn_minimize(self.h, first, last, int(minhash)))
