@@ -113,7 +113,7 @@ void RestoreSet(const RiderRead& r) {
   c.h_len.pop_back();
   c.h_ids.pop_back();
   c.h_tile_off.pop_back();
-  c.s_valid = c.q_valid = c.qt_valid = false;
+  MarkStale(c, Stale::kThresholds);
 }
 
 // The host read tables of a new set (offsets, lengths, pile offsets, ids); the device
@@ -122,7 +122,7 @@ void SetReadTables(Ctx& c, const uint64_t* word_off, const uint32_t* lens, const
                    uint32_t n_reads) {
   if (n_reads && (!word_off || !lens)) throw InvalidArgument("null read set");
   if (n_reads == 0xFFFFFFFFu) throw LimitError("too many reads");
-  c.s_valid = c.q_valid = c.qt_valid = c.i_valid = c.r_valid = c.st_valid = false;
+  MarkStale(c, Stale::kStage1);
   c.st_piles_on_device = false;
   c.reads_unset = c.fx_valid = false;
   c.tiles_k = 0;
@@ -354,7 +354,7 @@ RiderRead::RiderRead(Ctx& ctx, const uint64_t* words, uint32_t len, uint32_t id)
   c.h_ids.push_back(id);
   c.h_tile_off.push_back(tile_tail[1]);
   c.n_reads = n + 1;
-  c.s_valid = c.q_valid = c.qt_valid = false;
+  MarkStale(c, Stale::kThresholds);
   // the rider's bases are the only resident ones while it rides
   c.bases.res_first = n;
   c.bases.res_last = n + 1;

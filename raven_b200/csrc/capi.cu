@@ -220,7 +220,7 @@ RVN_API int rvn_engine_configure(rvn_ctx* ctx, uint32_t k, uint32_t w,
     c.prm.chain = chain;
     c.prm.matches = matches;
     c.prm.gap = gap;
-    c.s_valid = c.q_valid = c.qt_valid = c.i_valid = c.r_valid = false;
+    MarkStale(c, Stale::kIndex);
     c.tiles_k = 0;  // the tile table depends on (k, w)
     c.occurrence = 0xFFFFFFFFu;
   });
@@ -520,29 +520,18 @@ RVN_API int rvn_sketch(rvn_ctx* ctx, uint32_t first, uint32_t last, int minhash,
   return Guard(ctx, [&](Ctx& c) {
     CheckRange(c, first, last);
     const uint32_t nr = last - first;
-    const uint64_t *dv, *dorg;
-    const std::vector<uint64_t>* hoff;
-    uint64_t total;
     EnsureSketch(c, first, last);
-    if (minhash) {
-      EnsureMicromizers(c, first, last);
-      dv = c.q_val.get();
-      dorg = c.q_org.get();
-      hoff = &c.h_q_off;
-      total = c.q_n;
-    } else {
-      dv = c.s_val.get();
-      dorg = c.s_org.get();
-      hoff = &c.h_s_off;
-      total = c.s_n;
-    }
+    if (minhash) EnsureMicromizers(c, first, last);
+    const RecordSet& set = minhash ? c.mm : c.sk;
+    const uint64_t total = set.n;
     uint64_t* hv = c.x_val.reserve(total + 1);
     uint64_t* ho = c.x_org.reserve(total + 1);
     uint64_t* hf = c.x_off.reserve(nr + 2ULL);
-    const bool v32 = minhash ? c.q_is32 : c.s_is32;  // k <= 15: u32 values
-    RVN_CUDA(cudaMemcpyAsync(hv, dv, total * (v32 ? 4 : 8), cudaMemcpyDeviceToHost, c.stream));
-    RVN_CUDA(cudaMemcpyAsync(ho, dorg, total * 8, cudaMemcpyDeviceToHost, c.stream));
-    for (uint32_t i = 0; i <= nr; ++i) hf[i] = (*hoff)[i];
+    const bool v32 = set.is32;  // k <= 15: u32 values
+    RVN_CUDA(cudaMemcpyAsync(hv, set.val.get(), total * (v32 ? 4 : 8), cudaMemcpyDeviceToHost,
+                             c.stream));
+    RVN_CUDA(cudaMemcpyAsync(ho, set.org.get(), total * 8, cudaMemcpyDeviceToHost, c.stream));
+    for (uint32_t i = 0; i <= nr; ++i) hf[i] = set.h_off[i];
     RVN_CUDA(cudaStreamSynchronize(c.stream));
     if (v32) {  // widen in place, back to front
       const uint32_t* h32 = reinterpret_cast<const uint32_t*>(hv);
@@ -921,7 +910,7 @@ RVN_API int rvn_dist_overlaps_split(rvn_ctx* ctx, uint32_t n_parts, uint32_t ran
 
 RVN_API int rvn_dist_stage1_begin(rvn_ctx* ctx, uint32_t n_parts, uint32_t rank) {
   return Guard(ctx, [&](Ctx& c) {
-    c.s_valid = c.q_valid = c.qt_valid = c.i_valid = c.r_valid = false;
+    MarkStale(c, Stale::kIndex);
     TimerReset(c);
     std::memset(&c.stats, 0, sizeof(c.stats));
     DistStage1Begin(c, n_parts, rank);

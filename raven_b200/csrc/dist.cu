@@ -422,20 +422,15 @@ void DistSketchSplit(Ctx& c, uint32_t first, uint32_t last, int which, uint32_t 
                      const uint64_t** d_val, const uint64_t** d_org, uint64_t* counts) {
   CheckParts(parts, 0);
   EnsureSketch(c, first, last);
-  ValView sv{c.s_val.get(), c.s_is32 ? 1 : 0};
-  const uint64_t* so = c.s_org.get();
-  uint64_t n = c.s_n;
-  if (which == 1) {
-    EnsureMicromizers(c, first, last);
-    sv = ValView{c.q_val.get(), c.q_is32 ? 1 : 0};
-    so = c.q_org.get();
-    n = c.q_n;
-  }
+  if (which == 1) EnsureMicromizers(c, first, last);
+  const RecordSet& src = which == 1 ? c.mm : c.sk;
+  const ValView sv = src.Values();
+  const uint64_t n = src.n;
   if ((parts == 1 && !sv.is32) || n == 0) {  // nothing to move
     for (uint32_t p = 0; p < parts; ++p) counts[p] = 0;
     counts[0] = n;
     *d_val = static_cast<const uint64_t*>(sv.p);
-    *d_org = so;
+    *d_org = src.org.get();
     return;
   }
   // (one part with u32 sketch values: the partition below is the widening copy
@@ -455,7 +450,7 @@ void DistSketchSplit(Ctx& c, uint32_t first, uint32_t last, int which, uint32_t 
   ExclusiveScanU32(c, hist, base, parts * n_tiles);
   GatherBoundaries<<<1, 32, 0, c.stream>>>(base, n_tiles, parts, bnd);
   PartitionScatter<<<static_cast<unsigned>(n_tiles), kThreads, 0, c.stream>>>(
-      sv, so, n, parts, n_tiles, base, out_val, out_org);
+      sv, src.org.get(), n, parts, n_tiles, base, out_val, out_org);
   RVN_LAUNCH_CHECK();
   c.launches += 3;
   TimerEnd(c);
@@ -474,8 +469,7 @@ void DistHitsSplit(Ctx& c, const uint64_t* d_qval, const uint64_t* d_qorg, uint6
   if (!c.i_valid) throw StateError("no index");
   CheckParts(parts, 0);
   if (n_query > c.n_reads) throw InvalidArgument("query range out of bounds");
-  IndexView ix{ValView{c.i_val.get(), c.i_is32 ? 1 : 0}, c.i_org.get(), c.i_bucket.get(), c.i_n,
-               c.i_shift, c.occurrence, c.i_limit};
+  const IndexView ix = IndexOf(c);
   const uint32_t per_part = CeilDiv(n_query, parts);
   const uint64_t slots = static_cast<uint64_t>(per_part) * parts;
   uint32_t* cnt = c.m_cnt.reserve(n_q + 1);

@@ -2,8 +2,8 @@
 //
 // Data layout in HBM (all SoA, 8-byte fields, see DESIGN.md):
 //   reads      words[]           2-bit packed, biosoup layout, 0.25 B/base
-//   sketch     s_val[], s_org[]  minimizer records in (read, position) order
-//   queries    q_val[], q_org[]  micromizers (len/k smallest per read)
+//   sketch     sk.val, sk.org    minimizer records in (read, position) order
+//   queries    mm.val, mm.org    micromizers (len/k smallest per read)
 //   index      i_val[], i_org[]  sketch stably sorted by value + bucket table
 //   hits       h_grp[], h_pos[]  ram "Match" records grouped by query read
 //   overlaps   rvn_overlap[]     32 B records grouped by query read
@@ -123,6 +123,64 @@ struct Bases {
   CopyPieces upload;
 };
 
+// The records of reads [first, last) in (read, position) order: the sketch or the
+// micromizers. Read first + i has records [h_off[i], h_off[i + 1]) of val / org, n in all
+// (off: the same offsets on the device, bound at construction); the values are u32 when
+// is32 (2k <= 30), else u64.
+struct RecordSet {
+  RecordSet(DevBuf<uint64_t>& o, std::vector<uint64_t>& h) : off(o), h_off(h) {}
+  bool valid = false;
+  uint32_t first = 0, last = 0;
+  uint64_t n = 0;
+  bool is32 = false;
+  DevBuf<uint64_t> val, org;
+  DevBuf<uint64_t>& off;
+  std::vector<uint64_t>& h_off;
+  bool Exactly(uint32_t f, uint32_t l) const { return valid && first == f && last == l; }
+  bool Covers(uint32_t f, uint32_t l) const { return valid && first <= f && l <= last; }
+  ValView Values() const { return ValView{val.get(), is32 ? 1 : 0}; }
+  void Hold(uint32_t f, uint32_t l, uint64_t records, bool v32) {  // (once val / org are written)
+    first = f;
+    last = l;
+    n = records;
+    is32 = v32;
+    valid = true;
+  }
+};
+
+// Micromizer thresholds of reads [first, last): record (value, position) of read r is a
+// micromizer iff value < val[r - first] || (value == val[r - first] && position <
+// pos[r - first]). Read first + i has h_off[i + 1] - h_off[i] micromizers (off: the same
+// counts on the device, where Micromize selects by them).
+struct Thresholds {
+  bool valid = false;
+  uint32_t first = 0, last = 0;
+  DevBuf<uint64_t> val;
+  DevBuf<uint32_t> pos;
+  DevBuf<uint64_t> off;
+  std::vector<uint64_t> h_off;
+  bool Exactly(uint32_t f, uint32_t l) const { return valid && first == f && last == l; }
+  bool Covers(uint32_t f, uint32_t l) const { return valid && first <= f && l <= last; }
+  // an empty table of reads [f, f) with room for the values of `reads` reads
+  void Reset(uint32_t f, uint32_t reads) {
+    first = last = f;
+    val.reserve(reads + 1ULL);
+    pos.reserve(reads + 1ULL);
+    h_off.assign(1, 0);
+  }
+  // the table of the reads that follow (t.first == last) behind this one (no device counts)
+  void Append(const Thresholds& t, cudaStream_t stream) {
+    const uint32_t nr = t.last - t.first;
+    RVN_CUDA(cudaMemcpyAsync(val.get() + (t.first - first), t.val.get(), nr * sizeof(uint64_t),
+                             cudaMemcpyDeviceToDevice, stream));
+    RVN_CUDA(cudaMemcpyAsync(pos.get() + (t.first - first), t.pos.get(), nr * sizeof(uint32_t),
+                             cudaMemcpyDeviceToDevice, stream));
+    const uint64_t base = h_off.back();
+    for (uint32_t r = 1; r <= nr; ++r) h_off.push_back(base + t.h_off[r]);
+    last = t.last;
+  }
+};
+
 struct Ctx {
   // device bytes held by this context's buffers (first member: it outlives them)
   uint64_t held_bytes = 0;
@@ -164,29 +222,18 @@ struct Ctx {
   DevBuf<uint32_t> d_tile_read;  // read of every tile
   uint32_t tiles_k = 0;
 
-  // ---- current sketch (full minimizers of reads [s_first, s_last)) ----
-  bool s_valid = false;
-  uint32_t s_first = 0, s_last = 0;
-  uint64_t s_n = 0;
-  DevBuf<uint64_t> s_val, s_org, s_off;  // s_off: (s_last-s_first)+1
-  bool s_is32 = false;  // s_val holds u32 values (2k <= 30 bits)
-  std::vector<uint64_t> h_s_off;
+  // ---- current sketch: the full minimizers of reads [sk.first, sk.last) ----
+  DevBuf<uint64_t> sk_off;
+  std::vector<uint64_t> h_sk_off;
+  RecordSet sk{sk_off, h_sk_off};
   DevBuf<uint32_t> tile_cnt;
   DevBuf<uint64_t> tile_out, tile_status;
 
-  // ---- current micromizer set (of reads [q_first, q_last)) ----
-  bool q_valid = false;
-  uint32_t q_first = 0, q_last = 0;
-  uint64_t q_n = 0;
-  DevBuf<uint64_t> q_val, q_org, q_off;
-  bool q_is32 = false;  // q_val holds u32 values
-  std::vector<uint64_t> h_q_off;
-  // micromizer thresholds of reads [qt_first, qt_last): record (value, position) of read r
-  // is a micromizer iff value < qt_val[r] || (value == qt_val[r] && position < qt_pos[r])
-  bool qt_valid = false;
-  uint32_t qt_first = 0, qt_last = 0;
-  DevBuf<uint64_t> qt_val;
-  DevBuf<uint32_t> qt_pos;
+  // ---- current micromizer thresholds and micromizer set ----
+  Thresholds qt;
+  // One buffer pair: the micromizers' offsets are the counts of the thresholds. A Micromize
+  // of thresholds only rewrites them, and the set stays valid only for the same reads.
+  RecordSet mm{qt.off, qt.h_off};
   int t_b_low = 0;  // the bare keys of the upper tier are sorted above this many low bits
   uint64_t group_count_min = 0;  // fewer keys per group of equal upper bits: full sort instead
   bool i_from_sketch = false;  // the index holds the FULL sketches of reads [i_first, i_last)
@@ -215,12 +262,10 @@ struct Ctx {
   uint64_t tier_min_records = 1ULL << 18;  // smaller index batches are not worth a partition
   DevBuf<uint64_t> t_hist;  // chunked build: coarse value histogram (capacity of the tiers)
   // Chunked build (BuildIndexChunked): the micromizer thresholds and counts of the index
-  // batch [i_first, i_last), kept apart from c.qt_* / c.h_q_off, which the probe-path
-  // flushes of reads before the batch overwrite; valid while jt_gen == i_gen
+  // batch [i_first, i_last), kept apart from c.qt, which the probe-path flushes of reads
+  // before the batch overwrite; valid while jt_gen == i_gen
   uint64_t jt_gen = 0;
-  DevBuf<uint64_t> jt_val;
-  DevBuf<uint32_t> jt_pos;
-  std::vector<uint64_t> h_jt_off;
+  Thresholds jt;
   DevBuf<uint32_t> i_bucket;
   int i_bucket_bits = 0;
   DevBuf<uint64_t> i_gaps;  // long empty stretches of the bucket table (index.cu)
@@ -420,6 +465,15 @@ struct Ctx {
   uint64_t launches = 0;
 };
 
+// The cached sets a change makes stale (each level also clears those of the levels before it)
+enum class Stale { kRecords, kThresholds, kIndex, kStage1 };
+inline void MarkStale(Ctx& c, Stale s) {
+  c.sk.valid = c.mm.valid = false;  // kRecords: a new sketch, or the tile table changed
+  if (s >= Stale::kThresholds) c.qt.valid = false;  // a rider read joined or left the set
+  if (s >= Stale::kIndex) c.i_valid = c.r_valid = false;  // new parameters, a stage-1 pass
+  if (s >= Stale::kStage1) c.st_valid = false;  // a new read set
+}
+
 // ---- utilities (scan.cu) ----
 // out[i] = sum_{j<i} in[j] for i in [0, n]; out has n + 1 entries.
 void ExclusiveScanU32(Ctx& c, const uint32_t* in, uint64_t* out, uint64_t n);
@@ -482,11 +536,12 @@ void ParsedReads(Ctx& c, uint64_t* words, uint64_t* word_off, uint32_t* lens,
 
 // ---- sketch.cu ----
 void EnsureTiles(Ctx& c);
-// full minimizers of reads [first,last) into c.s_* (no-op if already there)
+// full minimizers of reads [first,last) into c.sk (no-op if already there)
 void EnsureSketch(Ctx& c, uint32_t first, uint32_t last);
-// micromizers of reads [first,last) into c.q_* (needs the sketch of a range
-// that contains [first,last))
+// micromizers of reads [first,last) into c.mm and their thresholds into c.qt (needs the
+// sketch of a range that contains [first,last))
 void EnsureMicromizers(Ctx& c, uint32_t first, uint32_t last);
+// only the thresholds and counts of reads [first, last) into c.qt
 void EnsureThresholds(Ctx& c, uint32_t first, uint32_t last);
 // The sketch records of reads [first, last) straight into the two tiers of an index build
 // (SketchFastKernel's tier-output mode; raven's stage-1 parameters k <= 15, w = 5 only,
@@ -519,7 +574,7 @@ uint64_t MaxMicromizerValue(Ctx& c, uint32_t first, uint32_t last);
 // `tmax` and the batch's micromizer values (returned; tmax itself with minhash), built
 // from chunks of reads of >= chunk bases: no sketch of the whole batch is ever held.
 // minhash: one sweep appends each chunk's micromizers to the sort's input. Otherwise
-// sweep 1 sketches each chunk and keeps its thresholds (c.jt_*); sweep 2 sketches it
+// sweep 1 sketches each chunk and keeps its thresholds (c.jt); sweep 2 sketches it
 // again and appends its records to the sort's input - tiered: split into tier A
 // (c.i_val_alt / c.i_org_alt) and bare keys (c.t_b0), at k <= 15, w = 5 straight from
 // the sketch kernel (SketchTiers).

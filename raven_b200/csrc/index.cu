@@ -579,40 +579,37 @@ void BareCount(Ctx& c, const uint32_t* keys, uint64_t n, int key_bits, uint32_t 
   ++c.launches;
 }
 
-}  // namespace
-
-// largest micromizer value of reads [first, last): the largest of their selection
-// thresholds (c.qt_val)
-uint64_t MaxMicromizerValue(Ctx& c, uint32_t first, uint32_t last) {
-  EnsureThresholds(c, first, last);
-  if (last <= first) return 0;
-  if (!c.s_is32) return ~0ULL;  // (tiers are only built over u32 values)
+// largest micromizer value of the reads of t: the largest of their selection thresholds
+uint64_t MaxThreshold(Ctx& c, const Thresholds& t) {
   uint64_t* w = c.m_counter.reserve(8);
   RVN_CUDA(cudaMemsetAsync(w, 0, sizeof(uint64_t), c.stream));
-  const uint64_t n = last - first;
+  const uint64_t n = t.last - t.first;
   MaxU64Kernel<<<std::min<unsigned>(CeilDiv(n, 256), c.sms * 8), 256, 0, c.stream>>>(
-      c.qt_val.get(), n, reinterpret_cast<unsigned long long*>(w));
+      t.val.get(), n, reinterpret_cast<unsigned long long*>(w));
   RVN_LAUNCH_CHECK();
   ++c.launches;
   return ReadU64(c, w);
+}
+
+}  // namespace
+
+// largest micromizer value of reads [first, last) (c.qt)
+uint64_t MaxMicromizerValue(Ctx& c, uint32_t first, uint32_t last) {
+  EnsureThresholds(c, first, last);
+  if (last <= first) return 0;
+  if (!c.sk.is32) return ~0ULL;  // (tiers are only built over u32 values)
+  return MaxThreshold(c, c.qt);
 }
 
 void BuildIndex(Ctx& c, uint32_t first, uint32_t last, bool minhash, uint64_t value_limit) {
   c.i_valid = false;
   c.occurrence = 0xFFFFFFFFu;
   EnsureSketch(c, first, last);
-  ValView src_val{c.s_val.get(), c.s_is32 ? 1 : 0};
-  const uint64_t* src_org = c.s_org.get();
-  uint64_t n = c.s_n;
-  if (minhash) {
-    EnsureMicromizers(c, first, last);
-    src_val = ValView{c.q_val.get(), c.q_is32 ? 1 : 0};
-    src_org = c.q_org.get();
-    n = c.q_n;
-  }
+  if (minhash) EnsureMicromizers(c, first, last);
+  const RecordSet& src = minhash ? c.mm : c.sk;
   c.i_first = first;
   c.i_last = last;
-  BuildIndexFrom(c, src_val, src_org, n, ReadBases(c, first, last),
+  BuildIndexFrom(c, src.Values(), src.org.get(), src.n, ReadBases(c, first, last),
                  minhash ? ~0ULL : value_limit, /*count_bare=*/true);
   c.i_sorted_ids = c.ids_ascending;
   c.i_from_sketch = !minhash;
@@ -927,14 +924,14 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
       stage_next(i, false);
       EnsureMicromizers(c, cuts[i], cuts[i + 1]);  // (sketches the chunk)
       TimerBegin(c, "sketch_tiers");
-      if (c.q_n) {
-        RVN_CUDA(cudaMemcpyAsync(reinterpret_cast<uint8_t*>(q_val) + n * vb, c.q_val.get(),
-                                 c.q_n * vb, cudaMemcpyDeviceToDevice, c.stream));
-        RVN_CUDA(cudaMemcpyAsync(q_org + n, c.q_org.get(), c.q_n * sizeof(uint64_t),
+      if (c.mm.n) {
+        RVN_CUDA(cudaMemcpyAsync(reinterpret_cast<uint8_t*>(q_val) + n * vb, c.mm.val.get(),
+                                 c.mm.n * vb, cudaMemcpyDeviceToDevice, c.stream));
+        RVN_CUDA(cudaMemcpyAsync(q_org + n, c.mm.org.get(), c.mm.n * sizeof(uint64_t),
                                  cudaMemcpyDeviceToDevice, c.stream));
       }
       TimerEnd(c);
-      n += c.q_n;
+      n += c.mm.n;
     }
     if (n >= 0xFFFFFFFFULL) throw LimitError("index batch holds 2^32 or more minimizers");
     c.i_first = first;
@@ -950,25 +947,18 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
   // that bounds the tiers ----
   uint64_t n = 0;
   std::vector<uint64_t> chunk_first{0};  // records before every chunk
-  c.jt_val.reserve(nr + 1ULL);
-  c.jt_pos.reserve(nr + 1ULL);
-  c.h_jt_off.assign(1, 0);
+  c.jt.Reset(first, nr);
   for (size_t i = 0; i + 1 < cuts.size(); ++i) {
     const uint32_t r0 = cuts[i], r1 = cuts[i + 1];
     stage_next(i, true);
-    EnsureSketch(c, r0, r1);  // (exactly the chunk: c.s_n and c.s_val are its records)
+    EnsureSketch(c, r0, r1);  // (exactly the chunk: c.sk holds its records)
     EnsureThresholds(c, r0, r1);
-    n += c.s_n;
+    n += c.sk.n;
     chunk_first.push_back(n);
-    RVN_CUDA(cudaMemcpyAsync(c.jt_val.get() + (r0 - first), c.qt_val.get(),
-                             (r1 - r0) * sizeof(uint64_t), cudaMemcpyDeviceToDevice, c.stream));
-    RVN_CUDA(cudaMemcpyAsync(c.jt_pos.get() + (r0 - first), c.qt_pos.get(),
-                             (r1 - r0) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, c.stream));
-    const uint64_t base = c.h_jt_off.back();
-    for (uint32_t r = 1; r <= r1 - r0; ++r) c.h_jt_off.push_back(base + c.h_q_off[r]);
-    if (tiers && k32 && c.s_n > 0) {
-      ValueHistKernel<<<std::min<unsigned>(CeilDiv(c.s_n, kThreads), c.sms * 4), kThreads, 0,
-                        c.stream>>>(reinterpret_cast<const uint32_t*>(c.s_val.get()), c.s_n,
+    c.jt.Append(c.qt, c.stream);
+    if (tiers && k32 && c.sk.n > 0) {
+      ValueHistKernel<<<std::min<unsigned>(CeilDiv(c.sk.n, kThreads), c.sms * 4), kThreads, 0,
+                        c.stream>>>(reinterpret_cast<const uint32_t*>(c.sk.val.get()), c.sk.n,
                                     hist_shift, vhist);
       RVN_LAUNCH_CHECK();
       ++c.launches;
@@ -976,19 +966,7 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
   }
   if (n >= 0xFFFFFFFFULL) throw LimitError("index batch holds 2^32 or more minimizers");
   // the tier bound: the largest micromizer value of every read sketched so far
-  if (tiers && nr > 0) {
-    if (!k32) {
-      tmax = ~0ULL;
-    } else {
-      uint64_t* w = c.m_counter.reserve(8);
-      RVN_CUDA(cudaMemsetAsync(w, 0, sizeof(uint64_t), c.stream));
-      MaxU64Kernel<<<std::min<unsigned>(CeilDiv(nr, 256), c.sms * 8), 256, 0, c.stream>>>(
-          c.jt_val.get(), nr, reinterpret_cast<unsigned long long*>(w));
-      RVN_LAUNCH_CHECK();
-      ++c.launches;
-      tmax = std::max(tmax, ReadU64(c, w));
-    }
-  }
+  if (tiers && nr > 0) tmax = k32 ? std::max(tmax, MaxThreshold(c, c.jt)) : ~0ULL;
   const uint64_t limit = tiers ? tmax : ~0ULL;
   const bool is32 = k32;
   const bool tiered = Tiered(c, is32, limit, n);
@@ -997,9 +975,9 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
   const bool fused = tiered && SketchTiersFused(c);
   const bool append = !tiered && SketchTiersFused(c);
   if (fused || append) {
-    c.s_valid = c.q_valid = false;
-    c.s_val.release();
-    c.s_org.release();
+    MarkStale(c, Stale::kRecords);
+    c.sk.val.release();
+    c.sk.org.release();
   }
 
   // ---- sweep 2: the chunks' records, appended in (read, position) order ----
@@ -1046,9 +1024,9 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
       continue;
     }
     EnsureSketch(c, r0, r1);  // (no-op for a batch of one chunk)
-    const uint64_t* sv = c.s_val.get();
-    const uint64_t* so = c.s_org.get();
-    const uint64_t m = c.s_n;
+    const uint64_t* sv = c.sk.val.get();
+    const uint64_t* so = c.sk.org.get();
+    const uint64_t m = c.sk.n;
     TimerBegin(c, "sketch_tiers");
     if (m == 0) {
     } else if (tiered) {
@@ -1095,9 +1073,9 @@ uint64_t BuildIndexChunked(Ctx& c, uint32_t first, uint32_t last, bool minhash, 
 }
 
 void ReleaseIndexBuild(Ctx& c) {
-  c.s_valid = false;
-  c.s_val.release();
-  c.s_org.release();
+  c.sk.valid = false;
+  c.sk.val.release();
+  c.sk.org.release();
   c.i_val_alt.release();
   c.i_org_alt.release();
   c.t_aval.release();

@@ -996,17 +996,13 @@ __global__ void ReorderOverlaps(const rvn_overlap* __restrict__ raw,
 // Reads before `first` are left out: their flushes took the probe path, and their
 // thresholds would cost a sketch of reads that are no longer sketched. The slot
 // offsets are kept with the slots, as a flush over reads outside the batch replaces
-// the micromizer counts (c.h_q_off). Needs the thresholds of reads [first, i_last): the
-// batch's own (c.jt_*) after a chunked build, else c.qt_*.
-void JoinSweep(Ctx& c, uint32_t first) {
-  const bool batch = c.jt_gen == c.i_gen;
-  const std::vector<uint64_t>& cnt_off = batch ? c.h_jt_off : c.h_q_off;
-  const uint64_t* thr_val = batch ? c.jt_val.get() : c.qt_val.get();
-  const uint32_t* thr_pos = batch ? c.jt_pos.get() : c.qt_pos.get();
+// the micromizer counts (c.qt.h_off). Needs the thresholds t of reads [first, i_last): the
+// batch's own (c.jt) after a chunked build, else c.qt.
+void JoinSweep(Ctx& c, uint32_t first, const Thresholds& t) {
   const uint32_t nr = c.i_last - first;
-  const uint64_t t0 = first - (batch ? c.i_first : c.qt_first), base = cnt_off[t0];
+  const uint64_t t0 = first - t.first, base = t.h_off[t0];
   c.h_j_off.resize(nr + 1ULL);
-  for (uint32_t i = 0; i <= nr; ++i) c.h_j_off[i] = cnt_off[t0 + i] - base;
+  for (uint32_t i = 0; i <= nr; ++i) c.h_j_off[i] = t.h_off[t0 + i] - base;
   const uint64_t n_q = c.h_j_off[nr];
   uint64_t* off = c.j_off.reserve(nr + 1ULL);
   RVN_CUDA(cudaMemcpyAsync(off, c.h_j_off.data(), (nr + 1ULL) * sizeof(uint64_t),
@@ -1016,8 +1012,9 @@ void JoinSweep(Ctx& c, uint32_t first) {
   RVN_CUDA(cudaMemsetAsync(cursor, 0, (nr + 1ULL) * sizeof(uint32_t), c.stream));
   RVN_CUDA(cudaMemsetAsync(packed, 0, (n_q + 1) * sizeof(uint64_t), c.stream));
   if (c.i_n > 0 && n_q > 0) {
-    JoinView jv{ValView{c.i_val.get(), c.i_is32 ? 1 : 0}, c.i_org.get(), c.i_n, c.occurrence,
-                thr_val + t0, thr_pos + t0, first, c.i_last};
+    const IndexView ix = IndexOf(c);
+    JoinView jv{ix.val, ix.org, ix.n, ix.occurrence, t.val.get() + t0, t.pos.get() + t0, first,
+                c.i_last};
     JoinSweepKernel<<<CeilDiv(c.i_n, kThreads), kThreads, 0, c.stream>>>(jv, off, cursor,
                                                                           packed);
     RVN_LAUNCH_CHECK();
@@ -1054,12 +1051,12 @@ HitCounts JoinHits(Ctx& c, uint32_t first, uint32_t last, uint64_t* read_hit_off
   const uint32_t nr = last - first;
   HitCounts h;
   const bool sweep = c.j_gen != c.i_gen || c.j_occurrence != c.occurrence || first < c.j_first;
-  if (sweep && c.jt_gen != c.i_gen &&
-      !(c.qt_valid && c.qt_first <= first && c.i_last <= c.qt_last)) {
+  const bool batch = c.jt_gen == c.i_gen;
+  if (sweep && !batch && !c.qt.Covers(first, c.i_last)) {
     EnsureThresholds(c, first, c.i_last);  // (its sketch and micromize time are not probe's)
   }
   TimerBegin(c, "probe");
-  if (sweep) JoinSweep(c, first);
+  if (sweep) JoinSweep(c, first, batch ? c.jt : c.qt);
   const uint64_t b0 = first - c.j_first;
   const uint64_t q_begin = c.h_j_off[b0];
   h.n_q = c.h_j_off[b0 + nr] - q_begin;
@@ -1133,35 +1130,18 @@ HitCounts ProbeHits(Ctx& c, uint32_t first, uint32_t last, bool avoid_equal,
   const uint32_t nr = last - first;
   HitCounts h;
   // ---- query records ----
-  const uint64_t *qo, *d_read_off;
-  ValView qv;  // query values: u32 for full sketches of k <= 15, else u64
-  const std::vector<uint64_t>* h_read_off;
-  uint64_t off_base_read;  // index of `first` inside the offsets arrays
-  if (minhash) {
-    if (!(c.q_valid && c.q_first <= first && last <= c.q_last)) {
-      EnsureMicromizers(c, first, last);
-    }
-    qv = ValView{c.q_val.get(), c.q_is32 ? 1 : 0};
-    qo = c.q_org.get();
-    d_read_off = c.q_off.get();
-    h_read_off = &c.h_q_off;
-    off_base_read = first - c.q_first;
-  } else {
-    if (!(c.s_valid && c.s_first <= first && last <= c.s_last)) {
-      EnsureSketch(c, first, last);
-    }
-    qv = ValView{c.s_val.get(), c.s_is32 ? 1 : 0};
-    qo = c.s_org.get();
-    d_read_off = c.s_off.get();
-    h_read_off = &c.h_s_off;
-    off_base_read = first - c.s_first;
-  }
-  const uint64_t q_begin = (*h_read_off)[off_base_read];
-  const uint64_t n_q = (*h_read_off)[off_base_read + nr] - q_begin;
+  const RecordSet& q = minhash ? c.mm : c.sk;
+  if (minhash && !q.Covers(first, last)) EnsureMicromizers(c, first, last);
+  if (!minhash && !q.Covers(first, last)) EnsureSketch(c, first, last);
+  const ValView qv = q.Values();  // query values: u32 for full sketches of k <= 15, else u64
+  const uint64_t* qo = q.org.get();
+  const uint64_t off_base_read = first - q.first;  // index of `first` inside the offsets arrays
+  const uint64_t* d_read_off = q.off.get();
+  const uint64_t q_begin = q.h_off[off_base_read];
+  const uint64_t n_q = q.h_off[off_base_read + nr] - q_begin;
   h.n_q = n_q;
 
-  IndexView ix{ValView{c.i_val.get(), c.i_is32 ? 1 : 0}, c.i_org.get(), c.i_bucket.get(), c.i_n,
-               c.i_shift, c.occurrence, c.i_limit};
+  const IndexView ix = IndexOf(c);
 
   // ---- probe + expand ----
   TimerBegin(c, "probe");

@@ -10,6 +10,7 @@
 #include <cstdint>
 
 #include "common.cuh"
+#include "engine.cuh"
 
 namespace rvn {
 namespace {
@@ -23,6 +24,12 @@ struct IndexView {
   uint32_t occurrence;
   uint64_t limit;  // values beyond it are not indexed (tiered build)
 };
+
+// the context's index as the probe kernels read it, filtered at its occurrence threshold
+inline IndexView IndexOf(const Ctx& c) {
+  return IndexView{ValView{c.i_val.get(), c.i_is32 ? 1 : 0}, c.i_org.get(), c.i_bucket.get(),
+                   c.i_n, c.i_shift, c.occurrence, c.i_limit};
+}
 
 // first record with value v and the run length capped at occurrence+1
 __device__ __forceinline__ void Lookup(const IndexView& ix, uint64_t v,

@@ -981,21 +981,20 @@ void EnsureTiles(Ctx& c) {
                            cudaMemcpyHostToDevice, c.stream));
   RVN_CUDA(cudaStreamSynchronize(c.stream));
   c.tiles_k = c.prm.k;
-  c.s_valid = c.q_valid = false;
+  MarkStale(c, Stale::kRecords);
 }
 
 void EnsureSketch(Ctx& c, uint32_t first, uint32_t last) {
-  if (c.s_valid && c.s_first == first && c.s_last == last) return;
+  if (c.sk.Exactly(first, last)) return;
   CheckResident(c, first, last);
   EnsureTiles(c);
-  c.s_valid = false;
-  c.q_valid = false;
+  MarkStale(c, Stale::kRecords);
   const uint32_t nr = last - first;
   const uint64_t n_tiles = c.h_tile_off[last] - c.h_tile_off[first];
   if (n_tiles >= (1ULL << 31)) throw LimitError("too many sketch tiles");
 
-  uint64_t* read_off = c.s_off.reserve(nr + 1ULL);
-  c.h_s_off.assign(nr + 1ULL, 0);
+  uint64_t* read_off = c.sk.off.reserve(nr + 1ULL);
+  c.sk.h_off.assign(nr + 1ULL, 0);
   uint64_t total = 0;
   if (n_tiles > 0) {
     TimerBegin(c, "sketch");
@@ -1012,7 +1011,7 @@ void EnsureSketch(Ctx& c, uint32_t first, uint32_t last) {
                        static_cast<double>(positions) *
                        std::min(1.0, 2.2 / (c.prm.w + 1.0))) + 4096;
     // (u32 values: two per element of the u64-typed buffer)
-    cap = std::max<uint64_t>(cap, std::min<uint64_t>(c.s_val.cap * (k32 ? 2 : 1), c.s_org.cap));
+    cap = std::max<uint64_t>(cap, std::min<uint64_t>(c.sk.val.cap * (k32 ? 2 : 1), c.sk.org.cap));
     uint64_t* tout = c.tile_out.reserve(n_tiles + 1);
     uint64_t* status = c.tile_status.reserve(n_tiles + 2);
     unsigned int* ticket = reinterpret_cast<unsigned int*>(status + n_tiles);
@@ -1020,8 +1019,8 @@ void EnsureSketch(Ctx& c, uint32_t first, uint32_t last) {
     // the pieces that have arrived, the others wait for all of them)
     const BaseView v = SketchBases(c, first, last);
     for (int attempt = 0; attempt < 2; ++attempt) {
-      uint64_t* val = c.s_val.reserve(k32 ? cap / 2 + 1 : cap);
-      uint64_t* org = c.s_org.reserve(cap);
+      uint64_t* val = c.sk.val.reserve(k32 ? cap / 2 + 1 : cap);
+      uint64_t* org = c.sk.org.reserve(cap);
       RVN_CUDA(cudaMemsetAsync(status, 0, (n_tiles + 2) * sizeof(uint64_t), c.stream));
       if (k32 && c.prm.w == 5) {  // raven's default window: the fast kernel
         // (status words of this kernel: one per group of kFastGroup tiles)
@@ -1060,7 +1059,7 @@ void EnsureSketch(Ctx& c, uint32_t first, uint32_t last) {
     RVN_LAUNCH_CHECK();
     ++c.launches;
     TimerEnd(c);
-    RVN_CUDA(cudaMemcpyAsync(c.h_s_off.data(), read_off,
+    RVN_CUDA(cudaMemcpyAsync(c.sk.h_off.data(), read_off,
                              (nr + 1ULL) * sizeof(uint64_t),
                              cudaMemcpyDeviceToHost, c.stream));
     RVN_CUDA(cudaStreamSynchronize(c.stream));
@@ -1069,11 +1068,7 @@ void EnsureSketch(Ctx& c, uint32_t first, uint32_t last) {
     RVN_CUDA(cudaMemsetAsync(read_off, 0, (nr + 1ULL) * sizeof(uint64_t),
                              c.stream));
   }
-  c.s_first = first;
-  c.s_last = last;
-  c.s_n = total;
-  c.s_is32 = 2 * c.prm.k <= 30;
-  c.s_valid = true;
+  c.sk.Hold(first, last, total, 2 * c.prm.k <= 30);
 }
 
 bool SketchTiersFused(const Ctx& c) { return 2 * c.prm.k <= 30 && c.prm.w == 5; }
@@ -1141,98 +1136,90 @@ uint64_t SketchAppendTotal(Ctx& c) { return ReadU64(c, c.tile_out.get()); }
 
 namespace {
 
-// write == true: micromizers (c.q_*) and thresholds (c.qt_*); false: thresholds only
+// write == true: micromizers (c.mm) and thresholds (c.qt); false: thresholds only
 void Micromize(Ctx& c, uint32_t first, uint32_t last, bool write) {
-  if (!c.s_valid || first < c.s_first || last > c.s_last) {
-    EnsureSketch(c, first, last);
-  }
-  if (write) c.q_valid = false;
-  c.qt_valid = false;
+  if (!c.sk.Covers(first, last)) EnsureSketch(c, first, last);
+  const RecordSet& sk = c.sk;
+  Thresholds& qt = c.qt;
+  if (write) c.mm.valid = false;
+  qt.valid = false;
   const uint32_t nr = last - first;
-  c.h_q_off.assign(nr + 1ULL, 0);
+  qt.h_off.assign(nr + 1ULL, 0);
   for (uint32_t i = 0; i < nr; ++i) {
     const uint32_t r = first + i;
-    const uint64_t cnt = c.h_s_off[r - c.s_first + 1] - c.h_s_off[r - c.s_first];
+    const uint64_t cnt = sk.h_off[r - sk.first + 1] - sk.h_off[r - sk.first];
     const uint64_t m = c.h_len[r] / c.prm.k;
-    c.h_q_off[i + 1] = c.h_q_off[i] + (m < cnt ? m : cnt);
+    qt.h_off[i + 1] = qt.h_off[i] + (m < cnt ? m : cnt);
   }
-  const uint64_t total = c.h_q_off[nr];
+  const uint64_t total = qt.h_off[nr];
   // shared memory for the longest sketch that is selected (len/k < its length), up to
   // kMicroStageBytes; longer ones are selected from global memory
-  const size_t val_bytes = c.s_is32 ? 4 : 8;
+  const size_t val_bytes = sk.is32 ? 4 : 8;
   uint64_t longest = 0;
   for (uint32_t i = 0; i < nr; ++i) {
     const uint32_t r = first + i;
-    const uint64_t cnt = c.h_s_off[r - c.s_first + 1] - c.h_s_off[r - c.s_first];
-    if (c.h_q_off[i + 1] - c.h_q_off[i] < cnt) longest = std::max(longest, cnt);
+    const uint64_t cnt = sk.h_off[r - sk.first + 1] - sk.h_off[r - sk.first];
+    if (qt.h_off[i + 1] - qt.h_off[i] < cnt) longest = std::max(longest, cnt);
   }
   const uint32_t stage_cap =
       static_cast<uint32_t>(std::min<uint64_t>(longest, kMicroStageBytes / val_bytes));
   const size_t smem = stage_cap * val_bytes;
-  uint64_t* qoff = c.q_off.reserve(nr + 1ULL);
-  RVN_CUDA(cudaMemcpyAsync(qoff, c.h_q_off.data(),
+  uint64_t* qoff = qt.off.reserve(nr + 1ULL);
+  RVN_CUDA(cudaMemcpyAsync(qoff, qt.h_off.data(),
                            (nr + 1ULL) * sizeof(uint64_t),
                            cudaMemcpyHostToDevice, c.stream));
-  uint64_t* qv = write ? c.q_val.reserve(total) : c.q_val.get();
-  uint64_t* qo = write ? c.q_org.reserve(total) : c.q_org.get();
-  uint64_t* tv = c.qt_val.reserve(nr + 1ULL);
-  uint32_t* tp = c.qt_pos.reserve(nr + 1ULL);
+  uint64_t* qv = write ? c.mm.val.reserve(total) : c.mm.val.get();
+  uint64_t* qo = write ? c.mm.org.reserve(total) : c.mm.org.get();
+  uint64_t* tv = qt.val.reserve(nr + 1ULL);
+  uint32_t* tp = qt.pos.reserve(nr + 1ULL);
   if (nr > 0) {
     TimerBegin(c, "micromize");
     RVN_CUDA(cudaMemsetAsync(tv, 0, (nr + 1ULL) * sizeof(uint64_t), c.stream));
     RVN_CUDA(cudaMemsetAsync(tp, 0, (nr + 1ULL) * sizeof(uint32_t), c.stream));
-    if (c.s_is32) {  // micromizer values stay u32 like the sketch's
-      auto* sv = reinterpret_cast<const uint32_t*>(c.s_val.get());
+    if (sk.is32) {  // micromizer values stay u32 like the sketch's
+      auto* sv = reinterpret_cast<const uint32_t*>(sk.val.get());
       auto* q32 = reinterpret_cast<uint32_t*>(qv);
       if (write) {
         MicromizeKernel<uint32_t, true><<<nr, kMicroThreads, smem, c.stream>>>(
-            sv, c.s_org.get(), c.s_off.get(), c.s_first, qoff, first, c.prm.k, stage_cap, q32, qo,
+            sv, sk.org.get(), sk.off.get(), sk.first, qoff, first, c.prm.k, stage_cap, q32, qo,
             tv, tp);
       } else {
         MicromizeKernel<uint32_t, false><<<nr, kMicroThreads, smem, c.stream>>>(
-            sv, c.s_org.get(), c.s_off.get(), c.s_first, qoff, first, c.prm.k, stage_cap, q32, qo,
+            sv, sk.org.get(), sk.off.get(), sk.first, qoff, first, c.prm.k, stage_cap, q32, qo,
             tv, tp);
       }
     } else if (write) {
       MicromizeKernel<uint64_t, true><<<nr, kMicroThreads, smem, c.stream>>>(
-          c.s_val.get(), c.s_org.get(), c.s_off.get(), c.s_first, qoff, first, c.prm.k, stage_cap,
+          sk.val.get(), sk.org.get(), sk.off.get(), sk.first, qoff, first, c.prm.k, stage_cap,
           qv, qo, tv, tp);
     } else {
       MicromizeKernel<uint64_t, false><<<nr, kMicroThreads, smem, c.stream>>>(
-          c.s_val.get(), c.s_org.get(), c.s_off.get(), c.s_first, qoff, first, c.prm.k, stage_cap,
+          sk.val.get(), sk.org.get(), sk.off.get(), sk.first, qoff, first, c.prm.k, stage_cap,
           qv, qo, tv, tp);
     }
     RVN_LAUNCH_CHECK();
     ++c.launches;
     TimerEnd(c);
   }
-  RVN_CUDA(cudaStreamSynchronize(c.stream));  // h_q_off staging is reusable
+  RVN_CUDA(cudaStreamSynchronize(c.stream));  // qt.h_off staging is reusable
   if (write) {
-    c.q_first = first;
-    c.q_last = last;
-    c.q_n = total;
-    c.q_is32 = c.s_is32;
-    c.q_valid = true;
-  } else if (c.q_valid) {
-    // (q_off / h_q_off now describe [first, last): an older micromizer set is gone)
-    c.q_valid = c.q_first == first && c.q_last == last;
+    c.mm.Hold(first, last, total, sk.is32);
+  } else {  // (the shared counts now describe [first, last): an older micromizer set is gone)
+    c.mm.valid = c.mm.Exactly(first, last);
   }
-  c.qt_first = first;
-  c.qt_last = last;
-  c.qt_valid = true;
+  qt.first = first;
+  qt.last = last;
+  qt.valid = true;
 }
 
 }  // namespace
 
 void EnsureMicromizers(Ctx& c, uint32_t first, uint32_t last) {
-  if (c.q_valid && c.q_first == first && c.q_last == last) return;
-  Micromize(c, first, last, true);
+  if (!c.mm.Exactly(first, last)) Micromize(c, first, last, true);
 }
 
-// only the per-read selection rule (c.qt_*) and the counts (c.h_q_off)
 void EnsureThresholds(Ctx& c, uint32_t first, uint32_t last) {
-  if (c.qt_valid && c.qt_first == first && c.qt_last == last) return;
-  Micromize(c, first, last, false);
+  if (!c.qt.Exactly(first, last)) Micromize(c, first, last, false);
 }
 
 }  // namespace rvn

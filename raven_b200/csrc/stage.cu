@@ -50,7 +50,7 @@ constexpr double kBatchBytesPerBase = 21.0;
 // - per base of the batch: the index the flushes probe (i_val, i_org, i_bucket, j_packed:
 //   1.8 B) and the build's sort buffers and bare keys, freed before the flushes but held
 //   next to the flush buffers of an earlier batch or pass (i_*_alt, t_b0, t_b1: 3.3 B);
-// - per base of one chunk: its sketch in sweep 1 (s_val, s_org: 4.7 B);
+// - per base of one chunk: its sketch in sweep 1 (sk.val, sk.org: 4.7 B);
 // - per query base of the largest flush: the flush's hits, chain scratch and overlaps,
 //   and on the probe path its queries' sketch and sorted micromizers. 27 B is the
 //   remainder of the 59.9 GB peak of a 2^32-base batch with 2^30-base query flushes
@@ -665,7 +665,7 @@ void Stage1(Ctx& c, double freq, uint64_t kmax, bool minhash, uint64_t ib,
   c.own_rem = 0;
   // a stage-1 pass owns its intermediates: nothing is carried over from an
   // earlier call (sketches, micromizers and the index are rebuilt)
-  c.s_valid = c.q_valid = c.qt_valid = c.i_valid = c.r_valid = false;
+  MarkStale(c, Stale::kIndex);
   TimerReset(c);
   std::memset(&c.stats, 0, sizeof(c.stats));
   const uint64_t launches0 = c.launches;
