@@ -135,7 +135,11 @@ int rvn_reads_upload_ids(rvn_ctx* ctx, const uint64_t* words,
  * parsed and packed on the device; the result is the context's read set (ids 0..n-1), as after
  * rvn_reads_upload. sizes (may be NULL): reads, words, block qualities, name bytes.
  * Plain and gzip files (multi-member included) are read with zlib's gzread on a thread of the
- * library's own, in chunks of option "fastx_chunk_bytes" (results do not depend on it).
+ * library's own, in chunks of option "fastx_chunk_bytes" (results do not depend on it). A file
+ * whose first member is a whole BGZF member (bgzip, samtools; any suffix) is read raw instead
+ * and its members are inflated on the device, to the same text: at the first gzip member that
+ * is not a whole BGZF member the rest of the file goes to zlib, and bytes after the last member
+ * that do not begin a gzip header are ignored, as zlib ignores them.
  * Option "host_bases" applies to the parsed set. Errors: RVN_ERR_INVALID with the message
  * the reference's loop prints for the first failing record in file order (an unsupported
  * suffix, a file that cannot be opened, "invalid file format" wherever the drop-in FASTA or
@@ -143,7 +147,9 @@ int rvn_reads_upload_ids(rvn_ctx* ctx, const uint64_t* words,
  * or words that do not fit the device while the set is parsed (naming the bytes). After a
  * failed call the context holds no read set (the calls on reads are RVN_ERR_STATE until the
  * next upload). Phases in rvn_get_timings: "fastx_read" (host read or inflate that nothing
- * hid), "fastx_copy" and "fastx_parse" (per chunk). */
+ * hid), "fastx_copy" (text, or a BGZF file's compressed bytes), "fastx_inflate" (BGZF files
+ * only) and "fastx_parse" (per chunk). A BGZF member that does not inflate to its CRC and
+ * ISIZE fails the call with the drop-in's "unable to read file". */
 int rvn_reads_upload_files(rvn_ctx* ctx, const char* const* paths, uint32_t n_paths,
                            uint64_t sizes[4]);
 

@@ -1,21 +1,24 @@
 """Reading C2 from FASTQ: the drop-in parser, seqio.parse and Engine.upload_files.
 
-    python profiles/fastx_load.py [--rounds 2] [--reads 200000] [--formats plain,gz]
+    python profiles/fastx_load.py [--rounds 2] [--reads 200000] [--formats plain,gz,bgzf]
                                   [--skip-seqio] [--out DIR]
 
 C2 is bench.py's seeded read set (200 k reads of 10 kb mean, 2 Gbp). It is written as plain
-FASTQ and as `gzip -1` FASTQ in a temporary directory, with seeded qualities. For each file,
-rounds that alternate the routes:
+FASTQ, as `gzip -1` FASTQ and as BGZF FASTQ (level 1, members of 65,280 text bytes as bgzip
+cuts them, written by tests/test_gpu_bgzf.py's writer) in a temporary directory, with seeded
+qualities. For each file, rounds that alternate the routes:
   dropin        main.cc's loop over the drop-in bioparser + biosoup::NucleicAcid
                 (profiles/fastx_load.cc, compiled into the temporary directory)
   upload_files  rvn_reads_upload_files on a fresh context, with its phase split:
-                fastx_read (read or inflate that nothing hid), fastx_copy, fastx_parse
+                fastx_read (read or inflate that nothing hid), fastx_copy, fastx_inflate
+                (BGZF only), fastx_parse
   seqio         seqio.parse, once per file (it takes tens of seconds)
 Wall times are host clocks around calls that end when the set is built. The kernels' rate is
 their algorithmic bytes (the line index and the pack read the text three times, the words and
 block qualities are written once) over fastx_parse, against the H100's 3.35 TB/s; the copy
-rate is the text bytes over fastx_copy. Last, the stage-1 result after upload_files must have
-the sha256 of the one after upload of the same set.
+rate is the bytes copied (the text, or the BGZF file's compressed bytes) over fastx_copy; the
+inflate rate is the text bytes over fastx_inflate. Last, the stage-1 result after upload_files
+of the plain and the BGZF file must have the sha256 of the one after upload of the same set.
 
 Needs an H100; prints the card's name and power limit with the numbers. The files are read
 right after they were written, so they are likely in the page cache.
@@ -37,6 +40,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "profiles"))
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 from index_chunks import FREQ, GENOME, K, KMAX, MEAN_LEN, READS, SEED, W, card  # noqa: E402
 
@@ -63,6 +67,21 @@ def write_fastq(rs, path, seed):
                 f.write(b"\n")
 
 
+def write_bgzf(src, path):
+    """src as BGZF at level 1, members of 65,280 text bytes, compressed on all cores"""
+    from concurrent.futures import ThreadPoolExecutor
+    from test_gpu_bgzf import BGZIP_CUT, EOF_MARKER, member
+    with open(src, "rb") as f, open(path, "wb") as out, ThreadPoolExecutor() as pool:
+        while True:
+            block = f.read(BGZIP_CUT * 1024)
+            if not block:
+                break
+            parts = [block[i:i + BGZIP_CUT] for i in range(0, len(block), BGZIP_CUT)]
+            for m in pool.map(member, parts):
+                out.write(m)
+        out.write(EOF_MARKER)
+
+
 def digest(res):
     h = hashlib.sha256()
     for k in ("overlaps", "ovl_off", "pile", "pile_off"):
@@ -74,7 +93,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--reads", type=int, default=READS)
-    ap.add_argument("--formats", default="plain,gz")
+    ap.add_argument("--formats", default="plain,gz,bgzf")
     ap.add_argument("--skip-seqio", action="store_true")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
@@ -92,6 +111,7 @@ def main():
     try:
         plain = os.path.join(tmp, "c2.fastq")
         gz = plain + ".gz"
+        bgz = os.path.join(tmp, "c2.bgzf.fastq.gz")
         write_fastq(rs, plain, SEED)
         print("wrote", plain, os.path.getsize(plain), "bytes", flush=True)
         if "gz" in formats and shutil.which("gzip"):
@@ -101,14 +121,17 @@ def main():
             import gzip
             with open(plain, "rb") as src, gzip.open(gz, "wb", compresslevel=1) as dst:
                 shutil.copyfileobj(src, dst, 1 << 24)
+        if "bgzf" in formats:
+            write_bgzf(plain, bgz)
         text = os.path.getsize(plain)
-        out.update(text_bytes=text, gz_bytes=os.path.getsize(gz) if "gz" in formats else None)
+        out.update(text_bytes=text, gz_bytes=os.path.getsize(gz) if "gz" in formats else None,
+                   bgzf_bytes=os.path.getsize(bgz) if "bgzf" in formats else None)
         exe = os.path.join(tmp, "fastx_load")
         subprocess.run(["/usr/bin/g++", "-O2", "-std=c++17", "-I" + os.path.join(ROOT, "include"),
                         "-o", exe, os.path.join(ROOT, "profiles", "fastx_load.cc"), "-lz"],
                        check=True)
         kernel_bytes = 3 * text + rs.words.size * 8 + (rs.bases + 63) // 64
-        for name, path in (("plain", plain), ("gz", gz)):
+        for name, path in (("plain", plain), ("gz", gz), ("bgzf", bgz)):
             if name not in formats:
                 continue
             rec = dict(dropin_s=[], upload_files_s=[], phases=[])
@@ -126,10 +149,14 @@ def main():
                 finally:
                     eng.close()
                 assert parsed.n == rs.n and np.array_equal(parsed.lens, rs.lens)
-                ph = {k: tm.get(k, 0.0) for k in ("fastx_read", "fastx_copy", "fastx_parse")}
+                ph = {k: tm.get(k, 0.0)
+                      for k in ("fastx_read", "fastx_copy", "fastx_inflate", "fastx_parse")}
                 ph["kernel_TBps"] = kernel_bytes / (ph["fastx_parse"] * 1e-3) / 1e12
                 ph["kernel_share_of_hbm"] = kernel_bytes / (ph["fastx_parse"] * 1e-3) / HBM
-                ph["copy_GBps"] = text / (ph["fastx_copy"] * 1e-3) / 1e9
+                copied = os.path.getsize(path) if name == "bgzf" else text
+                ph["copy_GBps"] = copied / (ph["fastx_copy"] * 1e-3) / 1e9
+                if ph["fastx_inflate"]:
+                    ph["inflate_GBps"] = text / (ph["fastx_inflate"] * 1e-3) / 1e9
                 rec["phases"].append(ph)
                 print(name, "dropin %.2f s" % rec["dropin_s"][-1],
                       "upload_files %.2f s" % rec["upload_files_s"][-1],
@@ -143,20 +170,21 @@ def main():
             out["routes"][name] = rec
         # the stage-1 result after upload_files is the one after upload of the same set
         digests = []
-        for route in ("upload", "upload_files"):
+        sources = [None, plain] + ([bgz] if "bgzf" in formats else [])
+        for src in sources:
             eng = engine.Engine(device=0)
             try:
                 eng.configure(K, W)
-                if route == "upload":
+                if src is None:
                     eng.upload(rs)
                 else:
-                    eng.upload_files([plain])
+                    eng.upload_files([src])
                 digests.append(digest(eng.find_overlaps_and_create_piles(FREQ, KMAX, False)))
             finally:
                 eng.close()
         out["stage1_sha256"] = digests
-        print("stage-1 sha256 upload / upload_files:", *digests, flush=True)
-        assert digests[0] == digests[1]
+        print("stage-1 sha256 upload / upload_files (plain, bgzf):", *digests, flush=True)
+        assert len(set(digests)) == 1
     finally:
         shutil.rmtree(tmp, ignore_errors=True)
     if args.out:

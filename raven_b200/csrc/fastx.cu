@@ -18,13 +18,25 @@
 //             qualities likewise, the name
 // Errors carry the message the reference's input loop prints (RavenExe/src/main.cc:258-299)
 // for the first failing record in file order.
+//
+// A file whose first member is a whole BGZF member (the blocked gzip of the SAM specification,
+// as bgzip and samtools write it) is read raw instead: the reader walks the member headers,
+// whose BC subfields give each member's compressed size, and FxInflateKernel inflates the
+// members side by side, a warp each, straight into the chunk text (inflate.cuh). At a member
+// boundary, bytes that do not begin with 1f 8b end the file, as zlib ignores them; a gzip
+// member that is not a whole BGZF member (another header, a truncated member, an ISIZE above
+// 64 KiB) hands the rest of the file to zlib, opened at that member. Every other file is read
+// with gzread as above.
+#include <fcntl.h>
 #include <sys/stat.h>
+#include <unistd.h>
 #include <zlib.h>
 
 #include <algorithm>
 #include <chrono>
 #include <condition_variable>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <thread>
 
@@ -32,6 +44,7 @@
 #include "../../include/biosoup/nucleic_acid.hpp"
 #pragma nv_diag_default 68
 #include "engine.cuh"
+#include "inflate.cuh"
 
 namespace rvn {
 
@@ -438,6 +451,51 @@ FxPackKernel(const uint8_t* __restrict__ text, const FxRec* __restrict__ rec, ui
   }
 }
 
+constexpr int kFxInfWarps = 8;  // members per CTA of FxInflateKernel
+
+// one BGZF member of a piece: its deflate data in the piece's compressed bytes, its text in
+// the piece's text, and its trailer
+struct FxMember {
+  uint64_t in_off, out_off;
+  uint32_t in_len, isize, crc, pad;
+};
+
+// A warp per member. Lane 0 inflates it (inflate.cuh, tables in shared memory) into the text;
+// then each lane takes the CRC-32 of a 32nd of the output, and the registers are shifted past
+// the bytes after their slices and XOR-ed. A member that fails, or whose CRC or ISIZE differ
+// from its trailer, records its index in *bad. (The bound of 4 CTAs per SM keeps ptxas from
+// spilling; shared memory allows 7.)
+__global__ void __launch_bounds__(kFxInfWarps * 32, 4)
+FxInflateKernel(const uint8_t* __restrict__ comp, const FxMember* __restrict__ mem,
+                uint32_t n_mem, uint8_t* text, unsigned* bad) {
+  __shared__ InfTables tabs[kFxInfWarps];
+  __shared__ uint32_t crc_tab[256];
+  for (int i = threadIdx.x; i < 256; i += blockDim.x) crc_tab[i] = InfCrcTableEntry(i);
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (uint32_t m = blockIdx.x * kFxInfWarps + warp; m < n_mem; m += gridDim.x * kFxInfWarps) {
+    const FxMember x = mem[m];
+    uint8_t* out = text + x.out_off;
+    int got = 0;  // (an output length of at most 2^16, or -1)
+    if (lane == 0) {
+      got = static_cast<int>(Inflate(comp + x.in_off, x.in_len, out, x.isize, tabs[warp]));
+    }
+    const bool whole = __shfl_sync(0xffffffffu, got, 0) == static_cast<int>(x.isize);
+    __syncwarp();
+    const uint32_t n = whole ? x.isize : 0;
+    const uint32_t slice = (n + 31) / 32;
+    const uint32_t b = min(n, lane * slice), e = min(n, b + slice);
+    uint32_t r = 0;
+    for (uint32_t i = b; i < e; ++i) r = crc_tab[(r ^ out[i]) & 255] ^ (r >> 8);
+    r = InfCrcShift(r, n - e);
+#pragma unroll
+    for (int d = 16; d; d >>= 1) r ^= __shfl_xor_sync(0xffffffffu, r, d);
+    if (lane == 0 && (!whole || ~(r ^ InfCrcShift(0xFFFFFFFFu, n)) != x.crc)) {
+      atomicMin(bad, m);
+    }
+  }
+}
+
 unsigned Grid(uint64_t n, const Ctx& c) {
   return static_cast<unsigned>(std::max<uint64_t>(1, std::min<uint64_t>((n + 255) / 256,
                                                                           c.sms * 16ULL)));
@@ -452,11 +510,90 @@ const char* kFastaInvalid = "[bioparser::FastaParser] error: invalid file format
 const char* kFastqInvalid = "[bioparser::FastqParser] error: invalid file format";
 const char* kNotNucleotide = "[biosoup::NucleicAcid::NucleicAcid] error: not a nucleotide";
 
-// One file's text, read ahead into two pinned slots on a thread of its own. Take(i) waits
-// for slot i (the pieces alternate between the slots), Release(i) hands it back.
+constexpr uint32_t kBgzfMaxMember = 65536;  // BSIZE + 1 of a BGZF member is at most 2^16
+
+// A file read raw, for its BGZF members: a window of preads, and Member() that finds the whole
+// member at an offset from its header alone.
+class BgzfFile {
+ public:
+  explicit BgzfFile(const std::string& path) : fd_(open(path.c_str(), O_RDONLY)) {
+    struct stat st;
+    if (fd_ >= 0 && fstat(fd_, &st) == 0) size_ = static_cast<uint64_t>(st.st_size);
+  }
+  ~BgzfFile() {
+    if (fd_ >= 0) close(fd_);
+  }
+  BgzfFile(const BgzfFile&) = delete;
+  BgzfFile& operator=(const BgzfFile&) = delete;
+  bool ok() const { return fd_ >= 0; }
+  uint64_t size() const { return size_; }
+  // bytes [pos, pos + n) of the file (n <= kBgzfMaxMember), or null when fewer can be read
+  const uint8_t* At(uint64_t pos, uint64_t n) {
+    if (pos >= lo_ && pos + n <= hi_) return win_.data() + (pos - lo_);
+    // the window grows from 64 KiB to 4 MiB, so a first look at a file that is not BGZF
+    // reads little
+    fill_ = std::min<uint64_t>(fill_ * 2, 4ULL << 20);
+    const uint64_t want = pos < size_ ? std::min(std::max(n, fill_), size_ - pos) : 0;
+    if (win_.size() < want) win_.resize(want);
+    uint64_t got = 0;
+    while (got < want) {
+      const ssize_t r = pread(fd_, win_.data() + got, want - got, static_cast<off_t>(pos + got));
+      if (r <= 0) break;
+      got += static_cast<uint64_t>(r);
+    }
+    lo_ = pos;
+    hi_ = pos + got;
+    return got >= n ? win_.data() : nullptr;
+  }
+  // The length of the whole BGZF member at pos (its deflate data relative to pos, ISIZE and
+  // CRC in *m), or 0 when the bytes there are not one: the header 1f 8b 08 with FLG = FEXTRA
+  // alone and a BC subfield of length 2 among well-formed subfields, BSIZE + 1 bytes inside
+  // the file, and an ISIZE of at most 64 KiB.
+  uint32_t Member(uint64_t pos, FxMember* m) {
+    const uint64_t left = pos < size_ ? size_ - pos : 0;
+    const uint64_t span = std::min<uint64_t>(left, kBgzfMaxMember);
+    if (span < 18) return 0;
+    const uint8_t* h = At(pos, span);
+    if (!h || h[0] != 0x1f || h[1] != 0x8b || h[2] != 8 || h[3] != 4) return 0;
+    const uint32_t xend = 12 + (h[10] | h[11] << 8);
+    if (xend + 8 > span) return 0;
+    uint32_t total = 0, q = 12;
+    while (q + 4 <= xend) {
+      const uint32_t slen = h[q + 2] | h[q + 3] << 8;
+      if (q + 4 + slen > xend) return 0;
+      if (h[q] == 'B' && h[q + 1] == 'C' && slen == 2 && total == 0) {
+        total = (h[q + 4] | h[q + 5] << 8) + 1;
+      }
+      q += 4 + slen;
+    }
+    if (q != xend || total < xend + 8 || total > span) return 0;
+    const uint8_t* t = h + total - 8;
+    m->crc = t[0] | t[1] << 8 | t[2] << 16 | static_cast<uint32_t>(t[3]) << 24;
+    m->isize = t[4] | t[5] << 8 | t[6] << 16 | static_cast<uint32_t>(t[7]) << 24;
+    if (m->isize > kInfMaxOutput) return 0;
+    m->in_off = xend;
+    m->in_len = total - xend - 8;
+    m->out_off = 0;
+    m->pad = 0;
+    return total;
+  }
+
+ private:
+  int fd_;
+  uint64_t size_ = 0;
+  std::vector<uint8_t> win_;
+  uint64_t lo_ = 0, hi_ = 0, fill_ = 32 << 10;
+};
+
+// One file, read ahead into two pinned slots on a thread of its own: as text with gzread, or,
+// while bgzf is set, as whole BGZF members (a piece then holds compressed bytes and the
+// member table, and ends once its members' ISIZEs reach the piece size). Take(i) waits for
+// slot i (the pieces alternate between the slots), Release(i) hands it back.
 class FxReader {
  public:
-  FxReader(gzFile f, PinBuf<uint8_t>* slots, uint64_t piece) : f_(f), slots_(slots), piece_(piece) {
+  FxReader(gzFile f, std::unique_ptr<BgzfFile> bgzf, const std::string& path,
+           PinBuf<uint8_t>* slots, uint64_t piece)
+      : f_(f), bgzf_(std::move(bgzf)), path_(path), slots_(slots), piece_(piece) {
     thread_ = std::thread([this] { Run(); });
   }
   ~FxReader() {
@@ -466,10 +603,12 @@ class FxReader {
     }
     cv_.notify_all();
     thread_.join();
-    gzclose(f_);
+    if (f_) gzclose(f_);
   }
   struct Piece {
-    uint64_t len;
+    uint64_t len;      // text bytes (once inflated)
+    uint64_t raw;      // compressed bytes in the slot (0: the slot holds the text)
+    uint32_t members;  // BGZF members in the slot
     bool last;
     bool failed;
   };
@@ -478,6 +617,8 @@ class FxReader {
     cv_.wait(l, [&] { return full_[i]; });
     return piece_of_[i];
   }
+  // the member table of the piece in slot i, until Release(i)
+  const std::vector<FxMember>& Members(int i) const { return members_[i]; }
   void Release(int i) {
     {
       std::lock_guard<std::mutex> l(m_);
@@ -494,21 +635,9 @@ class FxReader {
         cv_.wait(l, [&] { return stop_ || !full_[i]; });
         if (stop_) return;
       }
-      Piece p{0, false, false};
-      uint8_t* dst = slots_[i].get();
-      while (p.len < piece_) {
-        const unsigned want = static_cast<unsigned>(std::min<uint64_t>(piece_ - p.len, 1u << 30));
-        const int got = gzread(f_, dst + p.len, want);
-        if (got < 0) {
-          p.failed = p.last = true;
-          break;
-        }
-        if (got == 0) {
-          p.last = true;
-          break;
-        }
-        p.len += static_cast<uint64_t>(got);
-      }
+      Piece p{0, 0, 0, false, false};
+      if (bgzf_) ReadMembers(i, &p);
+      if (!bgzf_ && !p.last && p.members == 0) ReadText(i, &p);
       {
         std::lock_guard<std::mutex> l(m_);
         piece_of_[i] = p;
@@ -518,9 +647,78 @@ class FxReader {
       if (p.last) return;
     }
   }
+  void ReadText(int i, Piece* p) {
+    uint8_t* dst = slots_[i].get();
+    while (p->len < piece_) {
+      const unsigned want = static_cast<unsigned>(std::min<uint64_t>(piece_ - p->len, 1u << 30));
+      const int got = gzread(f_, dst + p->len, want);
+      if (got < 0) {
+        p->failed = p->last = true;
+        return;
+      }
+      if (got == 0) {
+        p->last = true;
+        return;
+      }
+      p->len += static_cast<uint64_t>(got);
+    }
+  }
+  // whole members at pos_, until the piece's text reaches piece_ or its slot is full
+  void ReadMembers(int i, Piece* p) {
+    std::vector<FxMember>& mem = members_[i];
+    mem.clear();
+    uint8_t* dst = slots_[i].get();
+    while (p->len < piece_) {
+      const uint64_t left = bgzf_->size() - pos_;
+      const uint8_t* h = left ? bgzf_->At(pos_, std::min<uint64_t>(left, 2)) : nullptr;
+      if (left && !h) {
+        p->failed = p->last = true;
+        return;
+      }
+      // the end of the file, or bytes after the last member that zlib ignores
+      if (left < 2 || h[0] != 0x1f || h[1] != 0x8b) {
+        p->last = true;
+        return;
+      }
+      FxMember m;
+      const uint32_t total = bgzf_->Member(pos_, &m);
+      if (total == 0) {
+        HandToZlib(p);
+        return;
+      }
+      if (p->raw + total > slots_[i].cap) return;
+      std::memcpy(dst + p->raw, bgzf_->At(pos_, total), total);
+      m.in_off += p->raw;
+      m.out_off = p->len;
+      mem.push_back(m);
+      p->raw += total;
+      p->len += m.isize;
+      ++p->members;
+      pos_ += total;
+    }
+  }
+  // zlib reads the rest of the file from the gzip member at pos_, with the multi-member
+  // rules the whole-file route has
+  void HandToZlib(Piece* p) {
+    const int fd = open(path_.c_str(), O_RDONLY);
+    if (fd >= 0 && lseek(fd, static_cast<off_t>(pos_), SEEK_SET) == static_cast<off_t>(pos_)) {
+      f_ = gzdopen(fd, "rb");
+    }
+    if (!f_) {
+      if (fd >= 0) close(fd);
+      p->failed = p->last = true;
+      return;
+    }
+    gzbuffer(f_, 1 << 20);
+    bgzf_.reset();
+  }
   gzFile f_;
+  std::unique_ptr<BgzfFile> bgzf_;
+  uint64_t pos_ = 0;
+  std::string path_;
   PinBuf<uint8_t>* slots_;
   uint64_t piece_;
+  std::vector<FxMember> members_[2];
   std::mutex m_;
   std::condition_variable cv_;
   bool full_[2] = {false, false};
@@ -548,6 +746,9 @@ struct FxScratch {
   DevBuf<uint8_t> mark, bq;
   DevBuf<char> names;
   DevBuf<FxRec> rec;
+  DevBuf<uint8_t> comp;
+  DevBuf<FxMember> members;
+  DevBuf<unsigned> bad;
   float read_ms = 0;
 };
 
@@ -730,12 +931,23 @@ uint64_t ParseChunk(Ctx& c, FxScratch& s, const uint8_t* text, uint64_t n, bool 
 // one file's records, chunk by chunk, appended to the set
 void ParseFile(Ctx& c, FxScratch& s, PinBuf<uint8_t>* slots, uint64_t chunk,
                const std::string& path, bool fastq, FxSet& set) {
-  gzFile f = gzopen(path.c_str(), "rb");
-  if (f == nullptr) {
-    throw InvalidArgument("[bioparser::Parser::Create] error: unable to open file " + path);
+  const std::string unreadable =
+      "[bioparser::Parser::Parse] error: unable to read file (" + path + ")";
+  auto raw = std::make_unique<BgzfFile>(path);
+  FxMember first;
+  gzFile f = nullptr;
+  if (raw->ok() && raw->Member(0, &first)) {
+    slots[0].reserve(kBgzfMaxMember);  // a slot holds at least one member
+    slots[1].reserve(kBgzfMaxMember);
+  } else {
+    raw.reset();
+    f = gzopen(path.c_str(), "rb");
+    if (f == nullptr) {
+      throw InvalidArgument("[bioparser::Parser::Create] error: unable to open file " + path);
+    }
+    gzbuffer(f, 1 << 20);
   }
-  gzbuffer(f, 1 << 20);
-  FxReader reader(f, slots, chunk);
+  FxReader reader(f, std::move(raw), path, slots, chunk);
   int cur = 0;
   uint64_t len = 0, fresh = 0, want = chunk;
   for (int slot = 0;; slot ^= 1) {
@@ -743,11 +955,27 @@ void ParseFile(Ctx& c, FxScratch& s, PinBuf<uint8_t>* slots, uint64_t chunk,
     const FxReader::Piece p = reader.Take(slot);
     s.read_ms += std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0)
                      .count();
-    if (p.failed) {
-      throw InvalidArgument("[bioparser::Parser::Parse] error: unable to read file (" + path + ")");
-    }
+    if (p.failed) throw InvalidArgument(unreadable);
     uint8_t* text = s.text[cur].reserve_keep(len + p.len + kFxPad, len, c.stream);
-    if (p.len) {
+    unsigned bad = ~0u;
+    if (p.members) {
+      TimerBegin(c, "fastx_copy");
+      uint8_t* comp = s.comp.reserve(p.raw);
+      FxMember* mem = s.members.reserve(p.members);
+      RVN_CUDA(cudaMemcpyAsync(comp, slots[slot].get(), p.raw, cudaMemcpyHostToDevice, c.stream));
+      RVN_CUDA(cudaMemcpyAsync(mem, reader.Members(slot).data(), p.members * sizeof(FxMember),
+                               cudaMemcpyHostToDevice, c.stream));
+      TimerEnd(c);
+      unsigned* d_bad = s.bad.reserve(1);
+      RVN_CUDA(cudaMemsetAsync(d_bad, 0xFF, sizeof(unsigned), c.stream));
+      TimerBegin(c, "fastx_inflate");
+      FxInflateKernel<<<CeilDiv(p.members, kFxInfWarps), kFxInfWarps * 32, 0, c.stream>>>(
+          comp, mem, p.members, text + len, d_bad);
+      RVN_LAUNCH_CHECK();
+      TimerEnd(c);
+      ++c.launches;
+      RVN_CUDA(cudaMemcpyAsync(&bad, d_bad, sizeof(unsigned), cudaMemcpyDeviceToHost, c.stream));
+    } else if (p.len) {
       TimerBegin(c, "fastx_copy");
       RVN_CUDA(cudaMemcpyAsync(text + len, slots[slot].get(), p.len, cudaMemcpyHostToDevice,
                                c.stream));
@@ -755,6 +983,7 @@ void ParseFile(Ctx& c, FxScratch& s, PinBuf<uint8_t>* slots, uint64_t chunk,
     }
     RVN_CUDA(cudaStreamSynchronize(c.stream));
     reader.Release(slot);
+    if (bad != ~0u) throw InvalidArgument(unreadable);
     len += p.len;
     fresh += p.len;
     if (!p.last && fresh < want) continue;
